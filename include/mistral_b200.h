@@ -258,7 +258,7 @@ int mb200_decode_step(const mb200_layer_desc* layers_dev, const int32_t* windows
  * (torch.zeros) and never writes to it afterwards.
  * Concurrency: a workspace carries state BETWEEN and DURING launches, so all calls that share one workspace must be ordered on
  * one stream (or by events); concurrent streams need one workspace each.  The library keeps no other mutable state that affects
- * results: process-wide state is limited to the debug hooks below, environment switches read once, and the driver entry point
+ * results: process-wide state is limited to the debug hooks below, environment switches, and the driver entry point
  * for tensor-map encoding.  mb200_last_error() is thread-local. */
 #define MB200_WORKSPACE_HEADER_BYTES (64 * 1024)
 
@@ -267,6 +267,11 @@ int mb200_decode_step(const mb200_layer_desc* layers_dev, const int32_t* windows
 int mb200_debug_set_decode_timeline(void* device_buffer);
 /* Debug: [n_sm][n_layers][6][2] uint64 arrive/leave stamps of every CTA at every grid barrier (NULL = off). */
 int mb200_debug_set_barrier_timeline(void* device_buffer);
+/* Debug, per calling thread: the attention and dense GEMM kernels launched since the last call, one line each, named like the
+ * kernel with its template arguments (e.g. "attn_decode_tma_kernel<8>", "gemm_wgmma_kernel<0, 1, 32, 64>").  Copies the log
+ * into `out` (NUL-terminated; NULL discards it), clears it, and switches recording on (enable != 0) or off.  MB200_E_INVALID
+ * when `out` is too small or launches were dropped because the log filled up.  Tests use it to check which kernel a call chose. */
+int mb200_debug_launch_log(int enable, char* out, size_t out_bytes);
 
 /* Test-only: CUDA-core fp32 GEMM c[T, N] = a[T, K] w[N, K]^T used to cross-check the tensor-core kernels. */
 int mb200_test_gemm_naive(const void* a, const void* w, float* c, int64_t T, int64_t N, int64_t K, void* stream);

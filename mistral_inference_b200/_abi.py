@@ -57,6 +57,7 @@ _SIGNATURES = {
                                   c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     "mb200_debug_set_decode_timeline": (c_int, [c_void_p]),
     "mb200_debug_set_barrier_timeline": (c_int, [c_void_p]),
+    "mb200_debug_launch_log": (c_int, [c_int, c_void_p, c_size_t]),
     "mb200_test_gemm_naive": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_void_p]),
 }
 
@@ -318,6 +319,14 @@ def set_decode_timeline(buf: Optional[torch.Tensor]) -> None:
 
 def set_barrier_timeline(buf: Optional[torch.Tensor]) -> None:
     _check(lib().mb200_debug_set_barrier_timeline(_ptr(buf)), "mb200_debug_set_barrier_timeline")
+
+
+def launch_log(enable: bool) -> list:
+    """Names of the attention / dense GEMM kernels launched from this thread since the last call (empty while recording is off);
+    clears the log and switches recording on or off (include/mistral_b200.h)."""
+    buf = ctypes.create_string_buffer(32768)
+    _check(lib().mb200_debug_launch_log(int(enable), ctypes.cast(buf, c_void_p), len(buf)), "mb200_debug_launch_log")
+    return buf.value.decode().splitlines()
 
 
 def test_gemm_naive(a, w) -> torch.Tensor:

@@ -18,6 +18,10 @@
 
 namespace mb200 {
 thread_local char g_err[512] = "";
+thread_local bool g_launch_log_on = false;
+thread_local bool g_launch_log_overflow = false;
+thread_local size_t g_launch_log_len = 0;
+thread_local char g_launch_log[kLaunchLogBytes] = "";
 static unsigned long long* g_mk_prof = nullptr;
 static unsigned long long* g_mk_prof_bar = nullptr;  // debug: decode megakernel phase timeline buffer (device)
 
@@ -206,6 +210,7 @@ int mb200_attn_decode(const void* q, const void* cache_k, const void* cache_v, c
     case 8: attn_decode_kernel<8><<<grid, AD_THREADS, 0, st>>>(p); break;
     default: return fail(MB200_E_INVALID, "attn_decode: H/KV=%d unsupported (1,2,4,6,8)", rep);
   }
+  note_launch("attn_decode_kernel<%d>", rep);
   MB_CHECK_LAUNCH("attn_decode_kernel");
   return MB200_OK;
 }
@@ -240,6 +245,7 @@ int mb200_attn_prefill(const void* q, const void* k_new, const void* v_new, cons
   const dim3 grid((unsigned)ceil_div(span, AP_BQ), (unsigned)n_heads, (unsigned)(causal ? B : 1));
   MB_CHECK_CUDA(cudaFuncSetAttribute(attn_prefill_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, AP_SMEM));
   attn_prefill_kernel<<<grid, AP_THREADS, AP_SMEM, (cudaStream_t)stream>>>(p);
+  note_launch("attn_prefill_kernel");
   MB_CHECK_LAUNCH("attn_prefill_kernel");
   return MB200_OK;
 }
@@ -568,6 +574,21 @@ int mb200_debug_set_decode_timeline(void* device_buffer) {
 }
 int mb200_debug_set_barrier_timeline(void* device_buffer) {
   g_mk_prof_bar = (unsigned long long*)device_buffer;
+  return MB200_OK;
+}
+
+int mb200_debug_launch_log(int enable, char* out, size_t out_bytes) {
+  const bool overflow = g_launch_log_overflow;
+  const size_t len = g_launch_log_len;
+  g_launch_log_on = enable != 0;
+  g_launch_log_overflow = false;
+  g_launch_log_len = 0;
+  if (out != nullptr) {
+    if (out_bytes < len + 1) return fail(MB200_E_INVALID, "launch log: %zu bytes recorded, buffer of %zu", len, out_bytes);
+    memcpy(out, g_launch_log, len);
+    out[len] = '\0';
+  }
+  if (overflow) return fail(MB200_E_INVALID, "launch log: more than %zu bytes of launches since the last read", kLaunchLogBytes);
   return MB200_OK;
 }
 

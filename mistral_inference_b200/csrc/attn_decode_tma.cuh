@@ -280,6 +280,7 @@ int launch_attn_decode_tma(const AttnDecodeParams& p, int64_t max_batch_rows, cu
   MB_CHECK_CUDA(cudaFuncSetAttribute(attn_decode_tma_kernel<REP>, cudaFuncAttributeMaxDynamicSharedMemorySize, ADT_SMEM));
   const dim3 grid((unsigned)p.S, (unsigned)p.KV, (unsigned)p.B);
   MB_CHECK_CUDA(launch_pdl(attn_decode_tma_kernel<REP>, grid, dim3(ADT_THREADS), (size_t)ADT_SMEM, st, map_k, map_v, p));
+  note_launch("attn_decode_tma_kernel<%d>", REP);
   return MB200_OK;
 }
 

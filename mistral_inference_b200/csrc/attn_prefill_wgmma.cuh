@@ -207,12 +207,11 @@ inline int make_tensor_map_rows(CUtensorMap* map, const void* base, int64_t rows
   return MB200_OK;
 }
 
+// MB200_ATTN=mma forces the mma.sync kernel.  Read at every launch, like the GEMM switches, so the tests can run both kernels on
+// the same cases inside one process.
 inline bool wgmma_attn_eligible(int64_t T, int64_t max_seqlen) {
-  static int forced = -1;
-  if (forced < 0) {
-    const char* e = getenv("MB200_ATTN");
-    forced = (e != nullptr && e[0] == 'm') ? 1 : 0;  // MB200_ATTN=mma forces the mma.sync kernel
-  }
+  const char* e = getenv("MB200_ATTN");
+  const bool forced = e != nullptr && e[0] == 'm';
   return !forced && T >= 128 && max_seqlen >= 128;
 }
 
@@ -237,6 +236,7 @@ inline int launch_attn_prefill_wgmma(const void* q, const void* k_new, const voi
   MB_CHECK_CUDA(cudaFuncSetAttribute(attn_prefill_wgmma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, FA_SMEM));
   const dim3 grid((unsigned)H, (unsigned)ceil_div(max_seqlen, FA_BM), (unsigned)B);
   attn_prefill_wgmma_kernel<<<grid, FA_THREADS, FA_SMEM, stream>>>(mq, mk, mv, p);
+  note_launch("attn_prefill_wgmma_kernel");
   MB_CHECK_LAUNCH("attn_prefill_wgmma_kernel");
   return MB200_OK;
 }

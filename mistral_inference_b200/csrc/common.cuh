@@ -36,6 +36,29 @@ inline int fail(int code, const char* fmt, ...) {
     if (e__ != cudaSuccess) return ::mb200::fail(MB200_E_CUDA, "%s: %s", #expr, cudaGetErrorString(e__)); \
   } while (0)
 
+// ---- launch log (mb200_debug_launch_log): which attention / dense GEMM kernel each call chose -----------------
+// Off unless switched on: one thread-local flag test per launch.  One line per launch, named like the kernel with its template
+// arguments ("attn_decode_tma_kernel<8>", "gemm_wgmma_kernel<0, 1, 32, 64>").
+constexpr size_t kLaunchLogBytes = 16384;
+extern thread_local bool g_launch_log_on;
+extern thread_local bool g_launch_log_overflow;
+extern thread_local size_t g_launch_log_len;
+extern thread_local char g_launch_log[kLaunchLogBytes];
+inline void note_launch(const char* fmt, ...) {
+  if (!g_launch_log_on) return;
+  char line[128];
+  va_list ap;
+  va_start(ap, fmt);
+  const int n = vsnprintf(line, sizeof(line), fmt, ap);
+  va_end(ap);
+  if (n < 0 || n >= (int)sizeof(line) || g_launch_log_len + n + 2 > kLaunchLogBytes) {
+    g_launch_log_overflow = true;
+    return;
+  }
+  snprintf(g_launch_log + g_launch_log_len, kLaunchLogBytes - g_launch_log_len, "%s\n", line);
+  g_launch_log_len += n + 1;
+}
+
 typedef __nv_bfloat16 bf16;
 
 constexpr int kHeadDim = 128;

@@ -150,6 +150,7 @@ int launch_gemm_mma(const GemmParams& p, cudaStream_t stream) {
   MB_CHECK_CUDA(cudaFuncSetAttribute(gemm_mma_kernel<MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, GM_SMEM));
   const dim3 grid(ceil_div(p.N, GM_BN), ceil_div(p.T, GM_BM));
   gemm_mma_kernel<MODE><<<grid, GM_THREADS, GM_SMEM, stream>>>(p);
+  note_launch("gemm_mma_kernel<%d>", MODE);
   MB_CHECK_LAUNCH("gemm_mma_kernel");
   return MB200_OK;
 }

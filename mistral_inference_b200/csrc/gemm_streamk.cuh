@@ -269,6 +269,7 @@ int launch_streamk_ta(const GemmParams& g, void* workspace, size_t workspace_byt
   const int grid = (int)(units < sms ? units : sms);
   MB_CHECK_CUDA(cudaFuncSetAttribute(gemm_streamk_kernel<MODE, TA>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmem));
   MB_CHECK_CUDA(launch_pdl(gemm_streamk_kernel<MODE, TA>, dim3((unsigned)grid), dim3(Cfg::kThreads), (size_t)Cfg::kSmem, stream, map_a, map_w, p));
+  note_launch("gemm_streamk_kernel<%d, %d>", MODE, TA);
   return MB200_OK;
 }
 

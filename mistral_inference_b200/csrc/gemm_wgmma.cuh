@@ -368,12 +368,14 @@ int launch_gemm_wgmma_bn(const GemmParams& g, bool pair, int sms, cudaStream_t s
     cfg.attrs = at;
     cfg.numAttrs = 1;
     MB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, gemm_wgmma_kernel<MODE, 2, BN>, map_a, map_w, p));
+    note_launch("gemm_wgmma_kernel<%d, 2, %d, %d>", MODE, BN, TG_BM);
     MB_CHECK_LAUNCH("gemm_wgmma_kernel<cluster 2>");
     return MB200_OK;
   }
   const int tiles = ceil_div(g.T, TG_BM) * (g.N / BN);
   MB_CHECK_CUDA(cudaFuncSetAttribute(gemm_wgmma_kernel<MODE, 1, BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmem));
   gemm_wgmma_kernel<MODE, 1, BN><<<tiles < sms ? tiles : sms, Cfg::kThreads, Cfg::kSmem, stream>>>(map_a, map_w, p);
+  note_launch("gemm_wgmma_kernel<%d, 1, %d, %d>", MODE, BN, TG_BM);
   MB_CHECK_LAUNCH("gemm_wgmma_kernel");
   return MB200_OK;
 }
@@ -417,6 +419,7 @@ int launch_gemm_wgmma_small_bn(const GemmParams& g, int sms, cudaStream_t stream
   const int tiles = g.N / BN;
   MB_CHECK_CUDA(cudaFuncSetAttribute(gemm_wgmma_kernel<MODE, 1, BN, TA>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmem));
   gemm_wgmma_kernel<MODE, 1, BN, TA><<<tiles < sms ? tiles : sms, Cfg::kThreads, Cfg::kSmem, stream>>>(map_a, map_w, p);
+  note_launch("gemm_wgmma_kernel<%d, 1, %d, %d>", MODE, BN, TA);
   MB_CHECK_LAUNCH("gemm_wgmma_kernel<small batch>");
   return MB200_OK;
 }

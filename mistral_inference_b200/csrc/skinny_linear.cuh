@@ -157,6 +157,7 @@ int launch_skinny(const SkinnyParams& p, int T, cudaStream_t stream) {
   auto go = [&](auto kernel) -> int {
     if (smem > 48 * 1024) MB_CHECK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     kernel<<<grid, kSkinnyThreads, smem, stream>>>(p);
+    note_launch("skinny_linear_kernel<%d, %d, %s>", T, MODE, NORM ? "true" : "false");
     MB_CHECK_LAUNCH("skinny_linear_kernel");
     return MB200_OK;
   };

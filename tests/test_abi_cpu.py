@@ -46,6 +46,13 @@ def test_argument_errors_do_not_need_a_gpu(built):
     assert rc == -1 and b"multiple of 8" in _abi.lib().mb200_last_error()
 
 
+def test_launch_log_records_nothing_for_rejected_calls(built):
+    _abi.launch_log(True)
+    assert _abi.lib().mb200_attn_decode(None, None, None, None, None, 1, 1, 4, 2, 128, 1, None, 0, None) == -1
+    assert _abi.launch_log(False) == []
+    assert _abi.launch_log(False) == []  # recording off: still empty
+
+
 def test_no_cpu_fallback():
     p = synth.shape("tiny")
     args = mi.TransformerArgs.from_dict(p)

@@ -19,7 +19,7 @@ from mistral_inference_b200.rope import precompute_freqs_cis
 from oracle import restatement as R
 from oracle.attention_ref import attend_block, local_causal_allowed
 
-from .util import assert_bf16_close
+from .util import assert_bf16_close, assert_launched
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
@@ -326,18 +326,42 @@ def test_kv_ring_write():
                                  (5120, 14336),     # Nemo down projection, K = 14336: 224 k-blocks through the deep ring
                                  (1024, 6144)])     # fewer tiles than half the SMs: narrow tiles
 def test_small_batch_gemm_vs_oracle(T, N, K, ws):
-    """5 <= T < 128 runs gemm_wgmma_kernel with 32/64-row A boxes (the MMA's upper rows read past the box; rows >= T are never
-    stored) and a tile width chosen per N: plain store and residual epilogues against the CPU oracle, and every legal tile width
-    against each other (bit-identical: same k order)."""
+    """5 <= T <= 128 with N a multiple of 128 runs gemm_streamk_kernel (32/64/128-row A boxes by T; the MMA's upper rows read past
+    the box; rows >= T are never stored): plain store and residual epilogues against the CPU oracle."""
     if K == 14336 and T not in (16, 33, 127):
         pytest.skip("long K: representative T only")
+    ta = 32 if T <= 32 else 64 if T <= 64 else 128
+    _small_batch_gemm_vs_oracle(T, N, K, ws, rf"gemm_streamk_kernel<\d+, {ta}>")
+
+
+def _small_batch_gemm_vs_oracle(T, N, K, ws, kernel):
     x, w, res = rnd(T, K, seed=50), rnd(N, K, seed=51, scale=K ** -0.5), rnd(T, N, seed=52)
     out = torch.full((T + 3, N), float("nan"), dtype=torch.bfloat16, device=DEV)  # 3 guard rows: rows >= T must stay untouched
-    _abi.linear_residual(x.to(DEV), w.to(DEV), res.to(DEV), out[:T], ws)
+    out2 = torch.empty(T, N, dtype=torch.bfloat16, device=DEV)
+
+    def launches():
+        _abi.linear_residual(x.to(DEV), w.to(DEV), res.to(DEV), out[:T], ws)
+        _abi.linear_residual(x.to(DEV), w.to(DEV), None, out2, ws)
+
+    assert_launched(launches, kernel, r"gemm_\w+_kernel", 2)
     assert_bf16_close(out[:T], res + F.linear(x, w), atol=2 * 2 ** -8 * res.abs().max().item(), what="small-batch gemm + residual")
     assert torch.isnan(out[T:].float()).all(), "rows past T were written"
-    _abi.linear_residual(x.to(DEV), w.to(DEV), None, out[:T], ws)
-    assert_bf16_close(out[:T], F.linear(x, w), what="small-batch gemm")
+    assert_bf16_close(out2, F.linear(x, w), what="small-batch gemm")
+
+
+@pytest.mark.parametrize("T", [5, 32, 33, 64, 65, 127])
+@pytest.mark.parametrize("N,K,streamk", [(4096, 4096, "0"),   # stream-K switched off: 32-wide tiles
+                                         (1024, 6144, "0"),   # fewer tiles than half the SMs
+                                         (1056, 4096, None)])  # N % 128 != 0: the default routing takes the small-batch kernel
+def test_small_batch_wgmma_gemm_vs_oracle(T, N, K, streamk, ws, monkeypatch):
+    """5 <= T < 128 off the stream-K path runs the small-batch gemm_wgmma_kernel with a 32-, 64- or 128-row A box (TA, the last
+    template argument) chosen by T: plain store and residual epilogues against the CPU oracle."""
+    if streamk is None:
+        monkeypatch.delenv("MB200_STREAMK", raising=False)
+    else:
+        monkeypatch.setenv("MB200_STREAMK", streamk)
+    ta = 32 if T <= 32 else 64 if T <= 64 else 128
+    _small_batch_gemm_vs_oracle(T, N, K, ws, rf"gemm_wgmma_kernel<\d+, 1, \d+, {ta}>")
 
 
 def test_small_batch_gemm_tile_widths_agree(ws, monkeypatch, rope):

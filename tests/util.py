@@ -77,6 +77,32 @@ def assert_bf16_close(got: torch.Tensor, want: torch.Tensor, max_ulp: int = 1, m
     return exact, worst
 
 
+# ----------------------------------------------------------------------------- which kernels a call launched
+def launched_kernels(fn) -> List[str]:
+    """Runs `fn()` and returns the attention and dense GEMM kernels libmb200 launched for it, in order, named like the kernels
+    with their template arguments ("attn_decode_tma_kernel<8>").  The library records each launch next to the launch statement
+    (mb200_debug_launch_log), so the record does not depend on a profiler being able to attach."""
+    from mistral_inference_b200 import _abi
+
+    _abi.launch_log(True)
+    try:
+        fn()
+    finally:
+        names = _abi.launch_log(False)
+    return names
+
+
+def assert_launched(fn, want: str, family: str, count: int) -> None:
+    """Runs `fn()` and asserts that the kernels it launched whose names match the regex `family` are exactly `count` launches of
+    kernels matching the regex `want` (no other kernel of the family ran in their place)."""
+    import re
+
+    mine = [n for n in launched_kernels(fn) if re.search(family, n)]
+    wrong = sorted(set(n for n in mine if not re.search(want, n)))
+    assert not wrong, f"expected only {want!r}, also launched: {wrong}"
+    assert len(mine) == count, f"expected {count} launches of {want!r}, saw {len(mine)}"
+
+
 # ----------------------------------------------------------------------------- tolerances at logit scale
 def bf16_ulp_at(x: float) -> float:
     """Spacing of bf16 numbers at magnitude |x| (8 significand bits)."""
