@@ -17,7 +17,8 @@
  *   - returns 0 on success, a negative MB200_E_* code otherwise; mb200_last_error() gives the
  *     thread-local message.  Nothing throws across the boundary.
  *   - integer metadata (positions, rows, lengths) are int32 device arrays.
- *   - head_dim must be 128 (every config in BASELINE.json); dims must be multiples of 8 (16-byte rows).
+ *   - head_dim must be 128 (every config in BASELINE.json); mb200_attn_qkv and the cache-less mode of mb200_attn_prefill
+ *     also take 64 (the vision encoder).  dims must be multiples of 8 (16-byte rows).
  */
 #ifndef MISTRAL_B200_H_
 #define MISTRAL_B200_H_
@@ -56,7 +57,9 @@ int mb200_rmsnorm(const void* x, const void* w, void* out, int64_t T, int64_t di
  *   x          [T, dim] bf16 (block input, un-normed)
  *   norm_w     [dim] bf16
  *   wqkv       [(H + 2*KV) * hd, dim] bf16: rows = wq ++ wk ++ wv ([out, in] like nn.Linear)
- *   rope       [n_pos, hd/2, 2] fp32 = view_as_real(precompute_freqs_cis(...)) (rope.py:6-10)
+ *   rope       [n_pos, hd/2, 2] fp32 = view_as_real(precompute_freqs_cis(...)) (rope.py:6-10); the vision encoder passes
+ *              the 2-D table [side, side, hd/2] flattened to [side^2, hd/2, 2] (rope.py:26-51) and positions row*side + col
+ *   head_dim   64 or 128
  *   positions  [T] int32 absolute positions (cache.py:228-230)
  *   q_out      [T, H*hd] bf16; k_out, v_out [T, KV*hd] bf16 (rotated k, raw v)
  *   cache_k/v  [n_rows, KV, hd] bf16 flat ring (cache.py:88-89) and cache_rows [T] int32 = slot + b*W
@@ -101,6 +104,7 @@ int mb200_attn_decode(const void* q, const void* cache_k, const void* cache_v, c
  *               comes from the ring, which lets large chunks run on the wgmma / TMA kernel.
  *   causal = 0: the cache-less forward (transformer_layers.py:72-73,88 with mask=None): every query attends
  *               to every new key of the whole flattened batch; ring, q_start, seqpos are ignored.
+ * head_dim 64 (the vision encoder, vision_encoder.py:99): causal = 0 only, on its own wgmma / TMA kernel, scale 64^-0.5.
  */
 int mb200_attn_prefill(const void* q, const void* k_new, const void* v_new, const void* cache_k, const void* cache_v,
                        const int32_t* q_start, const int32_t* seqpos, void* out, int64_t T, int64_t B, int64_t max_seqlen,
@@ -113,6 +117,32 @@ int mb200_attn_prefill(const void* q, const void* k_new, const void* v_new, cons
  */
 int mb200_linear_residual(const void* x, const void* w, const void* residual, void* out, int64_t T, int64_t N, int64_t K,
                           void* workspace, size_t workspace_bytes, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * nn.Linear with an optional bias and an optional exact-erf GELU (the vision-language adapter, vision_encoder.py:105-117).
+ *   out = bf16(x @ W^T + bias)                       gelu = 0   (bias = NULL: bf16(x @ W^T))
+ *   out = bf16(gelu_erf(bf16(x @ W^T + bias)))       gelu != 0
+ *   x [T, K]; w [N, K]; bias [N] or NULL; out [T, N]
+ */
+int mb200_linear_bias(const void* x, const void* w, const void* bias, void* out, int64_t T, int64_t N, int64_t K, int gelu,
+                      void* workspace, size_t workspace_bytes, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * Vision input data movement (vision_encoder.py, transformer.py:122-161).
+ * mb200_vision_patchify: one image [C, H, W] bf16 -> the A operand of the stride-p, bias-free patch Conv2d as a GEMM:
+ *     out [(H/p) * (W/p), k_pad] bf16, row py * (W/p) + px, column c*p*p + ky*p + kx (the conv weight's flatten order),
+ *     columns >= C*p*p zero.  Remainder pixels (H % p, W % p) are dropped, as the convolution floors.
+ * mb200_patch_merge: PatchMerger.permute (vision_encoder.py:180-228) of one image of h x w patch features x [h*w, d] ->
+ *     out [(h/s) * (w/s), d*s*s], row by * (w/s) + bx, column c*s*s + ky*s + kx = x[(by*s + ky) * w + bx*s + kx, c].
+ * mb200_embed_splice: out[t] = feats[number of image tokens before t] where ids[t] == image_token_id, else
+ *     emb[ids[t]] (Transformer.embed_vision_language_features).  ids [T] int64; emb [vocab, dim]; feats [n_feats, dim];
+ *     out [T, dim]; ordinal [T + 1] int32 scratch (device): on return ordinal[T] holds the number of image tokens -- the
+ *     caller compares it with n_feats.  Rows that would read past feats or emb are written as zeros.
+ */
+int mb200_vision_patchify(const void* image, void* out, int64_t C, int64_t H, int64_t W, int64_t patch, int64_t k_pad, void* stream);
+int mb200_patch_merge(const void* x, void* out, int64_t h, int64_t w, int64_t s, int64_t d, void* stream);
+int mb200_embed_splice(const int64_t* ids, const void* emb, const void* feats, void* out, int32_t* ordinal, int64_t T, int64_t dim,
+                       int64_t vocab, int64_t n_feats, int64_t image_token_id, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Fused FFN input: RMSNorm -> packed gate/up projection -> bf16(silu(a)) * b.
@@ -267,7 +297,7 @@ int mb200_decode_step(const mb200_layer_desc* layers_dev, const int32_t* windows
 int mb200_debug_set_decode_timeline(void* device_buffer);
 /* Debug: [n_sm][n_layers][6][2] uint64 arrive/leave stamps of every CTA at every grid barrier (NULL = off). */
 int mb200_debug_set_barrier_timeline(void* device_buffer);
-/* Debug, per calling thread: the attention and dense GEMM kernels launched since the last call, one line each, named like the
+/* Debug, per calling thread: the attention, dense GEMM and vision data-movement kernels launched since the last call, one line each, named like the
  * kernel with its template arguments (e.g. "attn_decode_tma_kernel<8>", "gemm_wgmma_kernel<0, 1, 32, 64>").  Copies the log
  * into `out` (NUL-terminated; NULL discards it), clears it, and switches recording on (enable != 0) or off.  MB200_E_INVALID
  * when `out` is too small or launches were dropped because the log filled up.  Tests use it to check which kernel a call chose. */

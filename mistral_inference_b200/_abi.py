@@ -33,6 +33,10 @@ _SIGNATURES = {
     "mb200_attn_prefill": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64,
                                    c_int64, c_int64, c_int64, c_int64, c_int64, c_int, c_void_p]),
     "mb200_linear_residual": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_void_p, c_size_t, c_void_p]),
+    "mb200_linear_bias": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int, c_void_p, c_size_t, c_void_p]),
+    "mb200_vision_patchify": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int64, c_int64, c_void_p]),
+    "mb200_patch_merge": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int64, c_void_p]),
+    "mb200_embed_splice": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int64, c_int64, c_void_p]),
     "mb200_ffn_gateup": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_float, c_void_p, c_size_t,
                                  c_void_p]),
     "mb200_lm_head": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_float, c_void_p, c_size_t,
@@ -202,6 +206,35 @@ def linear_residual(x, w, residual, out, ws: Workspace) -> None:
     N = w.shape[0]
     _check(lib().mb200_linear_residual(_ptr(x), _ptr(w), _ptr(residual), _ptr(out), T, N, K, ws.ptr, ws.nbytes, _stream()),
            "mb200_linear_residual")
+
+
+def linear_bias(x, w, bias, out, gelu: bool, ws: Workspace) -> None:
+    """out = bf16(x @ w^T + bias), optionally followed by the exact-erf GELU (bias may be None)."""
+    T, K = x.shape
+    _check(lib().mb200_linear_bias(_ptr(x), _ptr(w), _ptr(bias), _ptr(out), T, w.shape[0], K, int(gelu), ws.ptr, ws.nbytes, _stream()),
+           "mb200_linear_bias")
+
+
+def vision_patchify(image: torch.Tensor, out: torch.Tensor, patch: int) -> None:
+    """image [C, H, W] bf16 -> out [(H//p) * (W//p), k_pad] (the patch Conv2d's GEMM operand, zero-padded columns)."""
+    C, H, W = image.shape
+    _check(lib().mb200_vision_patchify(_ptr(image), _ptr(out), C, H, W, patch, out.shape[1], _stream()), "mb200_vision_patchify")
+
+
+def patch_merge(x: torch.Tensor, out: torch.Tensor, h: int, w: int, s: int) -> None:
+    """PatchMerger.permute of one image of h x w patch features x [h*w, d] -> out [(h//s) * (w//s), d*s*s]."""
+    _check(lib().mb200_patch_merge(_ptr(x), _ptr(out), h, w, s, x.shape[1], _stream()), "mb200_patch_merge")
+
+
+def embed_splice(ids: torch.Tensor, emb: torch.Tensor, feats: torch.Tensor, out: torch.Tensor, image_token_id: int) -> int:
+    """Text embedding rows with image feature rows at the image-token positions; returns the number of image tokens in `ids`
+    (one 4-byte device-to-host read)."""
+    T, V, dim = ids.shape[0], emb.shape[0], emb.shape[1]
+    assert ids.dtype == torch.long
+    ordinal = torch.empty(T + 1, dtype=torch.int32, device=ids.device)
+    _check(lib().mb200_embed_splice(_ptr(ids), _ptr(emb), _ptr(feats), _ptr(out), _ptr(ordinal), T, dim, V, feats.shape[0], image_token_id,
+                                    _stream()), "mb200_embed_splice")
+    return int(ordinal[T].item())
 
 
 def ffn_gateup(x, norm_w, w13, g_out, eps, ws: Workspace) -> None:

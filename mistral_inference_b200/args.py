@@ -27,6 +27,31 @@ class LoraArgs:
         return cls(**{f.name: d[f.name] for f in fields(cls) if f.name in d})
 
 
+PATCH_MERGE = "patch_merge"
+
+
+@dataclass
+class VisionEncoderArgs:
+    """args.py:12-26 (Pixtral).  The encoder's head_dim is hidden_size // num_attention_heads."""
+    hidden_size: int
+    num_channels: int
+    image_size: int
+    patch_size: int
+    intermediate_size: int
+    num_hidden_layers: int
+    num_attention_heads: int
+    rope_theta: float = 1e4  # for rope-2D
+    image_token_id: int = 10
+    adapter_bias: bool = True
+    spatial_merge_size: int = 1
+    add_pre_mm_projector_layer_norm: bool = False
+    mm_projector_id: str = ""
+
+    @classmethod
+    def from_dict(cls, d: dict) -> "VisionEncoderArgs":
+        return cls(**{f.name: d[f.name] for f in fields(cls) if f.name in d})
+
+
 @dataclass
 class TransformerArgs:
     dim: int
@@ -49,15 +74,15 @@ class TransformerArgs:
     _sliding_window: Union[None, int, List[Optional[int]]] = None
     model_type: str = "transformer"
 
-    vision_encoder: Optional[dict] = None
+    vision_encoder: Optional[VisionEncoderArgs] = None
 
     def __post_init__(self) -> None:
         assert self.model_type == "transformer", self.model_type
         assert self.sliding_window is None or self._sliding_window is None
         # same aliasing as args.py:58-59
         self.sliding_window = self.sliding_window if self.sliding_window is not None else self._sliding_window
-        if self.vision_encoder is not None:
-            raise NotImplementedError("vision_encoder (Pixtral) is outside the accelerated hot path (SURVEY.md 2, row 10)")
+        if isinstance(self.vision_encoder, dict):
+            self.vision_encoder = VisionEncoderArgs.from_dict(self.vision_encoder)
         if isinstance(self.moe, dict):
             self.moe = MoeArgs.from_dict(self.moe)
         if isinstance(self.lora, dict):

@@ -5,6 +5,7 @@
 
 #include "attn_decode.cuh"
 #include "attn_decode_tma.cuh"
+#include "attn_full_hd64.cuh"
 #include "attn_prefill.cuh"
 #include "attn_prefill_wgmma.cuh"
 #include "decode_megakernel.cuh"
@@ -15,6 +16,7 @@
 #include "moe.cuh"
 #include "sampling.cuh"
 #include "skinny_linear.cuh"
+#include "vision.cuh"
 
 namespace mb200 {
 thread_local char g_err[512] = "";
@@ -113,7 +115,7 @@ int mb200_attn_qkv(const void* x, const void* norm_w, const void* wqkv, const fl
                    void* v_out, void* cache_k, void* cache_v, const int32_t* cache_rows, int64_t T, int64_t dim, int64_t n_heads,
                    int64_t n_kv_heads, int64_t head_dim, float eps, void* workspace, size_t workspace_bytes, void* stream) {
   MB_CHECK_ARG(x && norm_w && wqkv && rope && positions && q_out && k_out && v_out, "attn_qkv: null pointer");
-  MB_CHECK_ARG(head_dim == kHeadDim, "attn_qkv: head_dim=%lld unsupported (128 only)", (long long)head_dim);
+  MB_CHECK_ARG(head_dim == kHeadDim || head_dim == 64, "attn_qkv: head_dim=%lld unsupported (64 or 128)", (long long)head_dim);
   MB_CHECK_ARG(cache_rows == nullptr || (cache_k && cache_v), "attn_qkv: cache_rows without cache pointers");
   EpiParams e;
   e.q_out = q_out;
@@ -126,6 +128,7 @@ int mb200_attn_qkv(const void* x, const void* norm_w, const void* wqkv, const fl
   e.rope = rope;
   e.q_dim = (int)(n_heads * head_dim);
   e.kv_dim = (int)(n_kv_heads * head_dim);
+  e.head_dim = (int)head_dim;
   const int64_t N = (n_heads + 2 * n_kv_heads) * head_dim;
   return run_linear<EPI_QKV_ROPE>(x, norm_w, wqkv, e, T, N, dim, eps, workspace, workspace_bytes, (cudaStream_t)stream);
 }
@@ -220,8 +223,13 @@ int mb200_attn_prefill(const void* q, const void* k_new, const void* v_new, cons
                        int64_t n_kv_heads, int64_t head_dim, int causal, void* stream) {
   MB_CHECK_ARG(q && k_new && v_new && out, "attn_prefill: null pointer");
   MB_CHECK_ARG(!causal || (cache_k && cache_v && q_start && seqpos), "attn_prefill: causal mode needs ring + metadata");
-  MB_CHECK_ARG(head_dim == kHeadDim, "attn_prefill: head_dim=%lld unsupported (128 only)", (long long)head_dim);
+  MB_CHECK_ARG(head_dim == kHeadDim || head_dim == 64, "attn_prefill: head_dim=%lld unsupported (64 or 128)", (long long)head_dim);
   MB_CHECK_ARG(n_heads % n_kv_heads == 0, "attn_prefill: H %% KV != 0");
+  if (head_dim == 64) {  // the vision encoder's attention: cache-less and unmasked only
+    MB_CHECK_ARG(causal == 0, "attn_prefill: head_dim=64 supports the cache-less mode (causal=0) only, got causal=%d", causal);
+    if (T == 0) return MB200_OK;
+    return launch_attn_full_hd64(q, k_new, v_new, out, T, n_heads, n_kv_heads, (cudaStream_t)stream);
+  }
   if (T == 0) return MB200_OK;
   if (causal == 2 && wgmma_attn_eligible(T, max_seqlen))  // first prefill: every key comes from the chunk -> wgmma / TMA kernel
     return launch_attn_prefill_wgmma(q, k_new, v_new, q_start, out, T, B, max_seqlen, W, n_heads, n_kv_heads, (cudaStream_t)stream);
@@ -259,6 +267,59 @@ int mb200_linear_residual(const void* x, const void* w, const void* residual, vo
   e.ld_out = N;
   if (residual) return run_linear<EPI_RESIDUAL>(x, nullptr, w, e, T, N, K, 0.f, workspace, workspace_bytes, (cudaStream_t)stream);
   return run_linear<EPI_STORE>(x, nullptr, w, e, T, N, K, 0.f, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+int mb200_linear_bias(const void* x, const void* w, const void* bias, void* out, int64_t T, int64_t N, int64_t K, int gelu, void* workspace,
+                      size_t workspace_bytes, void* stream) {
+  MB_CHECK_ARG(x && w && out, "linear_bias: null pointer");
+  EpiParams e;
+  e.out = out;
+  e.bias = bias;
+  e.ld_out = N;
+  if (gelu) return run_linear<EPI_BIAS_GELU>(x, nullptr, w, e, T, N, K, 0.f, workspace, workspace_bytes, (cudaStream_t)stream);
+  return run_linear<EPI_BIAS>(x, nullptr, w, e, T, N, K, 0.f, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+int mb200_vision_patchify(const void* image, void* out, int64_t C, int64_t H, int64_t W, int64_t patch, int64_t k_pad, void* stream) {
+  MB_CHECK_ARG(image && out, "vision_patchify: null pointer");
+  MB_CHECK_ARG(C >= 1 && patch >= 1 && H >= patch && W >= patch, "vision_patchify: image [%lld, %lld, %lld] has no whole %lld x %lld patch",
+               (long long)C, (long long)H, (long long)W, (long long)patch, (long long)patch);
+  MB_CHECK_ARG(k_pad >= C * patch * patch && k_pad % 8 == 0, "vision_patchify: k_pad=%lld < C*p*p=%lld or not a multiple of 8", (long long)k_pad,
+               (long long)(C * patch * patch));
+  const int64_t gh = H / patch, gw = W / patch;
+  patchify_kernel<<<(unsigned)(gh * gw), 256, 0, (cudaStream_t)stream>>>((const bf16*)image, (bf16*)out, (int)H, (int)W, (int)patch, (int)gw,
+                                                                       (int)(C * patch * patch), (int)k_pad);
+  note_launch("patchify_kernel");
+  MB_CHECK_LAUNCH("patchify_kernel");
+  return MB200_OK;
+}
+
+int mb200_patch_merge(const void* x, void* out, int64_t h, int64_t w, int64_t s, int64_t d, void* stream) {
+  MB_CHECK_ARG(x && out, "patch_merge: null pointer");
+  MB_CHECK_ARG(s >= 1 && h >= 1 && w >= 1 && d >= 1, "patch_merge: h=%lld w=%lld s=%lld d=%lld", (long long)h, (long long)w, (long long)s,
+               (long long)d);
+  const int64_t rows = (h / s) * (w / s);
+  if (rows == 0) return MB200_OK;
+  patch_merge_kernel<<<(unsigned)rows, 256, 0, (cudaStream_t)stream>>>((const bf16*)x, (bf16*)out, (int)w, (int)s, (int)d);
+  note_launch("patch_merge_kernel");
+  MB_CHECK_LAUNCH("patch_merge_kernel");
+  return MB200_OK;
+}
+
+int mb200_embed_splice(const int64_t* ids, const void* emb, const void* feats, void* out, int32_t* ordinal, int64_t T, int64_t dim, int64_t vocab,
+                       int64_t n_feats, int64_t image_token_id, void* stream) {
+  MB_CHECK_ARG(ids && emb && out && ordinal && (feats || n_feats == 0), "embed_splice: null pointer");
+  MB_CHECK_ARG(dim % 8 == 0 && T >= 0 && n_feats >= 0, "embed_splice: dim=%lld must be a multiple of 8", (long long)dim);
+  cudaStream_t st = (cudaStream_t)stream;
+  splice_scan_kernel<<<1, SPLICE_SCAN_THREADS, 0, st>>>((const long long*)ids, ordinal, (int)T, (long long)image_token_id);
+  note_launch("splice_scan_kernel");
+  MB_CHECK_LAUNCH("splice_scan_kernel");
+  if (T == 0) return MB200_OK;
+  splice_gather_kernel<<<(unsigned)T, 128, 0, st>>>((const long long*)ids, ordinal, (const uint4*)emb, (const uint4*)feats, (uint4*)out,
+                                                   (int)(dim / 8), (long long)vocab, (int)n_feats);
+  note_launch("splice_gather_kernel");
+  MB_CHECK_LAUNCH("splice_gather_kernel");
+  return MB200_OK;
 }
 
 int mb200_ffn_gateup(const void* x, const void* norm_w, const void* w13, void* g_out, int64_t T, int64_t dim, int64_t hidden, float eps,

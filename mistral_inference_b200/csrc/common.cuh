@@ -102,6 +102,8 @@ __device__ __forceinline__ float warp_max(float v) {
 __device__ __forceinline__ float ref_rsqrt(float x) { return __fdiv_rn(1.0f, __fsqrt_rn(x)); }
 // silu in fp32: x / (1 + exp(-x))  (transformer_layers.py:106 via nn.functional.silu on bf16 -> fp32 internally)
 __device__ __forceinline__ float ref_silu(float x) { return __fdiv_rn(x, 1.0f + expf(-x)); }
+// exact-erf GELU in fp32 on a bf16 input, as nn.GELU() computes it: x * 0.5 * (1 + erf(x / sqrt(2)))
+__device__ __forceinline__ float ref_gelu(float x) { return __fmul_rn(__fmul_rn(x, 0.5f), __fadd_rn(1.0f, erff(__fmul_rn(x, 0.70710678118654752f)))); }
 // complex multiply without FMA contraction, as torch's complex kernel computes it (rope.py:21-22)
 __device__ __forceinline__ void ref_cmul(float a, float b, float c, float d, float& re, float& im) {
   re = __fsub_rn(__fmul_rn(a, c), __fmul_rn(b, d));

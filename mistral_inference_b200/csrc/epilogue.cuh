@@ -15,6 +15,8 @@ enum EpiMode : int {
   EPI_SWIGLU = 3,    // g[t, n/2] = bf16( bf16(silu(bf16(acc0))) * bf16(acc1) )   (transformer_layers.py:106)
   EPI_QKV_ROPE = 4,  // split into q/k/v, rotate q,k pairs, optional ring scatter  (transformer_layers.py:66-70, cache.py:91-92)
   EPI_MOE_SCALE = 5, // yw[row, n] = bf16( w[row] * bf16(acc) ), stored on every rank of an expert-parallel group  (moe.py:31)
+  EPI_BIAS = 6,      // out[t, n] = bf16(acc + bias[n]) (bias may be null: bf16(acc))  nn.Linear(bias=True) (vision_encoder.py:108,114)
+  EPI_BIAS_GELU = 7, // out[t, n] = bf16( gelu_erf( bf16(acc + bias[n]) ) )           nn.GELU() after w_in (vision_encoder.py:117)
 };
 
 constexpr int kMaxPeers = 8;
@@ -32,8 +34,11 @@ struct EpiParams {
   void* cache_v = nullptr;
   const int32_t* positions = nullptr;   // [T]
   const int32_t* cache_rows = nullptr;  // [T] or null
-  const float* rope = nullptr;          // [n_pos, 64, 2]
+  const float* rope = nullptr;          // [n_pos, head_dim / 2, 2]
   int q_dim = 0, kv_dim = 0;
+  int head_dim = kHeadDim;              // 64 or 128 (a power of two: the pair index is a mask)
+  // EPI_BIAS / EPI_BIAS_GELU
+  const void* bias = nullptr;  // bf16 [N] or null
   // EPI_MOE_SCALE: routing weight of each (token, expert) row; the weighted expert output goes to `out` and to the same offset
   // of the mapped buffers of the other ranks (NVLink peer stores; n_peers == 0 when unsharded)
   const void* row_w = nullptr;  // bf16 [rows]
@@ -62,11 +67,23 @@ __device__ __forceinline__ void epi_pair(const EpiParams& p, int t, int n, float
     const int64_t off = (int64_t)t * p.ld_out + n;
     *reinterpret_cast<uint32_t*>(reinterpret_cast<uint16_t*>(p.out) + off) = packed;
     for (int r = 0; r < p.n_peers; ++r) *reinterpret_cast<uint32_t*>(reinterpret_cast<uint16_t*>(p.peer_out[r]) + off) = packed;
+  } else if constexpr (MODE == EPI_BIAS || MODE == EPI_BIAS_GELU) {
+    float b0 = y0, b1 = y1;
+    if (p.bias != nullptr) {  // addmm: the bias joins the fp32 accumulator before the single rounding
+      const uint32_t bb = *reinterpret_cast<const uint32_t*>(reinterpret_cast<const uint16_t*>(p.bias) + n);
+      b0 = round_bf16(acc0 + bf16lo(bb));
+      b1 = round_bf16(acc1 + bf16hi(bb));
+    }
+    if constexpr (MODE == EPI_BIAS_GELU) {
+      b0 = ref_gelu(b0);
+      b1 = ref_gelu(b1);
+    }
+    *reinterpret_cast<uint32_t*>(reinterpret_cast<uint16_t*>(p.out) + (int64_t)t * p.ld_out + n) = pack_bf16x2(b0, b1);
   } else if constexpr (MODE == EPI_QKV_ROPE) {
     if (n < p.q_dim + p.kv_dim) {  // q or k: rotate
       const int pos = p.positions[t];
-      const int i = (n & (kHeadDim - 1)) >> 1;
-      const float2 cs = *reinterpret_cast<const float2*>(p.rope + ((int64_t)pos * (kHeadDim / 2) + i) * 2);
+      const int i = (n & (p.head_dim - 1)) >> 1;
+      const float2 cs = *reinterpret_cast<const float2*>(p.rope + ((int64_t)pos * (p.head_dim >> 1) + i) * 2);
       float re, im;
       ref_cmul(y0, y1, cs.x, cs.y, re, im);
       const uint32_t packed = pack_bf16x2(re, im);

@@ -56,7 +56,13 @@ class _PromptPlan:
 def generate(encoded_prompts: List[List[int]], model: Transformer, images: List[List] = [], *, max_tokens: int,  # noqa: B006
              temperature: float, chunk_size: Optional[int] = None, eos_id: Optional[int] = None
              ) -> Tuple[List[List[int]], List[List[float]]]:
-    assert not images, "vision inputs are outside the accelerated hot path"
+    # images[b]: the images of prompt b; the model sees all of them, in prompt order (generate.py:54-60,89)
+    images_torch: List[List[torch.Tensor]] = []
+    if images:
+        assert chunk_size is None
+        images_torch = [[torch.tensor(im, device=model.device, dtype=model.dtype) for im in images_for_sample]
+                        for images_for_sample in images]
+    flattened_images: List[torch.Tensor] = sum(images_torch, [])
     model = model.eval()
     dev = model.device
     plan = _PromptPlan(encoded_prompts, chunk_size)
@@ -74,7 +80,7 @@ def generate(encoded_prompts: List[List[int]], model: Transformer, images: List[
     for flat, seqlens, targets, _ in plan.chunks:
         ids = torch.tensor(flat, dtype=torch.long, device=dev)
         tgt = torch.tensor(targets, dtype=torch.long, device=dev)
-        lp, last_logits = model.forward_logprobs(ids, seqlens, cache, tgt)
+        lp, last_logits = model.forward_logprobs(ids, seqlens, cache, tgt, images=flattened_images)
         prompt_lp.append(lp)
     assert last_logits is not None and last_logits.shape == (B, V)
 

@@ -14,3 +14,15 @@ def precompute_freqs_cis(dim: int, end: int, theta: float) -> torch.Tensor:
     t = torch.arange(end, device=freqs.device)
     freqs = torch.outer(t, freqs).float()
     return torch.polar(torch.ones_like(freqs), freqs)
+
+
+def precompute_freqs_cis_2d(dim: int, height: int, width: int, theta: float) -> torch.Tensor:
+    """complex64 [height, width, dim/2] (rope.py:26-51): the first dim/4 frequencies rotate by the patch row, the last dim/4 by
+    the column.  The vision encoder flattens it to [height * width, dim/2] and indexes it with row * width + col."""
+    freqs = 1.0 / (theta ** (torch.arange(0, dim, 2).float() / dim))
+    h = torch.arange(height, device=freqs.device)
+    w = torch.arange(width, device=freqs.device)
+    freqs_h = torch.outer(h, freqs[::2]).float()
+    freqs_w = torch.outer(w, freqs[1::2]).float()
+    freqs_2d = torch.cat([freqs_h[:, None, :].repeat(1, width, 1), freqs_w[None, :, :].repeat(height, 1, 1)], dim=-1)
+    return torch.polar(torch.ones_like(freqs_2d), freqs_2d)

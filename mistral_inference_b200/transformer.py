@@ -15,12 +15,14 @@ import torch
 from torch import nn
 
 from . import _abi
-from .args import TransformerArgs
+from .args import PATCH_MERGE, TransformerArgs
 from .cache import BufferCache, CacheInputMetadata
 from .rope import precompute_freqs_cis
 from .transformer_layers import RMSNorm, TransformerBlock
+from .vision_encoder import PatchMerger, VisionLanguageAdapter, VisionTransformer
 
 ROPE_TABLE_LEN = 128_000  # transformer.py:116
+_VISION_PREFIXES = ("vision_encoder.", "vision_language_adapter.", "patch_merger.", "pre_mm_projector_norm.")  # transformer.py:279-291
 _NVTX = os.environ.get("MB200_NVTX", "0") == "1"
 
 
@@ -72,9 +74,21 @@ class Transformer(nn.Module):
         self.tok_embeddings: Optional[nn.Embedding] = None
         self.norm: Optional[RMSNorm] = None
         self.output_weight: Optional[nn.Parameter] = None
+        self.vision_encoder: Optional[VisionTransformer] = None
+        self.vision_language_adapter: Optional[VisionLanguageAdapter] = None
+        self.pre_mm_projector_norm: Optional[RMSNorm] = None
+        self.patch_merger: Optional[PatchMerger] = None
         if pipeline_rank == 0:
             self.tok_embeddings = nn.Embedding(args.vocab_size, args.dim)
             self.tok_embeddings.weight.requires_grad_(False)
+            ve = args.vision_encoder
+            if ve is not None:  # transformer.py:59-75
+                self.vision_encoder = VisionTransformer(ve)
+                self.vision_language_adapter = VisionLanguageAdapter(ve.hidden_size, args.dim, ve.adapter_bias)
+                if ve.add_pre_mm_projector_layer_norm:
+                    self.pre_mm_projector_norm = RMSNorm(ve.hidden_size, eps=1e-5)
+                if ve.mm_projector_id == PATCH_MERGE:
+                    self.patch_merger = PatchMerger(vision_encoder_dim=ve.hidden_size, spatial_merge_size=ve.spatial_merge_size)
         if pipeline_rank == num_pipeline_ranks - 1:
             self.norm = RMSNorm(args.dim, eps=args.norm_eps)
             self.output_weight = nn.Parameter(torch.empty(args.vocab_size, args.dim), requires_grad=False)
@@ -144,7 +158,6 @@ class Transformer(nn.Module):
                         images: Optional[List[torch.Tensor]] = None) -> torch.Tensor:
         """Local forward pass (transformer.py:163-219): hidden states of this stage; the last stage returns
         the normalised final embeddings."""
-        assert not images, "vision inputs are outside the accelerated hot path"
         self._check_runnable()
         assert len(seqlens) <= self.args.max_batch_size, f"Max batch size is {self.args.max_batch_size}, got batch size of {len(seqlens)}"
         (num_toks,) = input_ids.shape
@@ -161,7 +174,7 @@ class Transformer(nn.Module):
 
         if self.pipeline_rank == 0:
             assert self.tok_embeddings is not None
-            h = self.tok_embeddings(input_ids)
+            h = self._embed(input_ids, images)
         else:
             h = torch.empty(num_toks, self.args.dim, device=self.device, dtype=self.dtype)
             torch.distributed.recv(h, src=self.pipeline_rank - 1)
@@ -183,22 +196,21 @@ class Transformer(nn.Module):
     def forward(self, input_ids: torch.Tensor, seqlens: List[int], cache: Optional[BufferCache] = None,
                 images: Optional[List[torch.Tensor]] = None) -> torch.Tensor:
         """transformer.py:221-242.  [T, vocab] logits, fp32 when softmax_fp32."""
-        assert not images, "vision inputs are outside the accelerated hot path"
         self._check_runnable()
         last = self.pipeline_rank == self.num_pipeline_ranks - 1
         if last and self.num_pipeline_ranks == 1:
-            if self._graph_decode_ok(seqlens, cache):
+            if not self._uses_images(images) and self._graph_decode_ok(seqlens, cache):
                 outs32 = self.decode_static(input_ids, cache).clone()
                 return outs32 if self.softmax_fp32 else outs32.to(self.dtype)
             # single stage: final norm + lm head + .float() are one fused call (no [T, dim] normed round trip)
-            h = self._hidden_no_norm(input_ids, seqlens, cache)
+            h = self._hidden_no_norm(input_ids, seqlens, cache, images=images)
             if cache is not None:
                 cache.update_seqlens(seqlens)
             outs32 = torch.empty(h.shape[0], self.vocab_size, device=h.device, dtype=torch.float32)
             assert self.norm is not None and self.output_weight is not None
             _abi.lm_head(h, self.norm.weight, self.output_weight, outs32, self.args.norm_eps, self.workspace(h.shape[0]))
             return outs32 if self.softmax_fp32 else outs32.to(self.dtype)
-        h = self.forward_partial(input_ids, seqlens, cache=cache)
+        h = self.forward_partial(input_ids, seqlens, cache=cache, images=images)
         if not last:
             outs = torch.empty(h.shape[0], self.vocab_size, device=h.device, dtype=h.dtype)
         else:
@@ -210,7 +222,8 @@ class Transformer(nn.Module):
         return outs.float() if self.softmax_fp32 else outs
 
     def _hidden_no_norm(self, input_ids: torch.Tensor, seqlens: List[int], cache: Optional[BufferCache],
-                        input_metadata: Optional[List[CacheInputMetadata]] = None) -> torch.Tensor:
+                        input_metadata: Optional[List[CacheInputMetadata]] = None,
+                        images: Optional[List[torch.Tensor]] = None) -> torch.Tensor:
         assert len(seqlens) <= self.args.max_batch_size, f"Max batch size is {self.args.max_batch_size}, got batch size of {len(seqlens)}"
         (num_toks,) = input_ids.shape
         assert sum(seqlens) == num_toks, (sum(seqlens), num_toks)
@@ -223,13 +236,46 @@ class Transformer(nn.Module):
         else:
             positions = torch.cat([torch.arange(0, s, dtype=torch.int32) for s in seqlens]).to(self.device)
         assert self.tok_embeddings is not None
-        h = self.tok_embeddings(input_ids)
+        h = self._embed(input_ids, images)
         rope = self.rope_table
         with _nvtx(f"mb200.layers[T={num_toks}]"):
             for local_layer_id, layer in enumerate(self.layers.values()):
                 view = cache.get_view(local_layer_id, input_metadata[local_layer_id]) if cache is not None else None
                 h = layer(h, rope, positions, view, ws)
         return h
+
+    # ------------------------------------------------------------------ images (transformer.py:122-161,188-193)
+    def _uses_images(self, images: Optional[List[torch.Tensor]]) -> bool:
+        """A model without a vision encoder ignores `images`; an empty list takes the text path."""
+        return self.vision_encoder is not None and bool(images)
+
+    def _embed(self, input_ids: torch.Tensor, images: Optional[List[torch.Tensor]]) -> torch.Tensor:
+        assert self.tok_embeddings is not None
+        if self._uses_images(images):
+            return self.embed_vision_language_features(input_ids, images)
+        return self.tok_embeddings(input_ids)
+
+    def embed_vision_language_features(self, input_ids: torch.Tensor, images: List[torch.Tensor]) -> torch.Tensor:
+        """Encoder -> [pre_mm_projector_norm] -> [patch merger] -> adapter, then one kernel places the image features at the
+        image-token positions (in order) and the text embeddings everywhere else."""
+        ve = self.args.vision_encoder
+        assert self.tok_embeddings is not None and self.vision_encoder is not None and self.vision_language_adapter is not None
+        assert ve is not None
+        with _nvtx(f"mb200.vision[{len(images)} images]"):
+            feats = self.vision_encoder(images)
+            ws = self.vision_encoder.workspace(feats.shape[0])
+            if self.pre_mm_projector_norm is not None:
+                feats = self.pre_mm_projector_norm(feats)
+            if self.patch_merger is not None:
+                p = ve.patch_size
+                feats = self.patch_merger(feats, [(img.shape[1] // p, img.shape[2] // p) for img in images], ws)
+            feats = self.vision_language_adapter(feats, ws)
+        seq_len = input_ids.shape[0]
+        out = torch.empty(seq_len, self.args.dim, dtype=self.tok_embeddings.weight.dtype, device=input_ids.device)
+        n_img_tokens = _abi.embed_splice(input_ids, self.tok_embeddings.weight, feats, out, ve.image_token_id)
+        assert n_img_tokens == feats.shape[0], (
+            f"seq_len {seq_len} should be equal to N_txt + N_img {(seq_len - n_img_tokens, feats.shape[0], n_img_tokens)}")
+        return out
 
     def _check_positions(self, cache: BufferCache, seqlens: List[int]) -> None:
         """The reference indexes freqs_cis[positions] and raises past the table (transformer.py:199); the kernels would read out of bounds."""
@@ -393,7 +439,7 @@ class Transformer(nn.Module):
 
     @torch.inference_mode()
     def forward_logprobs(self, input_ids: torch.Tensor, seqlens: List[int], cache: Optional[BufferCache],
-                         targets: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
+                         targets: torch.Tensor, images: Optional[List[torch.Tensor]] = None) -> Tuple[torch.Tensor, torch.Tensor]:
         """One prompt chunk for generate(): returns (lp [T] fp32 with lp[t] = log_softmax(logits[t])[targets[t]] where
         targets[t] >= 0, logits [B, V] fp32 of each sequence's last token).  Replaces forward + log_softmax over [T, V] +
         per-token gathers (generate.py:97-118): the lm head runs over blocks of rows, each followed by the fused
@@ -403,11 +449,11 @@ class Transformer(nn.Module):
         last_idx = torch.tensor(seqlens, device=input_ids.device).cumsum(0) - 1
         lp = torch.zeros(T, dtype=torch.float32, device=input_ids.device)
         if self.num_pipeline_ranks > 1:  # reference-compatible pipeline mode: logits arrive by broadcast (transformer.py:236-237)
-            logits = self.forward(input_ids, seqlens, cache).float().contiguous()
+            logits = self.forward(input_ids, seqlens, cache, images=images).float().contiguous()
             _abi.logprob_gather(logits, targets, out=lp)
             return lp, logits.index_select(0, last_idx)
         self._check_runnable()
-        h = self._hidden_no_norm(input_ids, seqlens, cache)
+        h = self._hidden_no_norm(input_ids, seqlens, cache, images=images)
         if cache is not None:
             cache.update_seqlens(seqlens)
         assert self.norm is not None and self.output_weight is not None
@@ -442,45 +488,82 @@ class Transformer(nn.Module):
             if self.output_weight is None:
                 return False
             put(self.output_weight)
+        elif k.startswith(_VISION_PREFIXES):
+            if self.pipeline_rank != 0:
+                return False
+            return self._assign_vision(k, v, put)
         elif k.startswith("layers."):
             _, lid, rest = k.split(".", 2)
             if lid not in self.layers:
                 return False
-            blk: TransformerBlock = self.layers[lid]  # type: ignore[assignment]
-            att = blk.attention
-            if rest == "attention.wq.weight":
-                put(att.wqkv[: att.q_dim])
-            elif rest == "attention.wk.weight":
-                put(att.wqkv[att.q_dim: att.q_dim + att.kv_dim])
-            elif rest == "attention.wv.weight":
-                put(att.wqkv[att.q_dim + att.kv_dim:])
-            elif rest == "attention.wo.weight":
-                put(att.wo_weight)
-            elif rest == "attention_norm.weight":
-                put(blk.attention_norm.weight)
-            elif rest == "ffn_norm.weight":
-                put(blk.ffn_norm.weight)
-            elif rest == "feed_forward.gate.weight":
-                put(blk.feed_forward.gate_weight)
+            return self._assign_block(self.layers[lid], k, rest, put)
+        else:
+            raise ValueError(f"Unexpected key {k}")
+        return True
+
+    @staticmethod
+    def _assign_block(blk: TransformerBlock, k: str, rest: str, put) -> bool:
+        """`rest` = the key below `layers.{i}.` of one TransformerBlock (text or vision)."""
+        att = blk.attention
+        if rest == "attention.wq.weight":
+            put(att.wqkv[: att.q_dim])
+        elif rest == "attention.wk.weight":
+            put(att.wqkv[att.q_dim: att.q_dim + att.kv_dim])
+        elif rest == "attention.wv.weight":
+            put(att.wqkv[att.q_dim + att.kv_dim:])
+        elif rest == "attention.wo.weight":
+            put(att.wo_weight)
+        elif rest == "attention_norm.weight":
+            put(blk.attention_norm.weight)
+        elif rest == "ffn_norm.weight":
+            put(blk.ffn_norm.weight)
+        elif rest == "feed_forward.gate.weight":
+            put(blk.feed_forward.gate_weight)
+        else:
+            parts = rest.split(".")
+            if parts[0] != "feed_forward":
+                raise ValueError(f"Unexpected key {k}")
+            ff = blk.feed_forward
+            if parts[1] == "experts":
+                if parts[2] not in ff.experts:
+                    return False  # an expert owned by another expert-parallel rank
+                ff = ff.experts[parts[2]]
+                parts = parts[2:]
+            name = parts[1]
+            if name == "w1":
+                put(ff.w13.view(ff.hidden_dim, 2, ff.dim)[:, 0])
+            elif name == "w3":
+                put(ff.w13.view(ff.hidden_dim, 2, ff.dim)[:, 1])
+            elif name == "w2":
+                put(ff.w2_weight)
             else:
-                parts = rest.split(".")
-                if parts[0] != "feed_forward":
-                    raise ValueError(f"Unexpected key {k}")
-                ff = blk.feed_forward
-                if parts[1] == "experts":
-                    if parts[2] not in ff.experts:
-                        return False  # an expert owned by another expert-parallel rank
-                    ff = ff.experts[parts[2]]
-                    parts = parts[2:]
-                name = parts[1]
-                if name == "w1":
-                    put(ff.w13.view(ff.hidden_dim, 2, ff.dim)[:, 0])
-                elif name == "w3":
-                    put(ff.w13.view(ff.hidden_dim, 2, ff.dim)[:, 1])
-                elif name == "w2":
-                    put(ff.w2_weight)
-                else:
-                    raise ValueError(f"Unexpected key {k}")
+                raise ValueError(f"Unexpected key {k}")
+        return True
+
+    def _assign_vision(self, k: str, v: torch.Tensor, put) -> bool:
+        ve, adapter = self.vision_encoder, self.vision_language_adapter
+        if ve is None or adapter is None:
+            raise ValueError(f"Unexpected key {k}")
+        if k == "vision_encoder.patch_conv.weight":
+            ve.patch_conv_weight[:, ve.k_conv:].zero_()  # the GEMM reads the padding columns
+            put(ve.patch_conv.weight)
+        elif k == "vision_encoder.ln_pre.weight":
+            put(ve.ln_pre.weight)
+        elif k.startswith("vision_encoder.transformer.layers."):
+            _, _, _, lid, rest = k.split(".", 4)
+            if not lid.isdigit() or int(lid) >= len(ve.transformer.layers):
+                raise ValueError(f"Unexpected key {k}")
+            return self._assign_block(ve.transformer.layers[int(lid)], k, rest, put)
+        elif k in ("vision_language_adapter.w_in.weight", "vision_language_adapter.w_out.weight",
+                   "vision_language_adapter.w_in.bias", "vision_language_adapter.w_out.bias"):
+            dst = getattr(adapter, k.split(".", 1)[1].replace(".", "_"))
+            if dst is None:
+                raise ValueError(f"Unexpected key {k}")
+            put(dst)
+        elif k == "pre_mm_projector_norm.weight" and self.pre_mm_projector_norm is not None:
+            put(self.pre_mm_projector_norm.weight)
+        elif k == "patch_merger.merging_layer.weight" and self.patch_merger is not None:
+            put(self.patch_merger.merging_layer_weight)
         else:
             raise ValueError(f"Unexpected key {k}")
         return True
@@ -488,6 +571,8 @@ class Transformer(nn.Module):
     def _owns_key(self, k: str) -> bool:
         """False for checkpoint tensors that belong to another pipeline / expert-parallel rank (decided from the key alone, so a
         loader can skip reading them)."""
+        if k.startswith(_VISION_PREFIXES):
+            return self.pipeline_rank == 0
         if not k.startswith("layers."):
             return True
         _, lid, rest = k.split(".", 2)
@@ -520,28 +605,46 @@ class Transformer(nn.Module):
         out: Dict[str, torch.Tensor] = {}
         if self.tok_embeddings is not None:
             out["tok_embeddings.weight"] = self.tok_embeddings.weight
+        if self.vision_encoder is not None and self.vision_language_adapter is not None:
+            ve = self.vision_encoder
+            out["vision_encoder.patch_conv.weight"] = ve.patch_conv.weight
+            out["vision_encoder.ln_pre.weight"] = ve.ln_pre.weight
+            for i, blk in enumerate(ve.transformer.layers):
+                self._block_state(out, f"vision_encoder.transformer.layers.{i}.", blk)
+            for n in ("w_in", "w_out"):
+                lin = getattr(self.vision_language_adapter, n)
+                out[f"vision_language_adapter.{n}.weight"] = lin.weight
+                if lin.bias is not None:
+                    out[f"vision_language_adapter.{n}.bias"] = lin.bias
+            if self.pre_mm_projector_norm is not None:
+                out["pre_mm_projector_norm.weight"] = self.pre_mm_projector_norm.weight
+            if self.patch_merger is not None:
+                out["patch_merger.merging_layer.weight"] = self.patch_merger.merging_layer_weight
         for lid, blk in self.layers.items():
-            p = f"layers.{lid}."
-            att = blk.attention
-            out[p + "attention.wq.weight"] = att.wq.weight
-            out[p + "attention.wk.weight"] = att.wk.weight
-            out[p + "attention.wv.weight"] = att.wv.weight
-            out[p + "attention.wo.weight"] = att.wo_weight
-            out[p + "attention_norm.weight"] = blk.attention_norm.weight
-            out[p + "ffn_norm.weight"] = blk.ffn_norm.weight
-            ff = blk.feed_forward
-            if hasattr(ff, "experts"):
-                out[p + "feed_forward.gate.weight"] = ff.gate_weight
-                for e, ex in ff.experts.items():  # keyed by the global expert id; the local ones only when sharded
-                    for n in ("w1", "w2", "w3"):
-                        out[p + f"feed_forward.experts.{e}.{n}.weight"] = getattr(ex, n).weight
-            else:
-                for n in ("w1", "w2", "w3"):
-                    out[p + f"feed_forward.{n}.weight"] = getattr(ff, n).weight
+            self._block_state(out, f"layers.{lid}.", blk)
         if self.norm is not None:
             out["norm.weight"] = self.norm.weight
             out["output.weight"] = self.output_weight
         return out
+
+    @staticmethod
+    def _block_state(out: Dict[str, torch.Tensor], p: str, blk: TransformerBlock) -> None:
+        att = blk.attention
+        out[p + "attention.wq.weight"] = att.wq.weight
+        out[p + "attention.wk.weight"] = att.wk.weight
+        out[p + "attention.wv.weight"] = att.wv.weight
+        out[p + "attention.wo.weight"] = att.wo_weight
+        out[p + "attention_norm.weight"] = blk.attention_norm.weight
+        out[p + "ffn_norm.weight"] = blk.ffn_norm.weight
+        ff = blk.feed_forward
+        if hasattr(ff, "experts"):
+            out[p + "feed_forward.gate.weight"] = ff.gate_weight
+            for e, ex in ff.experts.items():  # keyed by the global expert id; the local ones only when sharded
+                for n in ("w1", "w2", "w3"):
+                    out[p + f"feed_forward.experts.{e}.{n}.weight"] = getattr(ex, n).weight
+        else:
+            for n in ("w1", "w2", "w3"):
+                out[p + f"feed_forward.{n}.weight"] = getattr(ff, n).weight
 
     # ------------------------------------------------------------------ LoRA, merged path (lora.py:92-155 with args.lora is None)
     def load_lora(self, lora_path: Union[Path, str], scaling: float = 2.0) -> None:

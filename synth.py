@@ -75,11 +75,14 @@ def synth_tensor(key: str, shape: Tuple[int, ...], seed: int, dtype: torch.dtype
 
 
 def state_dict_shapes(p: dict) -> Iterator[Tuple[str, Tuple[int, ...]]]:
-    """(key, shape) for every tensor of a params.json dict `p` (single pipeline rank, no LoRA/vision)."""
+    """(key, shape) for every tensor of a params.json dict `p` (single pipeline rank, no LoRA).  The vision keys only when `p` has
+    a `vision_encoder` block."""
     dim, hd, hid = p["dim"], p["head_dim"], p["hidden_dim"]
     H, KV, V = p["n_heads"], p["n_kv_heads"], p["vocab_size"]
     moe = p.get("moe")
     yield "tok_embeddings.weight", (V, dim)
+    if p.get("vision_encoder"):
+        yield from vision_state_dict_shapes(p)
     for i in range(p["n_layers"]):
         pre = f"layers.{i}."
         yield pre + "attention.wq.weight", (H * hd, dim)
@@ -100,6 +103,38 @@ def state_dict_shapes(p: dict) -> Iterator[Tuple[str, Tuple[int, ...]]]:
             yield pre + "feed_forward.w3.weight", (hid, dim)
     yield "norm.weight", (dim,)
     yield "output.weight", (V, dim)
+
+
+def vision_state_dict_shapes(p: dict) -> Iterator[Tuple[str, Tuple[int, ...]]]:
+    """The Pixtral keys (transformer.py:59-75, vision_encoder.py) with the reference's defaults for absent fields."""
+    ve = p["vision_encoder"]
+    d, C, ps, inter = ve["hidden_size"], ve["num_channels"], ve["patch_size"], ve["intermediate_size"]
+    s = ve.get("spatial_merge_size", 1)
+    yield "vision_encoder.patch_conv.weight", (d, C, ps, ps)
+    yield "vision_encoder.ln_pre.weight", (d,)
+    for i in range(ve["num_hidden_layers"]):
+        pre = f"vision_encoder.transformer.layers.{i}."
+        for n in ("wq", "wk", "wv", "wo"):
+            yield pre + f"attention.{n}.weight", (d, d)
+        yield pre + "attention_norm.weight", (d,)
+        yield pre + "ffn_norm.weight", (d,)
+        yield pre + "feed_forward.w1.weight", (inter, d)
+        yield pre + "feed_forward.w2.weight", (d, inter)
+        yield pre + "feed_forward.w3.weight", (inter, d)
+    yield "vision_language_adapter.w_in.weight", (p["dim"], d)
+    yield "vision_language_adapter.w_out.weight", (p["dim"], p["dim"])
+    if ve.get("adapter_bias", True):
+        yield "vision_language_adapter.w_in.bias", (p["dim"],)
+        yield "vision_language_adapter.w_out.bias", (p["dim"],)
+    if ve.get("add_pre_mm_projector_layer_norm", False):
+        yield "pre_mm_projector_norm.weight", (d,)
+    if ve.get("mm_projector_id", "") == "patch_merge":
+        yield "patch_merger.merging_layer.weight", (d, d * s * s)
+
+
+def synth_image(channels: int, height: int, width: int, seed: int, dtype: torch.dtype = torch.bfloat16) -> torch.Tensor:
+    """A deterministic image [C, H, W] with values in [-1, 1) (normalised pixels)."""
+    return hash_uniform(channels * height * width, (seed * 6151 + 13) & 0xFFFFFF).to(dtype).view(channels, height, width)
 
 
 def synth_state_dict(p: dict, seed: int = 0, dtype: torch.dtype = torch.bfloat16,
@@ -143,6 +178,25 @@ SHAPES: Dict[str, dict] = {
     # the shape the reference's own tests use (tests/test_generate.py:40-50)
     "ref-test": dict(dim=512, n_layers=1, head_dim=128, hidden_dim=2048, n_heads=4, n_kv_heads=2,
                      norm_eps=1e-5, vocab_size=32000),
+    # Pixtral-12B: the Nemo-12B text model plus a 24-layer, head_dim-64 vision encoder (public params.json)
+    "pixtral-12b": dict(dim=5120, n_layers=40, head_dim=128, hidden_dim=14336, n_heads=32, n_kv_heads=8, norm_eps=1e-5,
+                        vocab_size=131072, rope_theta=1000000000.0,
+                        vision_encoder=dict(hidden_size=1024, num_channels=3, image_size=1024, patch_size=16, intermediate_size=4096,
+                                            num_hidden_layers=24, num_attention_heads=16, rope_theta=10000.0, image_token_id=10)),
+    # the reference's two Pixtral test configurations (tests/test_generate.py:78-99,127-152); image_token_id 2
+    "pixtral-ref-test": dict(dim=512, n_layers=1, head_dim=128, hidden_dim=2048, n_heads=4, n_kv_heads=2, norm_eps=1e-5, vocab_size=32000,
+                             vision_encoder=dict(hidden_size=128, num_channels=3, image_size=4, patch_size=2, intermediate_size=256,
+                                                 num_hidden_layers=1, num_attention_heads=2, rope_theta=10000, image_token_id=2)),
+    "pixtral-ref-test-merge": dict(dim=512, n_layers=1, head_dim=128, hidden_dim=2048, n_heads=4, n_kv_heads=2, norm_eps=1e-5,
+                                   vocab_size=32000,
+                                   vision_encoder=dict(hidden_size=128, num_channels=3, image_size=8, patch_size=2, intermediate_size=256,
+                                                       num_hidden_layers=1, num_attention_heads=2, rope_theta=10000, image_token_id=2,
+                                                       adapter_bias=False, spatial_merge_size=2, add_pre_mm_projector_layer_norm=True,
+                                                       mm_projector_id="patch_merge")),
+    # tiny text model + a vision encoder at the real layer shape (hidden 1024, 16 heads of 64), small enough for the CPU oracle
+    "tiny-pixtral": dict(dim=256, n_layers=2, head_dim=128, hidden_dim=512, n_heads=4, n_kv_heads=2, norm_eps=1e-5, vocab_size=512,
+                         vision_encoder=dict(hidden_size=1024, num_channels=3, image_size=256, patch_size=16, intermediate_size=4096,
+                                             num_hidden_layers=2, num_attention_heads=16, rope_theta=10000.0, image_token_id=10)),
 }
 
 
