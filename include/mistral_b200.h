@@ -154,6 +154,44 @@ int mb200_ffn_gateup(const void* x, const void* norm_w, const void* w13, void* g
                      int64_t hidden, float eps, void* workspace, size_t workspace_bytes, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * Un-merged LoRA adapters (params.json `lora` block: every wq/wk/wv/wo/w1/w2/w3 of the text layers is a LoRALinear,
+ * lora.py:22-89).  Each *_lora entry point below takes the arguments of its counterpart plus one adapter and computes, for every
+ * output column n of the packed weight, following LoRALinear.forward (lora.py:71-74) with xn = the (normed) input:
+ *   a   = bf16(xn @ a_w^T)            [T, rank_cols]  lora_A of every segment, fp32 accumulation       -> a_buf
+ *   l   = bf16(a  @ b_w^T)            [T, N]          lora_B                                             -> l_buf
+ *   y   = bf16(xn @ W^T)                              the base Linear, as in the counterpart
+ *   out = bf16(y + bf16(l * scaling))                 `linear(x) + lora * scaling`
+ * and then the counterpart's epilogue on `out` unchanged (RoPE + ring scatter / SiLU*mul / residual add).  RMSNorm runs once per
+ * call: the down projection and the base GEMM read the same normed rows.  Adapters that are exactly zero give the counterpart's
+ * result bit for bit.
+ * Packing (done once at load time by the caller), with S segments of rank r (q,k,v: S = 3; w1,w3: S = 2; wo, w2: S = 1):
+ *   a_w  [rank_cols, K]: rows s*r .. s*r + r - 1 = lora_A of segment s; rank_cols = S*r rounded up to a multiple of 64, the
+ *        padding rows zero.
+ *   b_w  [N, rank_cols]: row n = lora_B of n's segment (row n - first row of the segment) in columns s*r .. s*r + r - 1, zeros
+ *        elsewhere.  For w13 the rows interleave like w13: row 2i = [B1[i] | 0], row 2i+1 = [0 | B3[i]].
+ *   a_buf [T, rank_cols], l_buf [T, N] bf16 device scratch owned by the caller, 16-byte aligned (the workspace contract is
+ *        unchanged; MB200_E_INVALID otherwise); the down
+ *        projection splits K across CTAs and keeps its fp32 partials in l_buf before the up projection overwrites it.  The split
+ *        bounds and the summation order depend on the shape and the device's SM count only, so results are deterministic.
+ */
+typedef struct mb200_lora {
+  const void* a_w;   /* [rank_cols, K] bf16 */
+  const void* b_w;   /* [N, rank_cols] bf16 */
+  int64_t rank_cols; /* multiple of 64 */
+  float scaling;     /* args.lora.scaling */
+  void* a_buf;       /* [T, rank_cols] bf16 scratch */
+  void* l_buf;       /* [T, N] bf16 scratch */
+} mb200_lora;
+int mb200_attn_qkv_lora(const void* x, const void* norm_w, const void* wqkv, const float* rope, const int32_t* positions,
+                        void* q_out, void* k_out, void* v_out, void* cache_k, void* cache_v, const int32_t* cache_rows,
+                        int64_t T, int64_t dim, int64_t n_heads, int64_t n_kv_heads, int64_t head_dim, float eps,
+                        void* workspace, size_t workspace_bytes, void* stream, const mb200_lora* lora);
+int mb200_ffn_gateup_lora(const void* x, const void* norm_w, const void* w13, void* g_out, int64_t T, int64_t dim,
+                          int64_t hidden, float eps, void* workspace, size_t workspace_bytes, void* stream, const mb200_lora* lora);
+int mb200_linear_residual_lora(const void* x, const void* w, const void* residual, void* out, int64_t T, int64_t N, int64_t K,
+                               void* workspace, size_t workspace_bytes, void* stream, const mb200_lora* lora);
+
+/* ---------------------------------------------------------------------------------------------
  * Final RMSNorm + lm head, fp32 logits.  Replaces norm + output + .float() (transformer.py:219,235,240).
  *   x [T, dim]; norm_w [dim]; w_out [V, dim]; logits [T, V] fp32 (each value is a bf16-rounded number).
  */

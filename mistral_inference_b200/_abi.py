@@ -39,6 +39,12 @@ _SIGNATURES = {
     "mb200_embed_splice": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int64, c_int64, c_void_p]),
     "mb200_ffn_gateup": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_float, c_void_p, c_size_t,
                                  c_void_p]),
+    "mb200_attn_qkv_lora": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                    c_void_p, c_int64, c_int64, c_int64, c_int64, c_int64, c_float, c_void_p, c_size_t, c_void_p, c_void_p]),
+    "mb200_ffn_gateup_lora": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_float, c_void_p, c_size_t,
+                                      c_void_p, c_void_p]),
+    "mb200_linear_residual_lora": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_void_p, c_size_t, c_void_p,
+                                           c_void_p]),
     "mb200_lm_head": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_float, c_void_p, c_size_t,
                               c_void_p]),
     "mb200_decode_meta": (c_int, [c_void_p, c_void_p, c_int64, c_void_p, c_int64, c_void_p]),
@@ -242,6 +248,44 @@ def ffn_gateup(x, norm_w, w13, g_out, eps, ws: Workspace) -> None:
     hidden = w13.shape[0] // 2
     _check(lib().mb200_ffn_gateup(_ptr(x), _ptr(norm_w), _ptr(w13), _ptr(g_out), T, dim, hidden, eps, ws.ptr, ws.nbytes, _stream()),
            "mb200_ffn_gateup")
+
+
+class LoraStruct(ctypes.Structure):
+    """mb200_lora (include/mistral_b200.h)."""
+    _fields_ = [("a_w", c_void_p), ("b_w", c_void_p), ("rank_cols", c_int64), ("scaling", c_float), ("a_buf", c_void_p), ("l_buf", c_void_p)]
+
+
+def lora_struct(a_w: torch.Tensor, b_w: torch.Tensor, scaling: float, a_buf: torch.Tensor, l_buf: torch.Tensor) -> LoraStruct:
+    """One adapter of a fused Linear: packed a_w [R, K], b_w [N, R], scratch a_buf [>= T, R] and l_buf [>= T, N] (bf16)."""
+    R = a_w.shape[0]
+    assert b_w.shape[1] == R and a_buf.shape[-1] == R and l_buf.shape[-1] == b_w.shape[0]
+    return LoraStruct(_ptr(a_w), _ptr(b_w), R, scaling, _ptr(a_buf), _ptr(l_buf))
+
+
+def _lora_ref(lora: LoraStruct):
+    return ctypes.cast(ctypes.pointer(lora), c_void_p)
+
+
+def attn_qkv_lora(x, norm_w, wqkv, rope, positions, q_out, k_out, v_out, cache_k, cache_v, cache_rows, n_heads, n_kv_heads, head_dim, eps,
+                  ws: Workspace, lora: LoraStruct) -> None:
+    T, dim = x.shape
+    _check(lib().mb200_attn_qkv_lora(_ptr(x), _ptr(norm_w), _ptr(wqkv), _ptr(rope), _ptr(positions), _ptr(q_out), _ptr(k_out), _ptr(v_out),
+                                     _ptr(cache_k), _ptr(cache_v), _ptr(cache_rows), T, dim, n_heads, n_kv_heads, head_dim, eps, ws.ptr,
+                                     ws.nbytes, _stream(), _lora_ref(lora)), "mb200_attn_qkv_lora")
+
+
+def ffn_gateup_lora(x, norm_w, w13, g_out, eps, ws: Workspace, lora: LoraStruct) -> None:
+    T, dim = x.shape
+    hidden = w13.shape[0] // 2
+    _check(lib().mb200_ffn_gateup_lora(_ptr(x), _ptr(norm_w), _ptr(w13), _ptr(g_out), T, dim, hidden, eps, ws.ptr, ws.nbytes, _stream(),
+                                       _lora_ref(lora)), "mb200_ffn_gateup_lora")
+
+
+def linear_residual_lora(x, w, residual, out, ws: Workspace, lora: LoraStruct) -> None:
+    T, K = x.shape
+    N = w.shape[0]
+    _check(lib().mb200_linear_residual_lora(_ptr(x), _ptr(w), _ptr(residual), _ptr(out), T, N, K, ws.ptr, ws.nbytes, _stream(),
+                                            _lora_ref(lora)), "mb200_linear_residual_lora")
 
 
 def lm_head(x, norm_w, w_out, logits, eps, ws: Workspace) -> None:

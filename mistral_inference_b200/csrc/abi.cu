@@ -13,6 +13,7 @@
 #include "gemm_mma.cuh"
 #include "gemm_streamk.cuh"
 #include "gemm_wgmma.cuh"
+#include "lora.cuh"
 #include "moe.cuh"
 #include "sampling.cuh"
 #include "skinny_linear.cuh"
@@ -72,6 +73,55 @@ static int run_linear(const void* x, const void* norm_w, const void* w, const Ep
   if (wgmma_gemm_eligible(T, N, K)) return launch_gemm_wgmma<MODE>(g, st);
   return launch_gemm_mma<MODE>(g, st);
 }
+
+// Un-merged LoRA around one fused Linear (include/mistral_b200.h): down projection -> up projection -> base GEMM whose epilogue
+// adds bf16(l * scaling) before the mode's work.  For T > MB200_SKINNY_MAX_T the input is normed once into the workspace and both
+// the down kernel and the base GEMM read it; for T <= MB200_SKINNY_MAX_T both are weight-streaming GEMVs that norm in-kernel.
+template <int MODE>
+static int run_linear_lora(const void* x, const void* norm_w, const void* w, EpiParams epi, const mb200_lora* lora, int64_t T, int64_t N,
+                           int64_t K, float eps, void* workspace, size_t workspace_bytes, cudaStream_t st) {
+  MB_CHECK_ARG(lora && lora->a_w && lora->b_w && lora->a_buf && lora->l_buf, "lora: null pointer");
+  const int64_t R = lora->rank_cols;
+  MB_CHECK_ARG(R >= 64 && R % 64 == 0 && K % 64 == 0, "lora: rank_cols=%lld and K=%lld must be multiples of 64", (long long)R, (long long)K);
+  MB_CHECK_ARG(T >= 1, "lora: T=%lld", (long long)T);
+  MB_CHECK_ARG(((uintptr_t)lora->a_buf & 15) == 0 && ((uintptr_t)lora->l_buf & 15) == 0,
+               "lora: a_buf and l_buf must be 16-byte aligned (l_buf doubles as fp32 split-K scratch)");
+  const void* xn = x;
+  int rc;
+  if (T <= MB200_SKINNY_MAX_T) {
+    SkinnyParams p;
+    p.x = x;
+    p.norm_w = norm_w;
+    p.w = lora->a_w;
+    p.N = (int)R;
+    p.K = (int)K;
+    p.eps = eps;
+    p.epi.out = lora->a_buf;
+    p.epi.ld_out = R;
+    rc = norm_w ? launch_skinny<EPI_STORE, true>(p, (int)T, st) : launch_skinny<EPI_STORE, false>(p, (int)T, st);
+  } else {
+    if (norm_w) {
+      const size_t need = kWsHeader + SK_PARTIAL_BYTES + align256((size_t)T * K * 2);
+      if (workspace == nullptr || workspace_bytes < need) return fail(MB200_E_WORKSPACE, "linear: workspace %zu < %zu", workspace_bytes, need);
+      void* normed = (uint8_t*)workspace + kWsHeader + SK_PARTIAL_BYTES;  // where run_linear puts it
+      rc = run_rmsnorm(x, norm_w, normed, T, K, eps, st);
+      if (rc) return rc;
+      xn = normed;
+      norm_w = nullptr;
+    }
+    rc = launch_lora_down(xn, lora->a_w, lora->a_buf, T, R, K, lora->l_buf, (size_t)T * N * 2, st);
+  }
+  if (rc) return rc;
+  EpiParams up;
+  up.out = lora->l_buf;
+  up.ld_out = N;
+  rc = run_linear<EPI_STORE>(lora->a_buf, nullptr, lora->b_w, up, T, N, R, 0.f, workspace, workspace_bytes, st);
+  if (rc) return rc;
+  epi.lora_l = lora->l_buf;
+  epi.ld_lora = N;
+  epi.lora_scaling = lora->scaling;
+  return run_linear<MODE | EPI_LORA>(xn, norm_w, w, epi, T, N, K, eps, workspace, workspace_bytes, st);
+}
 }  // namespace mb200
 
 using namespace mb200;
@@ -111,9 +161,10 @@ int mb200_rmsnorm(const void* x, const void* w, void* out, int64_t T, int64_t di
   return run_rmsnorm(x, w, out, T, dim, eps, (cudaStream_t)stream);
 }
 
-int mb200_attn_qkv(const void* x, const void* norm_w, const void* wqkv, const float* rope, const int32_t* positions, void* q_out, void* k_out,
-                   void* v_out, void* cache_k, void* cache_v, const int32_t* cache_rows, int64_t T, int64_t dim, int64_t n_heads,
-                   int64_t n_kv_heads, int64_t head_dim, float eps, void* workspace, size_t workspace_bytes, void* stream) {
+static int attn_qkv_impl(const void* x, const void* norm_w, const void* wqkv, const float* rope, const int32_t* positions, void* q_out,
+                         void* k_out, void* v_out, void* cache_k, void* cache_v, const int32_t* cache_rows, int64_t T, int64_t dim,
+                         int64_t n_heads, int64_t n_kv_heads, int64_t head_dim, float eps, void* workspace, size_t workspace_bytes,
+                         void* stream, const mb200_lora* lora) {
   MB_CHECK_ARG(x && norm_w && wqkv && rope && positions && q_out && k_out && v_out, "attn_qkv: null pointer");
   MB_CHECK_ARG(head_dim == kHeadDim || head_dim == 64, "attn_qkv: head_dim=%lld unsupported (64 or 128)", (long long)head_dim);
   MB_CHECK_ARG(cache_rows == nullptr || (cache_k && cache_v), "attn_qkv: cache_rows without cache pointers");
@@ -130,7 +181,24 @@ int mb200_attn_qkv(const void* x, const void* norm_w, const void* wqkv, const fl
   e.kv_dim = (int)(n_kv_heads * head_dim);
   e.head_dim = (int)head_dim;
   const int64_t N = (n_heads + 2 * n_kv_heads) * head_dim;
+  if (lora) return run_linear_lora<EPI_QKV_ROPE>(x, norm_w, wqkv, e, lora, T, N, dim, eps, workspace, workspace_bytes, (cudaStream_t)stream);
   return run_linear<EPI_QKV_ROPE>(x, norm_w, wqkv, e, T, N, dim, eps, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+int mb200_attn_qkv(const void* x, const void* norm_w, const void* wqkv, const float* rope, const int32_t* positions, void* q_out, void* k_out,
+                   void* v_out, void* cache_k, void* cache_v, const int32_t* cache_rows, int64_t T, int64_t dim, int64_t n_heads,
+                   int64_t n_kv_heads, int64_t head_dim, float eps, void* workspace, size_t workspace_bytes, void* stream) {
+  return attn_qkv_impl(x, norm_w, wqkv, rope, positions, q_out, k_out, v_out, cache_k, cache_v, cache_rows, T, dim, n_heads, n_kv_heads,
+                       head_dim, eps, workspace, workspace_bytes, stream, nullptr);
+}
+
+int mb200_attn_qkv_lora(const void* x, const void* norm_w, const void* wqkv, const float* rope, const int32_t* positions, void* q_out,
+                        void* k_out, void* v_out, void* cache_k, void* cache_v, const int32_t* cache_rows, int64_t T, int64_t dim,
+                        int64_t n_heads, int64_t n_kv_heads, int64_t head_dim, float eps, void* workspace, size_t workspace_bytes,
+                        void* stream, const mb200_lora* lora) {
+  MB_CHECK_ARG(lora, "attn_qkv_lora: null adapter");
+  return attn_qkv_impl(x, norm_w, wqkv, rope, positions, q_out, k_out, v_out, cache_k, cache_v, cache_rows, T, dim, n_heads, n_kv_heads,
+                       head_dim, eps, workspace, workspace_bytes, stream, lora);
 }
 
 int mb200_decode_meta(int32_t* seqpos_dev, int32_t* meta_dev, int64_t B, const int32_t* windows_host, int64_t n_windows, void* stream) {
@@ -269,6 +337,18 @@ int mb200_linear_residual(const void* x, const void* w, const void* residual, vo
   return run_linear<EPI_STORE>(x, nullptr, w, e, T, N, K, 0.f, workspace, workspace_bytes, (cudaStream_t)stream);
 }
 
+int mb200_linear_residual_lora(const void* x, const void* w, const void* residual, void* out, int64_t T, int64_t N, int64_t K,
+                               void* workspace, size_t workspace_bytes, void* stream, const mb200_lora* lora) {
+  MB_CHECK_ARG(x && w && out && lora, "linear_residual_lora: null pointer");
+  EpiParams e;
+  e.out = out;
+  e.residual = residual;
+  e.ld_out = N;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (residual) return run_linear_lora<EPI_RESIDUAL>(x, nullptr, w, e, lora, T, N, K, 0.f, workspace, workspace_bytes, st);
+  return run_linear_lora<EPI_STORE>(x, nullptr, w, e, lora, T, N, K, 0.f, workspace, workspace_bytes, st);
+}
+
 int mb200_linear_bias(const void* x, const void* w, const void* bias, void* out, int64_t T, int64_t N, int64_t K, int gelu, void* workspace,
                       size_t workspace_bytes, void* stream) {
   MB_CHECK_ARG(x && w && out, "linear_bias: null pointer");
@@ -329,6 +409,15 @@ int mb200_ffn_gateup(const void* x, const void* norm_w, const void* w13, void* g
   e.out = g_out;
   e.ld_out = hidden;
   return run_linear<EPI_SWIGLU>(x, norm_w, w13, e, T, 2 * hidden, dim, eps, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+int mb200_ffn_gateup_lora(const void* x, const void* norm_w, const void* w13, void* g_out, int64_t T, int64_t dim, int64_t hidden, float eps,
+                          void* workspace, size_t workspace_bytes, void* stream, const mb200_lora* lora) {
+  MB_CHECK_ARG(x && w13 && g_out && lora, "ffn_gateup_lora: null pointer");
+  EpiParams e;
+  e.out = g_out;
+  e.ld_out = hidden;
+  return run_linear_lora<EPI_SWIGLU>(x, norm_w, w13, e, lora, T, 2 * hidden, dim, eps, workspace, workspace_bytes, (cudaStream_t)stream);
 }
 
 int mb200_lm_head(const void* x, const void* norm_w, const void* w_out, float* logits, int64_t T, int64_t dim, int64_t vocab, float eps,

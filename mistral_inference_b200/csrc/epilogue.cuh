@@ -18,6 +18,11 @@ enum EpiMode : int {
   EPI_BIAS = 6,      // out[t, n] = bf16(acc + bias[n]) (bias may be null: bf16(acc))  nn.Linear(bias=True) (vision_encoder.py:108,114)
   EPI_BIAS_GELU = 7, // out[t, n] = bf16( gelu_erf( bf16(acc + bias[n]) ) )           nn.GELU() after w_in (vision_encoder.py:117)
 };
+// Flag OR-ed into EPI_STORE / EPI_RESIDUAL / EPI_SWIGLU / EPI_QKV_ROPE: the un-merged LoRA combine (LoRALinear.forward,
+// lora.py:71-74) runs on the Linear's bf16 output before the mode's own work:
+//   y = bf16(y + bf16(L[t, n] * scaling))     L = the adapter's up-projection output, bf16 [T, ld_lora]
+// Instantiations without the flag compile to the same code as before.
+constexpr int EPI_LORA = 16;
 
 constexpr int kMaxPeers = 8;
 
@@ -44,12 +49,23 @@ struct EpiParams {
   const void* row_w = nullptr;  // bf16 [rows]
   void* peer_out[kMaxPeers] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
   int n_peers = 0;
+  // EPI_LORA
+  const void* lora_l = nullptr;  // bf16 [T, ld_lora], columns in the weight's row order
+  int64_t ld_lora = 0;
+  float lora_scaling = 0.f;
 };
 
-template <int MODE>
+template <int FLAGS>
 __device__ __forceinline__ void epi_pair(const EpiParams& p, int t, int n, float acc0, float acc1) {
+  constexpr int MODE = FLAGS & ~EPI_LORA;
   // the Linear's own output rounding (bf16 result of nn.Linear)
-  const float y0 = round_bf16(acc0), y1 = round_bf16(acc1);
+  float y0 = round_bf16(acc0), y1 = round_bf16(acc1);
+  if constexpr ((FLAGS & EPI_LORA) != 0) {
+    static_assert(MODE == EPI_STORE || MODE == EPI_RESIDUAL || MODE == EPI_SWIGLU || MODE == EPI_QKV_ROPE, "LoRA combine: unsupported mode");
+    const uint32_t l = *reinterpret_cast<const uint32_t*>(reinterpret_cast<const uint16_t*>(p.lora_l) + (int64_t)t * p.ld_lora + n);
+    y0 = round_bf16(y0 + round_bf16(bf16lo(l) * p.lora_scaling));
+    y1 = round_bf16(y1 + round_bf16(bf16hi(l) * p.lora_scaling));
+  }
   if constexpr (MODE == EPI_STORE) {
     *reinterpret_cast<uint32_t*>(reinterpret_cast<uint16_t*>(p.out) + (int64_t)t * p.ld_out + n) = pack_bf16x2(y0, y1);
   } else if constexpr (MODE == EPI_RESIDUAL) {

@@ -18,10 +18,16 @@ from . import _abi
 from .args import PATCH_MERGE, TransformerArgs
 from .cache import BufferCache, CacheInputMetadata
 from .rope import precompute_freqs_cis
-from .transformer_layers import RMSNorm, TransformerBlock
+from .transformer_layers import LoraAdapter, RMSNorm, TransformerBlock
 from .vision_encoder import PatchMerger, VisionLanguageAdapter, VisionTransformer
 
 ROPE_TABLE_LEN = 128_000  # transformer.py:116
+# the LoRALinear modules of a text block (transformer_layers.py:50-54,100-103): name -> (adapter attribute path, segment)
+_LORA_LINEARS = {"attention.wq": ("attention.wqkv_lora", 0), "attention.wk": ("attention.wqkv_lora", 1),
+                 "attention.wv": ("attention.wqkv_lora", 2), "attention.wo": ("attention.wo_lora", 0),
+                 "feed_forward.w1": ("feed_forward.w13_lora", 0), "feed_forward.w3": ("feed_forward.w13_lora", 1),
+                 "feed_forward.w2": ("feed_forward.w2_lora", 0)}
+_LORA_PARTS = (".linear.weight", ".lora_A.weight", ".lora_B.weight")
 _VISION_PREFIXES = ("vision_encoder.", "vision_language_adapter.", "patch_merger.", "pre_mm_projector_norm.")  # transformer.py:279-291
 _NVTX = os.environ.get("MB200_NVTX", "0") == "1"
 
@@ -57,6 +63,9 @@ class Transformer(nn.Module):
         `e % world == rank` over the ranks of `expert_group` (default process group), everything else replicated, one
         all-reduce of [T, dim] per MoE layer (SURVEY.md 8e)."""
         super().__init__()
+        if args.lora is not None and args.moe is not None:
+            raise NotImplementedError("un-merged LoRA on mixture-of-experts layers is not built: the grouped expert GEMMs have no "
+                                      "LoRA stage (merge the adapter instead: args.lora = None, then load_lora)")
         self.args = args
         self.expert_parallel = expert_parallel or (0, 1)
         assert 0 <= self.expert_parallel[0] < self.expert_parallel[1], self.expert_parallel
@@ -295,7 +304,9 @@ class Transformer(nn.Module):
                 and len(set(cache.cache_sizes)) <= 8)
 
     def _megakernel_ok(self, B: int) -> bool:
+        # the megakernel has no LoRA stage: with un-merged adapters batch 1 takes the per-layer graph path
         return (B == 1 and self.num_pipeline_ranks == 1 and self.expert_parallel[1] == 1 and self.args.n_kv_heads <= 8
+                and self.args.lora is None
                 and os.environ.get("MB200_MEGAKERNEL", "1") != "0"
                 and (self.args.moe is None or (self.args.moe.num_experts <= 32 and self.args.moe.num_experts_per_tok <= 4)))
 
@@ -472,9 +483,12 @@ class Transformer(nn.Module):
     def _assign(self, k: str, v: torch.Tensor) -> bool:
         """Copies reference-keyed tensor `v` into the packed parameters.  Returns False when the key belongs to
         another pipeline rank."""
-        def put(dst: torch.Tensor) -> None:
+        def put(dst: torch.Tensor, setter=None, seg: int = 0) -> None:
             assert dst.shape == v.shape, f"{k}: shape {tuple(v.shape)} != expected {tuple(dst.shape)}"
-            dst.copy_(v)
+            if setter is None:
+                dst.copy_(v)
+            else:
+                setter(seg, v)
 
         if k == "tok_embeddings.weight":
             if self.tok_embeddings is None:
@@ -505,6 +519,23 @@ class Transformer(nn.Module):
     def _assign_block(blk: TransformerBlock, k: str, rest: str, put) -> bool:
         """`rest` = the key below `layers.{i}.` of one TransformerBlock (text or vision)."""
         att = blk.attention
+        if att.lora is not None:
+            name, part = rest.rsplit(".", 1)[0], ""
+            for suffix in _LORA_PARTS:
+                if rest.endswith(suffix):
+                    name, part = rest[: -len(suffix)], suffix
+            if name in _LORA_LINEARS:
+                path, seg = _LORA_LINEARS[name]
+                adapter = blk.get_submodule(path)
+                if part == ".lora_A.weight":
+                    put(adapter.lora_A(seg), adapter.put_A, seg)
+                    return True
+                if part == ".lora_B.weight":
+                    put(adapter.lora_B(seg), adapter.put_B, seg)
+                    return True
+                if part == "":  # a full checkpoint's plain weight: zero adapter (lora.py:76-89)
+                    adapter.zero(seg)
+                rest = name + ".weight"
         if rest == "attention.wq.weight":
             put(att.wqkv[: att.q_dim])
         elif rest == "attention.wk.weight":
@@ -594,11 +625,20 @@ class Transformer(nn.Module):
                 else:
                     logging.debug("Skipping parameter %s at pipeline rank %d", k, self.pipeline_rank)
         if strict:
-            missing = set(self.reference_keys()) - loaded
+            missing = self._missing_keys(loaded)
             assert not missing, f"missing keys: {sorted(missing)[:8]}"
 
     def reference_keys(self) -> List[str]:
         return list(self.state_dict().keys())
+
+    def _missing_keys(self, loaded) -> set:
+        """Keys of this rank that a load left unset.  With un-merged adapters a plain `X.weight` provides `X.linear.weight` and
+        adapters may be absent (they stay zero); the reference's post-hook clears every missing key (lora.py:66-69), this keeps
+        the base weights strict."""
+        if self.args.lora is None:
+            return set(self.reference_keys()) - set(loaded)
+        have = set(loaded) | {k[: -len(".weight")] + ".linear.weight" for k in loaded}
+        return {k for k in self.reference_keys() if k not in have and not k.endswith((".lora_A.weight", ".lora_B.weight"))}
 
     def state_dict(self, *args: Any, **kwargs: Any) -> Dict[str, torch.Tensor]:  # type: ignore[override]
         """Reference-keyed views of the packed parameters."""
@@ -630,10 +670,8 @@ class Transformer(nn.Module):
     @staticmethod
     def _block_state(out: Dict[str, torch.Tensor], p: str, blk: TransformerBlock) -> None:
         att = blk.attention
-        out[p + "attention.wq.weight"] = att.wq.weight
-        out[p + "attention.wk.weight"] = att.wk.weight
-        out[p + "attention.wv.weight"] = att.wv.weight
-        out[p + "attention.wo.weight"] = att.wo_weight
+        for n in ("wq", "wk", "wv", "wo"):
+            Transformer._linear_state(out, p, blk, "attention." + n, getattr(att, n).weight)
         out[p + "attention_norm.weight"] = blk.attention_norm.weight
         out[p + "ffn_norm.weight"] = blk.ffn_norm.weight
         ff = blk.feed_forward
@@ -644,11 +682,24 @@ class Transformer(nn.Module):
                     out[p + f"feed_forward.experts.{e}.{n}.weight"] = getattr(ex, n).weight
         else:
             for n in ("w1", "w2", "w3"):
-                out[p + f"feed_forward.{n}.weight"] = getattr(ff, n).weight
+                Transformer._linear_state(out, p, blk, "feed_forward." + n, getattr(ff, n).weight)
 
-    # ------------------------------------------------------------------ LoRA, merged path (lora.py:92-155 with args.lora is None)
+    @staticmethod
+    def _linear_state(out: Dict[str, torch.Tensor], p: str, blk: TransformerBlock, name: str, weight: torch.Tensor) -> None:
+        """`X.weight`, or with un-merged adapters LoRALinear's `X.lora_A.weight`, `X.lora_B.weight`, `X.linear.weight`."""
+        if blk.attention.lora is None:
+            out[p + name + ".weight"] = weight
+            return
+        path, seg = _LORA_LINEARS[name]
+        adapter = blk.get_submodule(path)
+        out[p + name + ".lora_A.weight"] = adapter.lora_A(seg)
+        out[p + name + ".lora_B.weight"] = adapter.lora_B(seg)
+        out[p + name + ".linear.weight"] = weight
+
+    # ------------------------------------------------------------------ LoRA (lora.py:92-155)
     def load_lora(self, lora_path: Union[Path, str], scaling: float = 2.0) -> None:
-        """Loads a LoRA checkpoint and MERGES it into the packed weights (lora.py:93-101,120-139): the forward path is unchanged."""
+        """Loads a LoRA checkpoint.  args.lora None: MERGES it into the packed weights (lora.py:120-139).  args.lora set: copies
+        it into the un-merged adapters (lora.py:140-155), replacing the previous adapter of every Linear it names."""
         import safetensors.torch
 
         lora_path = Path(lora_path)
@@ -656,15 +707,25 @@ class Transformer(nn.Module):
         self._load_lora_state_dict(safetensors.torch.load_file(str(lora_path)), scaling=scaling)
 
     def _load_lora_state_dict(self, lora_state_dict: Dict[str, torch.Tensor], scaling: float = 2.0) -> None:
-        """weight <- weight + (lora_B @ lora_A) * scaling for every Linear of this rank except the output layer, with the same
-        torch ops and dtype as the reference (lora.py:129-137).  Un-merged adapters (args.lora set) are outside the hot path."""
+        """args.lora None: weight <- weight + (lora_B @ lora_A) * scaling for every Linear of this rank except the output layer,
+        with the same torch ops and dtype as the reference (lora.py:129-137).
+        args.lora set: each `X.lora_A/B.weight` is copied in place into this rank's adapter slots (captured decode graphs keep
+        their pointers).  `scaling` is ignored, as in the reference: every adapter keeps args.lora.scaling.  Keys of layers that
+        other pipeline ranks own are skipped (the reference's strict load_state_dict would raise on them)."""
         lora_dtypes = set(p.dtype for p in lora_state_dict.values())
         assert len(lora_dtypes) == 1, f"LoRA weights have multiple different dtypes {lora_dtypes}. All weights need to have the same dtype"
         lora_dtype = lora_dtypes.pop()
         assert lora_dtype == self.dtype, f"LoRA weights dtype differs from model's dtype {lora_dtype} != {self.dtype}"
         assert all("lora" in key for key in lora_state_dict.keys())
-        assert self.args.lora is None, "un-merged LoRA adapters are outside the accelerated hot path: merge them (args.lora = None)"
         lora_state_dict = {k: v.to(self.device) for k, v in lora_state_dict.items()}
+        if self.args.lora is not None:
+            with torch.no_grad():
+                for k, v in lora_state_dict.items():
+                    if not k.endswith((".lora_A.weight", ".lora_B.weight")) or not k.startswith("layers."):
+                        raise ValueError(f"Unexpected key {k}")
+                    if not self._assign(k, v):
+                        logging.debug("Skipping parameter %s at pipeline rank %d", k, self.pipeline_rank)
+            return
         with torch.no_grad():
             for key, weight in self.state_dict().items():
                 if not key.endswith(".weight") or key == "output.weight" or not key.startswith("layers."):
@@ -684,7 +745,13 @@ class Transformer(nn.Module):
             dev = torch.device("cuda", torch.cuda.current_device())
         with torch.device("meta"):
             m = Transformer(args, **kwargs)
-        return m.to(dtype=dtype).to_empty(device=dev)
+        m = m.to(dtype=dtype).to_empty(device=dev)
+        with torch.no_grad():
+            for mod in m.modules():  # the packed adapters' zeros outside the segments are part of the format
+                if isinstance(mod, LoraAdapter):
+                    mod.a.zero_()
+                    mod.b.zero_()
+        return m
 
     @staticmethod
     def from_folder(folder: Union[Path, str], max_batch_size: int = 1, num_pipeline_ranks: int = 1,
@@ -728,6 +795,6 @@ class Transformer(nn.Module):
                     for k in keys:
                         if model._owns_key(k) and model._assign(k, f.get_tensor(k)):
                             loaded_keys.add(k)
-                missing = set(model.reference_keys()) - loaded_keys
+                missing = model._missing_keys(loaded_keys)
                 assert not missing, f"missing keys: {sorted(missing)[:8]}"
         return model.eval()

@@ -5,8 +5,9 @@ include/mistral_b200.h); weights are stored pre-packed for the fused kernels:
   Attention.wqkv  [(H + 2*KV) * hd, dim] = wq ++ wk ++ wv        (one GEMM / one weight stream)
   FeedForward.w13 [2 * hidden, dim], row 2i = w1[i], row 2i+1 = w3[i]  (SiLU*mul in the epilogue)
 `wq/wk/wv/w1/w3` are exposed as zero-copy views for state-dict compatibility.
+With `lora` set (un-merged adapters) each fused call also owns a packed LoraAdapter and runs the `_lora` entry points.
 """
-from typing import Optional, Tuple
+from typing import List, Optional, Tuple
 
 import torch
 from torch import nn
@@ -28,6 +29,62 @@ class _WeightView:
         return self._getter()
 
 
+class LoraAdapter(nn.Module):
+    """The un-merged LoRA adapters (lora.py:22-89) of one fused call, packed for the `_lora` entry points (include/mistral_b200.h):
+      a [R, in]  rows s*r .. s*r + r - 1 = lora_A of segment s, R = S*r rounded up to 64, padding rows zero
+      b [N, R]   row n = lora_B of n's segment in that segment's r columns, zeros elsewhere; `interleaved` (w13): segment s owns
+                 rows 2i + s, like FeedForward.w13
+    `lora_A(s)` / `lora_B(s)` are zero-copy views under the reference's names.  Loads copy in place (captured decode graphs hold
+    the pointers) and keep the zeros: every entry outside a segment's views stays zero."""
+
+    def __init__(self, in_features: int, segments: List[int], lora: LoraArgs, interleaved: bool = False):
+        super().__init__()
+        assert not interleaved or (len(segments) == 2 and segments[0] == segments[1])
+        self.rank = lora.rank
+        self.scaling = float(lora.scaling)  # fixed at construction, like LoRALinear.scaling
+        self.segments = list(segments)
+        self.interleaved = interleaved
+        self.rank_cols = -(-len(segments) * lora.rank // 64) * 64
+        self.a = nn.Parameter(torch.zeros(self.rank_cols, in_features), requires_grad=False)
+        self.b = nn.Parameter(torch.zeros(sum(segments), self.rank_cols), requires_grad=False)
+
+    def _cols(self, s: int) -> slice:
+        return slice(s * self.rank, (s + 1) * self.rank)
+
+    def _rows(self, s: int) -> torch.Tensor:
+        if self.interleaved:
+            return self.b.view(self.segments[0], 2, self.rank_cols)[:, s]
+        o = sum(self.segments[:s])
+        return self.b[o: o + self.segments[s]]
+
+    def lora_A(self, s: int) -> torch.Tensor:
+        return self.a[self._cols(s)]
+
+    def lora_B(self, s: int) -> torch.Tensor:
+        return self._rows(s)[:, self._cols(s)]
+
+    def put_A(self, s: int, v: torch.Tensor) -> None:
+        assert v.shape == self.lora_A(s).shape, f"lora_A: shape {tuple(v.shape)} != {tuple(self.lora_A(s).shape)} (rank {self.rank})"
+        self.lora_A(s).copy_(v)
+
+    def put_B(self, s: int, v: torch.Tensor) -> None:
+        assert v.shape == self.lora_B(s).shape, f"lora_B: shape {tuple(v.shape)} != {tuple(self.lora_B(s).shape)} (rank {self.rank})"
+        self.lora_B(s).copy_(v)
+
+    def zero(self, s: int) -> None:
+        """A plain `X.weight` checkpoint entry: segment s gets a zero adapter (lora.py:76-89)."""
+        self.lora_A(s).zero_()
+        self.lora_B(s).zero_()
+
+    def call(self, T: int) -> "_abi.LoraStruct":
+        """The adapter argument of one `_lora` call over T tokens, with its own scratch."""
+        a_buf = torch.empty(T, self.rank_cols, dtype=self.a.dtype, device=self.a.device)
+        l_buf = torch.empty(T, self.b.shape[0], dtype=self.a.dtype, device=self.a.device)
+        st = _abi.lora_struct(self.a, self.b, self.scaling, a_buf, l_buf)
+        st.keep = (a_buf, l_buf)  # alive until the call has been enqueued
+        return st
+
+
 class RMSNorm(nn.Module):
     """transformer_layers.py:109-120."""
 
@@ -45,7 +102,6 @@ class Attention(nn.Module):
 
     def __init__(self, dim: int, n_heads: int, head_dim: int, n_kv_heads: int, lora: Optional[LoraArgs] = None):
         super().__init__()
-        assert lora is None, "LoRA adapters must be merged into the weights (lora.py:118-139); unmerged LoRA is out of scope"
         self.dim = dim
         self.n_heads = n_heads
         self.head_dim = head_dim
@@ -56,6 +112,10 @@ class Attention(nn.Module):
         self.kv_dim = n_kv_heads * head_dim
         self.wqkv = nn.Parameter(torch.empty(self.q_dim + 2 * self.kv_dim, dim), requires_grad=False)
         self.wo_weight = nn.Parameter(torch.empty(dim, self.q_dim), requires_grad=False)
+        self.lora = lora
+        if lora is not None:
+            self.wqkv_lora = LoraAdapter(dim, [self.q_dim, self.kv_dim, self.kv_dim], lora)
+            self.wo_lora = LoraAdapter(self.q_dim, [dim], lora)
 
     # state-dict compatible views
     @property
@@ -85,22 +145,37 @@ class Attention(nn.Module):
         H, KV, hd = self.n_heads, self.n_kv_heads, self.head_dim
         if cache is None:
             # cache-less forward: unmasked over the whole flattened batch (SURVEY.md Appendix E-2)
-            _abi.attn_qkv(x, norm_w, self.wqkv, rope, positions, q, k, v, None, None, None, H, KV, hd, eps, ws)
+            self._qkv(x, norm_w, rope, positions, q, k, v, None, None, None, eps, ws)
             _abi.attn_prefill(q, k, v, None, None, None, None, out, 1, T, 0, H, KV, hd, causal=False)
             return out
         md = cache.metadata
         if md.prefill:
             # read the old ring, THEN write (transformer_layers.py:75-76)
-            _abi.attn_qkv(x, norm_w, self.wqkv, rope, positions, q, k, v, None, None, None, H, KV, hd, eps, ws)
+            self._qkv(x, norm_w, rope, positions, q, k, v, None, None, None, eps, ws)
             _abi.attn_prefill(q, k, v, cache.cache_k, cache.cache_v, md.q_start, md.seqpos, out, len(md.seqlens), md.max_seqlen,
                               md.window, H, KV, hd, causal=True, first_prefill=md.first_prefill)
             _abi.kv_ring_write(k, v, cache.cache_k, cache.cache_v, md.cache_rows, KV, hd)
         else:
             # write, THEN read the ring (transformer_layers.py:78-81); the scatter is the QKV kernel's epilogue
-            _abi.attn_qkv(x, norm_w, self.wqkv, rope, positions, q, k, v, cache.cache_k, cache.cache_v, md.cache_rows, H, KV, hd, eps, ws)
+            self._qkv(x, norm_w, rope, positions, q, k, v, cache.cache_k, cache.cache_v, md.cache_rows, eps, ws)
             B = len(md.seqlens)
             _abi.attn_decode(q, cache.cache_k, cache.cache_v, md.kv_len, out, H, KV, hd, decode_splits(B, KV, md.window), ws)
         return out
+
+    def _qkv(self, x, norm_w, rope, positions, q, k, v, cache_k, cache_v, cache_rows, eps, ws) -> None:
+        H, KV, hd = self.n_heads, self.n_kv_heads, self.head_dim
+        if self.lora is None:
+            _abi.attn_qkv(x, norm_w, self.wqkv, rope, positions, q, k, v, cache_k, cache_v, cache_rows, H, KV, hd, eps, ws)
+        else:
+            _abi.attn_qkv_lora(x, norm_w, self.wqkv, rope, positions, q, k, v, cache_k, cache_v, cache_rows, H, KV, hd, eps, ws,
+                               self.wqkv_lora.call(x.shape[0]))
+
+    def project_out(self, a: torch.Tensor, residual: torch.Tensor, out: torch.Tensor, ws: "_abi.Workspace") -> None:
+        """out = residual + wo(a)."""
+        if self.lora is None:
+            _abi.linear_residual(a, self.wo_weight, residual, out, ws)
+        else:
+            _abi.linear_residual_lora(a, self.wo_weight, residual, out, ws, self.wo_lora.call(a.shape[0]))
 
 
 def decode_splits(B: int, KV: int, W: int, n_sm: int = 132) -> int:
@@ -116,11 +191,14 @@ class FeedForward(nn.Module):
 
     def __init__(self, dim: int, hidden_dim: int, lora: Optional[LoraArgs] = None):
         super().__init__()
-        assert lora is None
         self.dim = dim
         self.hidden_dim = hidden_dim
         self.w13 = nn.Parameter(torch.empty(2 * hidden_dim, dim), requires_grad=False)
         self.w2_weight = nn.Parameter(torch.empty(dim, hidden_dim), requires_grad=False)
+        self.lora = lora
+        if lora is not None:
+            self.w13_lora = LoraAdapter(dim, [hidden_dim, hidden_dim], lora, interleaved=True)
+            self.w2_lora = LoraAdapter(hidden_dim, [dim], lora)
 
     @property
     def w1(self) -> _WeightView:
@@ -139,9 +217,13 @@ class FeedForward(nn.Module):
         """[norm] -> gate/up -> silu*mul -> down [+ residual]."""
         T = x.shape[0]
         g = torch.empty(T, self.hidden_dim, dtype=x.dtype, device=x.device)
-        _abi.ffn_gateup(x, norm_w, self.w13, g, eps, ws)
         out = torch.empty(T, self.dim, dtype=x.dtype, device=x.device)
-        _abi.linear_residual(g, self.w2_weight, residual, out, ws)
+        if self.lora is None:
+            _abi.ffn_gateup(x, norm_w, self.w13, g, eps, ws)
+            _abi.linear_residual(g, self.w2_weight, residual, out, ws)
+        else:
+            _abi.ffn_gateup_lora(x, norm_w, self.w13, g, eps, ws, self.w13_lora.call(T))
+            _abi.linear_residual_lora(g, self.w2_weight, residual, out, ws, self.w2_lora.call(T))
         return out
 
     def forward(self, x: torch.Tensor, ws: Optional["_abi.Workspace"] = None) -> torch.Tensor:
@@ -155,6 +237,9 @@ class TransformerBlock(nn.Module):
     def __init__(self, dim: int, hidden_dim: int, n_heads: int, n_kv_heads: int, head_dim: int, norm_eps: float,
                  lora: Optional[LoraArgs] = None, moe: Optional[MoeArgs] = None, expert_shard: Tuple[int, int] = (0, 1), expert_group=None):
         super().__init__()
+        if lora is not None and moe is not None:
+            raise NotImplementedError("un-merged LoRA on mixture-of-experts layers is not built: the grouped expert GEMMs have no "
+                                      "LoRA stage (merge the adapter instead: args.lora = None, then load_lora)")
         self.n_heads = n_heads
         self.dim = dim
         self.norm_eps = norm_eps
@@ -175,7 +260,7 @@ class TransformerBlock(nn.Module):
         # r = attention(attention_norm(x)); h = x + r        (transformer_layers.py:165-166)
         a = self.attention.attend(x, self.attention_norm.weight, self.norm_eps, rope, positions, cache, ws)
         h = torch.empty_like(x)
-        _abi.linear_residual(a, self.attention.wo_weight, x, h, ws)
+        self.attention.project_out(a, x, h, ws)
         # r = feed_forward(ffn_norm(h)); out = h + r          (transformer_layers.py:167-168)
         if isinstance(self.feed_forward, MoeLayer):
             hn = _abi.rmsnorm(h, self.ffn_norm.weight, self.norm_eps)

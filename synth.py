@@ -17,7 +17,7 @@ Folder layout is the reference's on-disk contract (transformer.py:297-336): `par
 import json
 import zlib
 from pathlib import Path
-from typing import Dict, Iterator, Tuple, Union
+from typing import Dict, Iterator, Optional, Tuple, Union
 
 import torch
 
@@ -142,14 +142,35 @@ def synth_state_dict(p: dict, seed: int = 0, dtype: torch.dtype = torch.bfloat16
     return {k: synth_tensor(k, shp, seed, dtype, device) for k, shp in state_dict_shapes(p)}
 
 
-def write_model_folder(folder: Union[str, Path], p: dict, seed: int = 0, dtype: torch.dtype = torch.bfloat16) -> Path:
-    """Writes `params.json` + `consolidated.safetensors` (the reference's on-disk contract)."""
+LORA_LINEARS = (("attention.wq", "q"), ("attention.wk", "kv"), ("attention.wv", "kv"), ("attention.wo", "o"), ("feed_forward.w1", "h"),
+                ("feed_forward.w2", "d"), ("feed_forward.w3", "h"))
+
+
+def synth_lora_state_dict(p: dict, rank: int, seed: int = 0, dtype: torch.dtype = torch.bfloat16, scale: float = 1.0,
+                          device: Union[str, torch.device] = "cpu") -> Dict[str, torch.Tensor]:
+    """A LoRA adapter for every LoRALinear of the text layers (lora.py:22-89): `X.lora_A.weight` [rank, in] and
+    `X.lora_B.weight` [out, rank], values of synth_tensor times `scale`."""
+    dim, hd, hid = p["dim"], p["head_dim"], p["hidden_dim"]
+    outs = {"q": p["n_heads"] * hd, "kv": p["n_kv_heads"] * hd, "o": dim, "h": hid, "d": dim}
+    ins = {"q": dim, "kv": dim, "o": p["n_heads"] * hd, "h": dim, "d": hid}
+    out: Dict[str, torch.Tensor] = {}
+    for i in range(p["n_layers"]):
+        for name, kind in LORA_LINEARS:
+            for key, shp in ((f"layers.{i}.{name}.lora_A.weight", (rank, ins[kind])), (f"layers.{i}.{name}.lora_B.weight", (outs[kind], rank))):
+                out[key] = (synth_tensor(key, shp, seed, torch.float32, device) * scale).to(dtype)
+    return out
+
+
+def write_model_folder(folder: Union[str, Path], p: dict, seed: int = 0, dtype: torch.dtype = torch.bfloat16,
+                       lora: Optional[dict] = None) -> Path:
+    """Writes `params.json` + `consolidated.safetensors` (the reference's on-disk contract).  `lora` = {"rank", "scaling"} adds
+    the params.json block that makes every text Linear a LoRALinear; the checkpoint stays a full one (zero adapters on load)."""
     import safetensors.torch
 
     folder = Path(folder)
     folder.mkdir(parents=True, exist_ok=True)
     with open(folder / "params.json", "w") as f:
-        json.dump(p, f)
+        json.dump(p if lora is None else dict(p, lora=lora), f)
     safetensors.torch.save_file(synth_state_dict(p, seed, dtype), str(folder / "consolidated.safetensors"))
     return folder
 
