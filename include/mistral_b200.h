@@ -340,6 +340,11 @@ int mb200_debug_set_barrier_timeline(void* device_buffer);
  * into `out` (NUL-terminated; NULL discards it), clears it, and switches recording on (enable != 0) or off.  MB200_E_INVALID
  * when `out` is too small or launches were dropped because the log filled up.  Tests use it to check which kernel a call chose. */
 int mb200_debug_launch_log(int enable, char* out, size_t out_bytes);
+/* Debug, host only: byte offsets into `workspace` at which mb200_decode_step leaves q of the last layer ([H*hd] bf16, after RoPE)
+ * and that layer's attention output ([H*hd] bf16, head-major) for the given geometry.  Both are 256-byte aligned.  Tests use it
+ * to check the attention phases of the step on their own. */
+int mb200_debug_decode_scratch(int64_t dim, int64_t hidden, int64_t n_heads, int64_t n_kv_heads, int64_t head_dim, int64_t n_experts,
+                               int64_t top_k, size_t* q_offset, size_t* attn_offset);
 
 /* Test-only: CUDA-core fp32 GEMM c[T, N] = a[T, K] w[N, K]^T used to cross-check the tensor-core kernels. */
 int mb200_test_gemm_naive(const void* a, const void* w, float* c, int64_t T, int64_t N, int64_t K, void* stream);

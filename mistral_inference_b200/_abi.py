@@ -68,6 +68,7 @@ _SIGNATURES = {
     "mb200_debug_set_decode_timeline": (c_int, [c_void_p]),
     "mb200_debug_set_barrier_timeline": (c_int, [c_void_p]),
     "mb200_debug_launch_log": (c_int, [c_int, c_void_p, c_size_t]),
+    "mb200_debug_decode_scratch": (c_int, [c_int64] * 7 + [ctypes.POINTER(c_size_t), ctypes.POINTER(c_size_t)]),
     "mb200_test_gemm_naive": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_void_p]),
 }
 
@@ -404,6 +405,14 @@ def launch_log(enable: bool) -> list:
     buf = ctypes.create_string_buffer(32768)
     _check(lib().mb200_debug_launch_log(int(enable), ctypes.cast(buf, c_void_p), len(buf)), "mb200_debug_launch_log")
     return buf.value.decode().splitlines()
+
+
+def decode_scratch(dim, hidden, n_heads, n_kv_heads, head_dim, n_experts: int = 0, top_k: int = 0):
+    """(q offset, attention-output offset) in bytes of the workspace that decode_step writes (include/mistral_b200.h)."""
+    q, a = c_size_t(0), c_size_t(0)
+    _check(lib().mb200_debug_decode_scratch(dim, hidden, n_heads, n_kv_heads, head_dim, n_experts, top_k, ctypes.byref(q), ctypes.byref(a)),
+           "mb200_debug_decode_scratch")
+    return q.value, a.value
 
 
 def test_gemm_naive(a, w) -> torch.Tensor:

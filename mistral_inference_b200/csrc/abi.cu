@@ -31,6 +31,26 @@ static unsigned long long* g_mk_prof_bar = nullptr;  // debug: decode megakernel
 constexpr size_t kWsHeader = 64 * 1024;  // persistent, zero-initialised by the caller once: self-resetting counters
 inline size_t align256(size_t v) { return (v + 255) & ~(size_t)255; }
 
+// Global scratch of mb200_decode_step after the workspace header, as byte offsets: each buffer starts on a 256-byte boundary.
+// mb200_debug_decode_scratch reports qbuf / abuf from the same function, so tests read what the kernel wrote.
+struct DecodeScratch {
+  size_t xbuf, hbuf, qbuf, abuf, gbuf, partial, end;
+};
+inline DecodeScratch decode_scratch(int64_t dim, int64_t hidden, int64_t n_heads, int64_t n_experts, int64_t top_k, int sms) {
+  const size_t q_dim = (size_t)n_heads * kHeadDim;
+  DecodeScratch s;
+  size_t off = kWsHeader;
+  auto take = [&](size_t bytes) { const size_t r = off; off += align256(bytes); return r; };
+  s.xbuf = take((size_t)2 * dim * 2);
+  s.hbuf = take((size_t)dim * 2);
+  s.qbuf = take(q_dim * 2);
+  s.abuf = take(q_dim * 2);
+  s.gbuf = take((size_t)(n_experts ? top_k : 1) * hidden * 2);
+  s.partial = take((size_t)sms * n_heads * (kHeadDim + 2) * sizeof(float));  // [slice = CTA][H][m, l, acc[128]]
+  s.end = off;
+  return s;
+}
+
 static int run_rmsnorm(const void* x, const void* w, void* out, int64_t T, int64_t dim, float eps, cudaStream_t st) {
   MB_CHECK_ARG(dim % 8 == 0 && T >= 0, "rmsnorm: dim=%lld must be a multiple of 8", (long long)dim);
   if (T == 0) return MB200_OK;
@@ -690,17 +710,16 @@ int mb200_decode_step(const mb200_layer_desc* layers_dev, const int32_t* windows
   p.bar_flags = (unsigned*)(ws + 16384);
   p.bar_epoch = (unsigned*)(ws + 20480);
   p.done_counter = (int*)(ws + 20480 + 128);
-  size_t off = kWsHeader;
-  auto take = [&](size_t bytes) { uint8_t* r = ws + off; off += align256(bytes); return r; };
-  p.xbuf = (bf16*)take((size_t)2 * dim * 2);
-  p.hbuf = (bf16*)take((size_t)dim * 2);
-  p.qbuf = (bf16*)take((size_t)q_dim * 2);
-  p.abuf = (bf16*)take((size_t)q_dim * 2);
-  p.gbuf = (bf16*)take((size_t)(n_experts ? top_k : 1) * hidden * 2);
-  p.partial = (float*)take((size_t)sms * n_heads * (kHeadDim + 2) * sizeof(float));  // [slice = CTA][H][m, l, acc[128]]
+  const DecodeScratch sc = decode_scratch(dim, hidden, n_heads, n_experts, top_k, sms);
+  p.xbuf = (bf16*)(ws + sc.xbuf);
+  p.hbuf = (bf16*)(ws + sc.hbuf);
+  p.qbuf = (bf16*)(ws + sc.qbuf);
+  p.abuf = (bf16*)(ws + sc.abuf);
+  p.gbuf = (bf16*)(ws + sc.gbuf);
+  p.partial = (float*)(ws + sc.partial);
   p.prof = g_mk_prof;
   p.prof_bar = g_mk_prof_bar;
-  if (workspace_bytes < off) return fail(MB200_E_WORKSPACE, "decode_step: workspace %zu < %zu", workspace_bytes, off);
+  if (workspace_bytes < sc.end) return fail(MB200_E_WORKSPACE, "decode_step: workspace %zu < %zu", workspace_bytes, sc.end);
 
   void* args[] = {(void*)&p};
   const void* fn = nullptr;
@@ -712,8 +731,20 @@ int mb200_decode_step(const mb200_layer_desc* layers_dev, const int32_t* windows
     case 8: fn = (const void*)decode_megakernel<8>; break;
     default: return fail(MB200_E_INVALID, "decode_step: H/KV=%d unsupported (1,2,4,6,8)", rep);
   }
+  note_launch("decode_megakernel<%d>", rep);
   MB_CHECK_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   MB_CHECK_CUDA(cudaLaunchCooperativeKernel(fn, dim3((unsigned)sms), dim3(MK_THREADS), args, smem, (cudaStream_t)stream));
+  return MB200_OK;
+}
+
+int mb200_debug_decode_scratch(int64_t dim, int64_t hidden, int64_t n_heads, int64_t n_kv_heads, int64_t head_dim, int64_t n_experts,
+                               int64_t top_k, size_t* q_offset, size_t* attn_offset) {
+  MB_CHECK_ARG(q_offset && attn_offset, "debug_decode_scratch: null pointer");
+  MB_CHECK_ARG(head_dim == kHeadDim && n_kv_heads > 0 && n_heads % n_kv_heads == 0 && dim > 0 && hidden > 0,
+               "debug_decode_scratch: bad shape (H=%lld, KV=%lld, hd=%lld)", (long long)n_heads, (long long)n_kv_heads, (long long)head_dim);
+  const DecodeScratch sc = decode_scratch(dim, hidden, n_heads, n_experts, top_k, 0);  // the SM count only sizes the last buffer
+  *q_offset = sc.qbuf;
+  *attn_offset = sc.abuf;
   return MB200_OK;
 }
 

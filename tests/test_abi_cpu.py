@@ -53,6 +53,20 @@ def test_launch_log_records_nothing_for_rejected_calls(built):
     assert _abi.launch_log(False) == []  # recording off: still empty
 
 
+@pytest.mark.parametrize("dim,hidden,H,KV,E,k", [(256, 256, 4, 2, 0, 0), (4096, 14336, 32, 8, 0, 0), (5120, 14336, 32, 8, 0, 0),
+                                                (6144, 16384, 48, 8, 8, 2), (256, 256, 40, 5, 0, 0)])
+def test_decode_scratch_offsets(built, dim, hidden, H, KV, E, k):
+    """Where decode_step leaves q and the attention output: 256-byte aligned, after the header, apart, inside the workspace."""
+    q, a = _abi.decode_scratch(dim, hidden, H, KV, 128, E, k)
+    nb = H * 128 * 2
+    total = _abi.workspace_bytes(1, dim, H, KV, 128, hidden, 32000, 1)
+    assert q % 256 == 0 and a % 256 == 0
+    assert _abi.WORKSPACE_HEADER_BYTES <= q and _abi.WORKSPACE_HEADER_BYTES <= a
+    assert q + nb <= a or a + nb <= q
+    assert max(q, a) + nb <= total
+    assert _abi.lib().mb200_debug_decode_scratch(dim, hidden, H, KV, 64, E, k, None, None) == -1
+
+
 def test_no_cpu_fallback():
     p = synth.shape("tiny")
     args = mi.TransformerArgs.from_dict(p)

@@ -23,7 +23,8 @@ from mistral_inference_b200.cache import BufferCache
 from mistral_inference_b200.transformer import Transformer
 from oracle import restatement as R
 
-from .util import (GOLDEN_CASES, LOGPROB_TOL, RouterProbe, case_params_prompts, load_golden, logit_tol, oracle_args, oracle_model)
+from .util import (GOLDEN_CASES, LOGPROB_TOL, RouterProbe, case_params_prompts, launched_kernels, load_golden, logit_tol, oracle_args,
+                   oracle_model)
 
 pytestmark = pytest.mark.gpu
 BF16_CASES = [c for c in GOLDEN_CASES if not c.endswith("fp32")]
@@ -398,6 +399,39 @@ def test_decode_megakernel(shape, over, prompt_len, steps, monkeypatch):
         ok = torch.isfinite(b)
         assert torch.equal(torch.isfinite(a), ok)
         assert (a[ok] - b[ok]).abs().max() <= 2 * 2.0 ** -7 * max(1.0, b[ok].abs().max().item())
+
+
+def test_decode_megakernel_long_context_ring_wrap(monkeypatch):
+    """Mistral-7B layer shapes with a 4096-slot ring: a 4090-token prompt, then 12 teacher-forced decode steps that wrap the ring
+    at position 4096 -- the megakernel (every step one decode_megakernel<4>) against the per-op path, whose decode attention is
+    exact-set tested at W = 4096 (tests/test_gpu_attention_edges.py)."""
+    p = synth.shape("mistral-7b", n_layers=2, vocab_size=4096, sliding_window=4096)
+    m = gpu_model(p, 1)
+    prompt_len, steps = 4090, 12
+    prompt = synth.synth_prompt(prompt_len, p["vocab_size"], 31)
+    toks = synth.synth_prompt(steps, p["vocab_size"], 32)
+
+    def run(megakernel: bool):
+        monkeypatch.setenv("MB200_MEGAKERNEL", "1" if megakernel else "0")
+        cache = new_cache(m, prompt_len + steps + 1)
+        m.forward(torch.tensor(prompt, device="cuda"), [prompt_len], cache)
+        out = []
+        names = launched_kernels(lambda: out.extend(m.forward(torch.tensor([t], device="cuda"), [1], cache).clone() for t in toks))
+        assert names.count("decode_megakernel<4>") == (steps if megakernel else 0), names
+        return torch.cat(out, 0), cache
+
+    mk, c1 = run(True)
+    per_op, c2 = run(False)
+    d = report("megakernel vs per-op, 7B shape, ring wrap at 4096", mk, per_op)
+    check_rows(d, per_op, None, "megakernel vs per-op at a 4096-slot ring")
+    top2 = per_op.float().topk(2, dim=-1).values
+    decisive = (top2[:, 0] - top2[:, 1]) > 2 * logit_tol(per_op)
+    assert torch.equal(mk.argmax(-1)[decisive], per_op.argmax(-1)[decisive])
+    for i in c1.cache_k:
+        for a, b in ((c1.cache_k[i][0].float(), c2.cache_k[i][0].float()), (c1.cache_v[i][0].float(), c2.cache_v[i][0].float())):
+            ok = torch.isfinite(b)
+            assert torch.equal(torch.isfinite(a), ok)
+            assert (a[ok] - b[ok]).abs().max() <= 2 * 2.0 ** -7 * max(1.0, b[ok].abs().max().item())
 
 
 @pytest.mark.parametrize("shape,over,B,prompt_len,steps", [
