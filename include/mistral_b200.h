@@ -342,9 +342,27 @@ int mb200_debug_set_barrier_timeline(void* device_buffer);
 int mb200_debug_launch_log(int enable, char* out, size_t out_bytes);
 /* Debug, host only: byte offsets into `workspace` at which mb200_decode_step leaves q of the last layer ([H*hd] bf16, after RoPE)
  * and that layer's attention output ([H*hd] bf16, head-major) for the given geometry.  Both are 256-byte aligned.  Tests use it
- * to check the attention phases of the step on their own. */
+ * to check the attention phases of the step on their own.  (offsets[2] and [3] of mb200_debug_decode_buffers.) */
 int mb200_debug_decode_scratch(int64_t dim, int64_t hidden, int64_t n_heads, int64_t n_kv_heads, int64_t head_dim, int64_t n_experts,
                                int64_t top_k, size_t* q_offset, size_t* attn_offset);
+/* Debug, host only: byte offsets into `workspace` of every buffer mb200_decode_step leaves behind, for the given geometry, in
+ * offsets[6]:
+ *   [0] x: the residual stream ping-pong, [2][dim] bf16; layer l writes its output to half (l + 1) & 1, the final norm reads
+ *       half n_layers & 1
+ *   [1] h of the last layer ([dim] bf16, after wo + residual)
+ *   [2] q of the last layer ([H*hd] bf16, after RoPE)
+ *   [3] the last layer's attention output ([H*hd] bf16, head-major)
+ *   [4] g of the last layer ([hidden] bf16 after SiLU * up; for MoE [top_k][hidden], the selected experts in ascending index)
+ *   [5] the attention slice partials ([SM count][H][hd + 2] fp32)
+ * Each buffer starts on a 256-byte boundary after the workspace header.  Tests use it to check the phases of the step on their own. */
+int mb200_debug_decode_buffers(int64_t dim, int64_t hidden, int64_t n_heads, int64_t n_kv_heads, int64_t head_dim, int64_t n_experts,
+                               int64_t top_k, size_t* offsets);
+/* Host only: MB200_OK when mb200_decode_step accepts these shapes on a device with `smem_optin` bytes of opt-in shared memory
+ * per block (<= 0: the current device's), else MB200_E_INVALID with the reason in mb200_last_error().  The same checks run at the
+ * start of mb200_decode_step: head_dim, H/KV, KV <= 8, the K chunking of dim / hidden / H*hd, an even vocab, the MoE limits and
+ * a ring of at least 9 stages next to the activation buffer (top_k * hidden bf16 for MoE). */
+int mb200_decode_step_supported(int64_t dim, int64_t hidden, int64_t n_heads, int64_t n_kv_heads, int64_t head_dim, int64_t vocab,
+                                int64_t n_experts, int64_t top_k, int64_t smem_optin);
 
 /* Test-only: CUDA-core fp32 GEMM c[T, N] = a[T, K] w[N, K]^T used to cross-check the tensor-core kernels. */
 int mb200_test_gemm_naive(const void* a, const void* w, float* c, int64_t T, int64_t N, int64_t K, void* stream);

@@ -8,7 +8,7 @@ import ctypes
 import os
 from ctypes import c_char_p, c_float, c_int, c_int64, c_size_t, c_void_p
 from pathlib import Path
-from typing import Optional
+from typing import NamedTuple, Optional
 
 import torch
 
@@ -69,6 +69,8 @@ _SIGNATURES = {
     "mb200_debug_set_barrier_timeline": (c_int, [c_void_p]),
     "mb200_debug_launch_log": (c_int, [c_int, c_void_p, c_size_t]),
     "mb200_debug_decode_scratch": (c_int, [c_int64] * 7 + [ctypes.POINTER(c_size_t), ctypes.POINTER(c_size_t)]),
+    "mb200_debug_decode_buffers": (c_int, [c_int64] * 7 + [ctypes.POINTER(c_size_t)]),
+    "mb200_decode_step_supported": (c_int, [c_int64] * 9),
     "mb200_test_gemm_naive": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_void_p]),
 }
 
@@ -413,6 +415,32 @@ def decode_scratch(dim, hidden, n_heads, n_kv_heads, head_dim, n_experts: int = 
     _check(lib().mb200_debug_decode_scratch(dim, hidden, n_heads, n_kv_heads, head_dim, n_experts, top_k, ctypes.byref(q), ctypes.byref(a)),
            "mb200_debug_decode_scratch")
     return q.value, a.value
+
+
+class DecodeBuffers(NamedTuple):
+    """Byte offsets into the workspace of every buffer decode_step leaves behind (include/mistral_b200.h)."""
+    x: int        # [2][dim] bf16 residual ping-pong: layer l writes half (l + 1) & 1
+    h: int        # [dim] bf16
+    q: int        # [H * 128] bf16
+    attn: int     # [H * 128] bf16
+    g: int        # [hidden] bf16, or [top_k][hidden] for MoE
+    partial: int  # [SM count][H][130] fp32
+
+
+def decode_buffers(dim, hidden, n_heads, n_kv_heads, head_dim, n_experts: int = 0, top_k: int = 0) -> DecodeBuffers:
+    off = (c_size_t * 6)()
+    _check(lib().mb200_debug_decode_buffers(dim, hidden, n_heads, n_kv_heads, head_dim, n_experts, top_k, off), "mb200_debug_decode_buffers")
+    return DecodeBuffers(*[int(v) for v in off])
+
+
+def decode_step_unsupported(dim, hidden, n_heads, n_kv_heads, head_dim, vocab, n_experts: int = 0, top_k: int = 0,
+                            smem_optin: int = 0) -> Optional[str]:
+    """None when decode_step accepts these shapes on a device with `smem_optin` bytes of opt-in shared memory per block (0: the
+    current device), else the reason it would refuse them."""
+    if lib().mb200_decode_step_supported(dim, hidden, n_heads, n_kv_heads, head_dim, vocab, n_experts, top_k, smem_optin) == 0:
+        return None
+    msg = lib().mb200_last_error()
+    return msg.decode() if msg else "?"
 
 
 def test_gemm_naive(a, w) -> torch.Tensor:

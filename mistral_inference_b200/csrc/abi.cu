@@ -32,7 +32,7 @@ constexpr size_t kWsHeader = 64 * 1024;  // persistent, zero-initialised by the 
 inline size_t align256(size_t v) { return (v + 255) & ~(size_t)255; }
 
 // Global scratch of mb200_decode_step after the workspace header, as byte offsets: each buffer starts on a 256-byte boundary.
-// mb200_debug_decode_scratch reports qbuf / abuf from the same function, so tests read what the kernel wrote.
+// mb200_debug_decode_buffers (and mb200_debug_decode_scratch) report the offsets from the same function, so tests read what the kernel wrote.
 struct DecodeScratch {
   size_t xbuf, hbuf, qbuf, abuf, gbuf, partial, end;
 };
@@ -49,6 +49,47 @@ inline DecodeScratch decode_scratch(int64_t dim, int64_t hidden, int64_t n_heads
   s.partial = take((size_t)sms * n_heads * (kHeadDim + 2) * sizeof(float));  // [slice = CTA][H][m, l, acc[128]]
   s.end = off;
   return s;
+}
+
+// Every shape rule of mb200_decode_step and its shared-memory plan, for a device with `smem_max` bytes of opt-in shared memory
+// per block.  mb200_decode_step_supported exposes the same function, so a caller learns before launching whether the step runs.
+struct DecodePlan {
+  int rep, n_stages;
+  size_t xs_bytes, smem;
+};
+static int decode_plan(int64_t dim, int64_t hidden, int64_t n_heads, int64_t n_kv_heads, int64_t head_dim, int64_t vocab, int64_t n_experts,
+                       int64_t top_k, int64_t smem_max, DecodePlan* out) {
+  MB_CHECK_ARG(head_dim == kHeadDim, "decode_step: head_dim=%lld unsupported (128 only)", (long long)head_dim);
+  MB_CHECK_ARG(dim > 0 && hidden > 0 && n_kv_heads >= 1 && n_heads % n_kv_heads == 0, "decode_step: H %% KV != 0");
+  const int64_t rep = n_heads / n_kv_heads;
+  MB_CHECK_ARG(rep == 1 || rep == 2 || rep == 4 || rep == 6 || rep == 8, "decode_step: H/KV=%lld unsupported (1,2,4,6,8)", (long long)rep);
+  MB_CHECK_ARG(n_kv_heads <= MK_CONSUMER_WARPS, "decode_step: n_kv_heads=%lld > %d (one consumer warp per kv head)", (long long)n_kv_heads,
+               MK_CONSUMER_WARPS);
+  MB_CHECK_ARG(n_kv_heads * kHeadDim * 2 + MK_KV_PAD <= MK_STAGE_BYTES / 8, "decode_step: a ring stage must hold 8 padded K/V position rows");
+  const int64_t q_dim = n_heads * head_dim;
+  auto cut_ok = [](int64_t K) { const int64_t nch = (K + MK_MAX_KC - 1) / MK_MAX_KC; return K % (nch * 8) == 0; };
+  MB_CHECK_ARG(cut_ok(dim) && cut_ok(hidden) && cut_ok(q_dim), "decode_step: dim/hidden/q_dim must split into 16-byte-aligned row chunks");
+  MB_CHECK_ARG(vocab > 0 && vocab % 2 == 0, "decode_step: vocab must be even");
+  MB_CHECK_ARG(n_experts == 0 || (top_k >= 1 && top_k <= MK_MAX_TOPK && top_k <= n_experts && n_experts <= 32),
+               "decode_step: bad MoE arguments (E=%lld, k=%lld)", (long long)n_experts, (long long)top_k);
+  // shared memory plan: x buffer (also the attention merge scratch), barriers + reduction scratch, the rest is the ring
+  int64_t widest = dim > hidden ? dim : hidden;
+  if (q_dim > widest) widest = q_dim;
+  size_t xs_bytes = (size_t)widest * 2;
+  if (n_experts && xs_bytes < (size_t)top_k * hidden * 2) xs_bytes = (size_t)top_k * hidden * 2;  // g of every selected expert
+  if (xs_bytes < 2048) xs_bytes = 2048;  // also the slice-merge scratch of phase 2b
+  xs_bytes = (xs_bytes + 127) & ~(size_t)127;
+  const size_t tail = 2 * MK_MAX_STAGES * sizeof(uint64_t) + 48 * sizeof(float) + sizeof(MoeRoute) + 8 + 64;
+  const int64_t room = smem_max - (int64_t)(xs_bytes + tail);
+  int n_stages = room > 0 ? (int)(room / MK_STAGE_BYTES) : 0;
+  if (n_stages > MK_MAX_STAGES) n_stages = MK_MAX_STAGES;
+  MB_CHECK_ARG(n_stages > MK_CONSUMER_WARPS, "decode_step: not enough shared memory for the weight ring (%d stages, %zu B of activations)",
+               n_stages, xs_bytes);
+  out->rep = (int)rep;
+  out->n_stages = n_stages;
+  out->xs_bytes = xs_bytes;
+  out->smem = (size_t)n_stages * MK_STAGE_BYTES + xs_bytes + tail;
+  return MB200_OK;
 }
 
 static int run_rmsnorm(const void* x, const void* w, void* out, int64_t T, int64_t dim, float eps, cudaStream_t st) {
@@ -630,20 +671,17 @@ int mb200_decode_step(const mb200_layer_desc* layers_dev, const int32_t* windows
                       void* workspace, size_t workspace_bytes, void* stream) {
   static_assert(sizeof(mb200_layer_desc) == sizeof(MkLayer), "layer descriptor layout");
   MB_CHECK_ARG(layers_dev && windows_dev && emb && final_norm && w_out && rope && token_dev && logits && workspace, "decode_step: null pointer");
-  MB_CHECK_ARG(head_dim == kHeadDim, "decode_step: head_dim=%lld unsupported (128 only)", (long long)head_dim);
-  MB_CHECK_ARG(n_heads % n_kv_heads == 0, "decode_step: H %% KV != 0");
-  const int rep = (int)(n_heads / n_kv_heads);
-  const int64_t q_dim = n_heads * head_dim;
-  auto cut_ok = [](int64_t K) { const int64_t nch = (K + MK_MAX_KC - 1) / MK_MAX_KC; return K % (nch * 8) == 0; };
-  MB_CHECK_ARG(n_kv_heads * kHeadDim * 2 + MK_KV_PAD <= MK_STAGE_BYTES / 8, "decode_step: a ring stage must hold 8 padded K/V position rows");
-  MB_CHECK_ARG(cut_ok(dim) && cut_ok(hidden) && cut_ok(q_dim), "decode_step: dim/hidden/q_dim must split into 16-byte-aligned row chunks");
-  MB_CHECK_ARG(vocab % 2 == 0 && hidden % 1 == 0, "decode_step: vocab must be even");
+  MB_CHECK_ARG(n_experts == 0 || (moe_gate_dev && moe_w13_dev && moe_w2_dev), "decode_step: MoE weight tables missing");
   int dev = 0, sms = 0, smem_max = 0, coop = 0;
   MB_CHECK_CUDA(cudaGetDevice(&dev));
   MB_CHECK_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   MB_CHECK_CUDA(cudaDeviceGetAttribute(&smem_max, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
   MB_CHECK_CUDA(cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev));
   MB_CHECK_ARG(coop, "decode_step: device does not support cooperative launch");
+  DecodePlan plan;
+  const int rc = decode_plan(dim, hidden, n_heads, n_kv_heads, head_dim, vocab, n_experts, top_k, smem_max, &plan);
+  if (rc) return rc;
+  const int rep = plan.rep;
 
   MkParams p;
   p.layers = reinterpret_cast<const MkLayer*>(layers_dev);
@@ -658,8 +696,6 @@ int mb200_decode_step(const mb200_layer_desc* layers_dev, const int32_t* windows
   p.batch_row = (int)batch_row;
   p.logits = logits;
   p.next_token = (long long*)next_token_dev;
-  MB_CHECK_ARG(n_experts == 0 || (moe_gate_dev && moe_w13_dev && moe_w2_dev && top_k >= 1 && top_k <= MK_MAX_TOPK && top_k <= n_experts && n_experts <= 32),
-               "decode_step: bad MoE arguments (E=%lld, k=%lld)", (long long)n_experts, (long long)top_k);
   p.n_experts = (int)n_experts;
   p.top_k = (int)(n_experts ? top_k : 0);
   p.moe_gate = (const bf16* const*)moe_gate_dev;
@@ -671,19 +707,8 @@ int mb200_decode_step(const mb200_layer_desc* layers_dev, const int32_t* windows
   p.KV = (int)n_kv_heads;
   p.vocab = (int)vocab;
   p.eps = eps;
-  // shared memory plan: x buffer (also the attention merge scratch), barriers + reduction scratch, the rest is the ring
-  int64_t widest = dim > hidden ? dim : hidden;
-  if (q_dim > widest) widest = q_dim;
-  size_t xs_bytes = (size_t)widest * 2;
-  if (n_experts && xs_bytes < (size_t)top_k * hidden * 2) xs_bytes = (size_t)top_k * hidden * 2;  // g of every selected expert
-  if (xs_bytes < 2048) xs_bytes = 2048;  // also the slice-merge scratch of phase 2b
-  xs_bytes = (xs_bytes + 127) & ~(size_t)127;
-  const size_t tail = 2 * MK_MAX_STAGES * sizeof(uint64_t) + 48 * sizeof(float) + sizeof(MoeRoute) + 8 + 64;
-  int n_stages = (int)(((size_t)smem_max - xs_bytes - tail) / MK_STAGE_BYTES);
-  if (n_stages > MK_MAX_STAGES) n_stages = MK_MAX_STAGES;
-  MB_CHECK_ARG(n_stages > MK_CONSUMER_WARPS, "decode_step: not enough shared memory for the weight ring (%d stages)", n_stages);
-  p.n_stages = n_stages;
-  p.xs_bytes = (int)xs_bytes;
+  p.n_stages = plan.n_stages;
+  p.xs_bytes = (int)plan.xs_bytes;
   {
     static int cap = -1;
     if (cap < 0) {
@@ -698,10 +723,7 @@ int mb200_decode_step(const mb200_layer_desc* layers_dev, const int32_t* windows
     }
     p.kv_uncapped = kvu;
   }
-  const size_t smem = (size_t)n_stages * MK_STAGE_BYTES + xs_bytes + tail;
-
-  MB_CHECK_ARG(n_kv_heads <= MK_CONSUMER_WARPS, "decode_step: n_kv_heads=%lld > %d (one consumer warp per kv head)", (long long)n_kv_heads,
-               MK_CONSUMER_WARPS);
+  const size_t smem = plan.smem;
   // global scratch: header words + activations + per-slice attention partials
   uint8_t* ws = (uint8_t*)workspace;
   p.attn_counters = (int*)(ws + 8192);
@@ -740,12 +762,39 @@ int mb200_decode_step(const mb200_layer_desc* layers_dev, const int32_t* windows
 int mb200_debug_decode_scratch(int64_t dim, int64_t hidden, int64_t n_heads, int64_t n_kv_heads, int64_t head_dim, int64_t n_experts,
                                int64_t top_k, size_t* q_offset, size_t* attn_offset) {
   MB_CHECK_ARG(q_offset && attn_offset, "debug_decode_scratch: null pointer");
+  size_t off[6];
+  const int rc = mb200_debug_decode_buffers(dim, hidden, n_heads, n_kv_heads, head_dim, n_experts, top_k, off);
+  if (rc) return rc;
+  *q_offset = off[2];
+  *attn_offset = off[3];
+  return MB200_OK;
+}
+
+int mb200_debug_decode_buffers(int64_t dim, int64_t hidden, int64_t n_heads, int64_t n_kv_heads, int64_t head_dim, int64_t n_experts,
+                               int64_t top_k, size_t* offsets) {
+  MB_CHECK_ARG(offsets, "debug_decode_buffers: null pointer");
   MB_CHECK_ARG(head_dim == kHeadDim && n_kv_heads > 0 && n_heads % n_kv_heads == 0 && dim > 0 && hidden > 0,
                "debug_decode_scratch: bad shape (H=%lld, KV=%lld, hd=%lld)", (long long)n_heads, (long long)n_kv_heads, (long long)head_dim);
   const DecodeScratch sc = decode_scratch(dim, hidden, n_heads, n_experts, top_k, 0);  // the SM count only sizes the last buffer
-  *q_offset = sc.qbuf;
-  *attn_offset = sc.abuf;
+  offsets[0] = sc.xbuf;
+  offsets[1] = sc.hbuf;
+  offsets[2] = sc.qbuf;
+  offsets[3] = sc.abuf;
+  offsets[4] = sc.gbuf;
+  offsets[5] = sc.partial;
   return MB200_OK;
+}
+
+int mb200_decode_step_supported(int64_t dim, int64_t hidden, int64_t n_heads, int64_t n_kv_heads, int64_t head_dim, int64_t vocab,
+                                int64_t n_experts, int64_t top_k, int64_t smem_optin) {
+  if (smem_optin <= 0) {
+    int dev = 0, smem_max = 0;
+    MB_CHECK_CUDA(cudaGetDevice(&dev));
+    MB_CHECK_CUDA(cudaDeviceGetAttribute(&smem_max, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
+    smem_optin = smem_max;
+  }
+  DecodePlan plan;
+  return decode_plan(dim, hidden, n_heads, n_kv_heads, head_dim, vocab, n_experts, top_k, smem_optin, &plan);
 }
 
 // Debug: device buffer of n_layers*12 uint64 that CTA 0 of the decode megakernel fills with %globaltimer stamps (NULL = off).

@@ -74,6 +74,7 @@ class Transformer(nn.Module):
         self.vocab_size = args.vocab_size
         self.n_layers = args.n_layers
         self._rope_table: Optional[torch.Tensor] = None
+        self._megakernel_refused: Optional[str] = None  # why the decode megakernel refuses this model's shapes ("" = it runs them)
         assert self.vocab_size > 0
         assert pipeline_rank < num_pipeline_ranks, (pipeline_rank, num_pipeline_ranks)
         self.pipeline_rank = pipeline_rank
@@ -305,10 +306,17 @@ class Transformer(nn.Module):
 
     def _megakernel_ok(self, B: int) -> bool:
         # the megakernel has no LoRA stage: with un-merged adapters batch 1 takes the per-layer graph path
-        return (B == 1 and self.num_pipeline_ranks == 1 and self.expert_parallel[1] == 1 and self.args.n_kv_heads <= 8
-                and self.args.lora is None
-                and os.environ.get("MB200_MEGAKERNEL", "1") != "0"
-                and (self.args.moe is None or (self.args.moe.num_experts <= 32 and self.args.moe.num_experts_per_tok <= 4)))
+        # the shape limits (head ratio, K chunking, KV <= 8, MoE sizes, a shared-memory ring of >= 9 stages next to the
+        # activations) are the library's, asked once per model: a model it refuses takes the per-layer path
+        if not (B == 1 and self.num_pipeline_ranks == 1 and self.expert_parallel[1] == 1 and self.args.lora is None
+                and os.environ.get("MB200_MEGAKERNEL", "1") != "0"):
+            return False
+        if self._megakernel_refused is None:
+            a, moe = self.args, self.args.moe
+            self._megakernel_refused = _abi.decode_step_unsupported(
+                a.dim, a.hidden_dim, a.n_heads, a.n_kv_heads, a.head_dim, self.vocab_size,
+                moe.num_experts if moe is not None else 0, moe.num_experts_per_tok if moe is not None else 0) or ""
+        return self._megakernel_refused == ""
 
     def _decode_state(self, cache: BufferCache, key: Any) -> Dict[str, Any]:
         """Per-(cache, kind) decode state (descriptor tables, static buffers, captured graph).  It lives ON THE CACHE OBJECT, so

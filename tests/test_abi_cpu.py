@@ -54,9 +54,13 @@ def test_launch_log_records_nothing_for_rejected_calls(built):
 
 
 @pytest.mark.parametrize("dim,hidden,H,KV,E,k", [(256, 256, 4, 2, 0, 0), (4096, 14336, 32, 8, 0, 0), (5120, 14336, 32, 8, 0, 0),
-                                                (6144, 16384, 48, 8, 8, 2), (256, 256, 40, 5, 0, 0)])
+                                                (6144, 16384, 48, 8, 8, 2), (256, 256, 40, 5, 0, 0), (4096, 14336, 32, 8, 8, 4),
+                                                (4112, 4112, 8, 1, 16, 4)])
 def test_decode_scratch_offsets(built, dim, hidden, H, KV, E, k):
-    """Where decode_step leaves q and the attention output: 256-byte aligned, after the header, apart, inside the workspace."""
+    """Where decode_step leaves q and the attention output: 256-byte aligned, after the header, apart, inside the workspace.
+    The same for every buffer mb200_debug_decode_buffers reports (both residual halves, h, q, the attention output, g of every
+    selected expert, the slice partials of up to 256 SMs): aligned, after the header, disjoint, inside the workspace, and q /
+    attention where mb200_debug_decode_scratch puts them."""
     q, a = _abi.decode_scratch(dim, hidden, H, KV, 128, E, k)
     nb = H * 128 * 2
     total = _abi.workspace_bytes(1, dim, H, KV, 128, hidden, 32000, 1)
@@ -65,6 +69,48 @@ def test_decode_scratch_offsets(built, dim, hidden, H, KV, E, k):
     assert q + nb <= a or a + nb <= q
     assert max(q, a) + nb <= total
     assert _abi.lib().mb200_debug_decode_scratch(dim, hidden, H, KV, 64, E, k, None, None) == -1
+
+    b = _abi.decode_buffers(dim, hidden, H, KV, 128, E, k)
+    assert (b.q, b.attn) == (q, a)
+    sizes = {"x": 2 * dim * 2, "h": dim * 2, "q": nb, "attn": nb, "g": (k if E else 1) * hidden * 2, "partial": 256 * H * 130 * 4}
+    spans = sorted((getattr(b, name), getattr(b, name) + n, name) for name, n in sizes.items())
+    for lo, hi, name in spans:
+        assert lo % 256 == 0, name
+        assert lo >= _abi.WORKSPACE_HEADER_BYTES, name
+        assert hi <= total, f"{name} ends at {hi} > workspace {total}"
+    for (_, hi, x), (lo, _, y) in zip(spans, spans[1:]):
+        assert hi <= lo, f"{x} overlaps {y}"
+    assert _abi.lib().mb200_debug_decode_buffers(dim, hidden, H, KV, 64, E, k, None) == -1
+    assert _abi.lib().mb200_debug_decode_buffers(dim, hidden, H, KV, 128, E, k, None) == -1
+
+
+H100_SMEM = 227 * 1024  # opt-in shared memory per block of an H100
+
+
+@pytest.mark.parametrize("name,shape,E,k,ok", [
+    ("mistral-7b", (4096, 14336, 32, 8, 32000), 0, 0, True),
+    ("nemo-12b", (5120, 14336, 32, 8, 131072), 0, 0, True),
+    ("mixtral-8x7b", (4096, 14336, 32, 8, 32000), 8, 2, True),
+    ("mixtral-8x7b-k3", (4096, 14336, 32, 8, 32000), 8, 3, False),
+    ("mixtral-8x7b-k4", (4096, 14336, 32, 8, 32000), 8, 4, False),
+    ("mixtral-8x22b", (6144, 16384, 48, 8, 32768), 8, 2, True),
+    ("mixtral-8x22b-k3", (6144, 16384, 48, 8, 32768), 8, 3, False),
+    ("k4-widest", (4096, 10272, 32, 8, 32000), 8, 4, True),
+    ("k4-one-step-wider", (4096, 10296, 32, 8, 32000), 8, 4, False),
+    ("k5", (4096, 4096, 32, 8, 32000), 8, 5, False),
+    ("kv16", (4096, 4096, 32, 16, 32000), 0, 0, False),
+    ("rep3", (4096, 4096, 24, 8, 32000), 0, 0, False),
+    ("odd-vocab", (4096, 4096, 32, 8, 32001), 0, 0, False),
+    ("hidden-4100", (4096, 4100, 32, 8, 32000), 0, 0, False),
+    ("hidden-4112", (4096, 4112, 32, 8, 32000), 0, 0, True),
+])
+def test_decode_step_supported_on_h100(built, name, shape, E, k, ok):
+    """The megakernel's shape rules at an H100's 227 KB of opt-in shared memory, without a GPU: the real dense and k = 2 MoE
+    shapes run; k = 3 on Mixtral-8x7B / 8x22B and k = 4 on Mixtral-8x7B leave fewer than 9 ring stages and are refused, like the
+    K chunking that is not 16-byte aligned (4100 = 2 x 2050), an odd vocab, KV > 8 and uncompiled head ratios."""
+    dim, hidden, H, KV, V = shape
+    why = _abi.decode_step_unsupported(dim, hidden, H, KV, 128, V, E, k, smem_optin=H100_SMEM)
+    assert (why is None) == ok, why
 
 
 def test_no_cpu_fallback():
