@@ -3,7 +3,6 @@
 #include <cstdlib>
 #include <cstring>
 
-#include "attn_decode.cuh"
 #include "attn_decode_tma.cuh"
 #include "attn_full_hd64.cuh"
 #include "attn_prefill.cuh"
@@ -18,6 +17,7 @@
 #include "sampling.cuh"
 #include "skinny_linear.cuh"
 #include "vision.cuh"
+#include "workspace.cuh"
 
 namespace mb200 {
 thread_local char g_err[512] = "";
@@ -28,28 +28,7 @@ thread_local char g_launch_log[kLaunchLogBytes] = "";
 static unsigned long long* g_mk_prof = nullptr;
 static unsigned long long* g_mk_prof_bar = nullptr;  // debug: decode megakernel phase timeline buffer (device)
 
-constexpr size_t kWsHeader = 64 * 1024;  // persistent, zero-initialised by the caller once: self-resetting counters
-inline size_t align256(size_t v) { return (v + 255) & ~(size_t)255; }
-
-// Global scratch of mb200_decode_step after the workspace header, as byte offsets: each buffer starts on a 256-byte boundary.
-// mb200_debug_decode_buffers (and mb200_debug_decode_scratch) report the offsets from the same function, so tests read what the kernel wrote.
-struct DecodeScratch {
-  size_t xbuf, hbuf, qbuf, abuf, gbuf, partial, end;
-};
-inline DecodeScratch decode_scratch(int64_t dim, int64_t hidden, int64_t n_heads, int64_t n_experts, int64_t top_k, int sms) {
-  const size_t q_dim = (size_t)n_heads * kHeadDim;
-  DecodeScratch s;
-  size_t off = kWsHeader;
-  auto take = [&](size_t bytes) { const size_t r = off; off += align256(bytes); return r; };
-  s.xbuf = take((size_t)2 * dim * 2);
-  s.hbuf = take((size_t)dim * 2);
-  s.qbuf = take(q_dim * 2);
-  s.abuf = take(q_dim * 2);
-  s.gbuf = take((size_t)(n_experts ? top_k : 1) * hidden * 2);
-  s.partial = take((size_t)sms * n_heads * (kHeadDim + 2) * sizeof(float));  // [slice = CTA][H][m, l, acc[128]]
-  s.end = off;
-  return s;
-}
+static_assert(MK_BAR_WORDS * 128 <= kWsMkBarFlags.bytes, "one grid-barrier counter per 128-byte line");
 
 // Every shape rule of mb200_decode_step and its shared-memory plan, for a device with `smem_max` bytes of opt-in shared memory
 // per block.  mb200_decode_step_supported exposes the same function, so a caller learns before launching whether the step runs.
@@ -116,9 +95,9 @@ static int run_linear(const void* x, const void* norm_w, const void* w, const Ep
   }
   const void* a = x;
   if (norm_w) {
-    const size_t need = kWsHeader + SK_PARTIAL_BYTES + align256((size_t)T * K * 2);
-    if (workspace == nullptr || workspace_bytes < need) return fail(MB200_E_WORKSPACE, "linear: workspace %zu < %zu", workspace_bytes, need);
-    void* normed = (uint8_t*)workspace + kWsHeader + SK_PARTIAL_BYTES;  // after the stream-K partial slots
+    const WsRegion nr = ws_normed(T, K);
+    if (workspace == nullptr || workspace_bytes < nr.end()) return fail(MB200_E_WORKSPACE, "linear: workspace %zu < %zu", workspace_bytes, nr.end());
+    void* normed = (uint8_t*)workspace + nr.offset;
     int rc = run_rmsnorm(x, norm_w, normed, T, K, eps, st);
     if (rc) return rc;
     a = normed;
@@ -130,7 +109,7 @@ static int run_linear(const void* x, const void* norm_w, const void* w, const Ep
   g.N = (int)N;
   g.K = (int)K;
   g.epi = epi;
-  if (streamk_eligible(T, N, K)) return launch_streamk<MODE>(g, workspace, workspace_bytes, kWsHeader, st);  // decode-sized batches: HBM-bound
+  if (streamk_eligible(T, N, K)) return launch_streamk<MODE>(g, workspace, workspace_bytes, st);  // decode-sized batches: HBM-bound
   if (wgmma_gemm_eligible(T, N, K)) return launch_gemm_wgmma<MODE>(g, st);
   return launch_gemm_mma<MODE>(g, st);
 }
@@ -162,9 +141,9 @@ static int run_linear_lora(const void* x, const void* norm_w, const void* w, Epi
     rc = norm_w ? launch_skinny<EPI_STORE, true>(p, (int)T, st) : launch_skinny<EPI_STORE, false>(p, (int)T, st);
   } else {
     if (norm_w) {
-      const size_t need = kWsHeader + SK_PARTIAL_BYTES + align256((size_t)T * K * 2);
-      if (workspace == nullptr || workspace_bytes < need) return fail(MB200_E_WORKSPACE, "linear: workspace %zu < %zu", workspace_bytes, need);
-      void* normed = (uint8_t*)workspace + kWsHeader + SK_PARTIAL_BYTES;  // where run_linear puts it
+      const WsRegion nr = ws_normed(T, K);
+      if (workspace == nullptr || workspace_bytes < nr.end()) return fail(MB200_E_WORKSPACE, "linear: workspace %zu < %zu", workspace_bytes, nr.end());
+      void* normed = (uint8_t*)workspace + nr.offset;
       rc = run_rmsnorm(x, norm_w, normed, T, K, eps, st);
       if (rc) return rc;
       xn = normed;
@@ -206,15 +185,11 @@ size_t mb200_workspace_bytes(int64_t T, int64_t dim, int64_t n_heads, int64_t n_
   (void)head_dim;
   const int64_t widest = dim > hidden ? dim : hidden;
   const int64_t rep = n_kv_heads > 0 ? n_heads / n_kv_heads : 1;
-  size_t s = kWsHeader;
-  s += SK_PARTIAL_BYTES;                                                  // stream-K partial accumulators (decode-sized GEMMs)
-  s += align256((size_t)T * widest * 2);                                  // normed activations
-  s += attn_decode_workspace(max_batch, n_kv_heads, 64, rep);             // split-KV partials (n_splits <= 64)
-  // decode_step scratch (residual ping-pong, h, q, attn, g) lives in the same region as the normed activations
-  const size_t mk = 6 * 256 + (size_t)(3 * dim + 2 * n_heads * head_dim + MK_MAX_TOPK * hidden) * 2 +
-                    (size_t)256 * n_heads * (kHeadDim + 2) * sizeof(float) + 256;  // up to 256 SMs worth of attention slices
-  if (s < kWsHeader + mk) s = kWsHeader + mk;
-  return s;
+  // stream-K partial slots + normed activations, then room for the split-KV partials (n_splits <= 64) on top
+  const size_t s = ws_normed(T, widest).end() + align256(ws_splitkv_partials(max_batch, n_kv_heads, 64, rep).bytes);
+  // decode_step scratch for any MoE top-k and up to 256 SMs worth of attention slices
+  const size_t mk = decode_scratch(dim, hidden, n_heads, 1, MK_MAX_TOPK, 256).end;
+  return s > mk ? s : mk;
 }
 
 int mb200_rmsnorm(const void* x, const void* w, void* out, int64_t T, int64_t dim, float eps, void* stream) {
@@ -299,7 +274,7 @@ int mb200_attn_decode(const void* q, const void* cache_k, const void* cache_v, c
   MB_CHECK_ARG(n_heads % n_kv_heads == 0, "attn_decode: H %% KV != 0");
   const int rep = (int)(n_heads / n_kv_heads);
   MB_CHECK_ARG(n_splits >= 1 && n_splits <= 64, "attn_decode: n_splits=%lld out of [1, 64]", (long long)n_splits);
-  MB_CHECK_ARG((size_t)B * n_kv_heads * sizeof(int) <= 8192, "attn_decode: B*KV too large for the counter block");
+  MB_CHECK_ARG((size_t)B * n_kv_heads * sizeof(int) <= kWsSplitKvCounters.bytes, "attn_decode: B*KV too large for the counter block");
   AttnDecodeParams p;
   p.q = (const bf16*)q;
   p.cache_k = (const bf16*)cache_k;
@@ -315,36 +290,20 @@ int mb200_attn_decode(const void* q, const void* cache_k, const void* cache_v, c
   p.partial = nullptr;
   p.counters = nullptr;
   if (n_splits > 1) {
-    const size_t need = kWsHeader + (size_t)B * n_kv_heads * n_splits * rep * (kHeadDim + 2) * sizeof(float);
-    if (workspace == nullptr || workspace_bytes < need) return fail(MB200_E_WORKSPACE, "attn_decode: workspace %zu < %zu", workspace_bytes, need);
-    p.counters = (int*)workspace;
-    p.partial = (float*)((uint8_t*)workspace + kWsHeader);
+    const WsRegion pr = ws_splitkv_partials(B, n_kv_heads, n_splits, rep);
+    if (workspace == nullptr || workspace_bytes < pr.end()) return fail(MB200_E_WORKSPACE, "attn_decode: workspace %zu < %zu", workspace_bytes, pr.end());
+    p.counters = (int*)((uint8_t*)workspace + kWsSplitKvCounters.offset);
+    p.partial = (float*)((uint8_t*)workspace + pr.offset);
   }
-  const dim3 grid((unsigned)n_splits, (unsigned)n_kv_heads, (unsigned)B);
   cudaStream_t st = (cudaStream_t)stream;
-  const char* which = getenv("MB200_ATTN_DECODE");  // "plain": the register-staged kernel of attn_decode.cuh (A/B comparisons)
-  if (!(which != nullptr && which[0] == 'p')) {
-    if (n_splits > 1) p.counters = (int*)workspace;
-    switch (rep) {
-      case 1: return launch_attn_decode_tma<1>(p, B * W, st);
-      case 2: return launch_attn_decode_tma<2>(p, B * W, st);
-      case 4: return launch_attn_decode_tma<4>(p, B * W, st);
-      case 6: return launch_attn_decode_tma<6>(p, B * W, st);
-      case 8: return launch_attn_decode_tma<8>(p, B * W, st);
-      default: return fail(MB200_E_INVALID, "attn_decode: H/KV=%d unsupported (1,2,4,6,8)", rep);
-    }
-  }
   switch (rep) {
-    case 1: attn_decode_kernel<1><<<grid, AD_THREADS, 0, st>>>(p); break;
-    case 2: attn_decode_kernel<2><<<grid, AD_THREADS, 0, st>>>(p); break;
-    case 4: attn_decode_kernel<4><<<grid, AD_THREADS, 0, st>>>(p); break;
-    case 6: attn_decode_kernel<6><<<grid, AD_THREADS, 0, st>>>(p); break;
-    case 8: attn_decode_kernel<8><<<grid, AD_THREADS, 0, st>>>(p); break;
+    case 1: return launch_attn_decode_tma<1>(p, B * W, st);
+    case 2: return launch_attn_decode_tma<2>(p, B * W, st);
+    case 4: return launch_attn_decode_tma<4>(p, B * W, st);
+    case 6: return launch_attn_decode_tma<6>(p, B * W, st);
+    case 8: return launch_attn_decode_tma<8>(p, B * W, st);
     default: return fail(MB200_E_INVALID, "attn_decode: H/KV=%d unsupported (1,2,4,6,8)", rep);
   }
-  note_launch("attn_decode_kernel<%d>", rep);
-  MB_CHECK_LAUNCH("attn_decode_kernel");
-  return MB200_OK;
 }
 
 int mb200_attn_prefill(const void* q, const void* k_new, const void* v_new, const void* cache_k, const void* cache_v, const int32_t* q_start,
@@ -591,7 +550,7 @@ int mb200_moe_grouped_ffn(const void* xs, const void* const* w13_host, const voi
   EpiParams e1;
   e1.out = g;
   e1.ld_out = hidden;
-  int rc = launch_grouped<EPI_SWIGLU>(xs, rows_cap, dim, 2 * hidden, w13_host, (int)n_experts, est, tile_rows, plan, e1, workspace, workspace_bytes, kWsHeader, st);
+  int rc = launch_grouped<EPI_SWIGLU>(xs, rows_cap, dim, 2 * hidden, w13_host, (int)n_experts, est, tile_rows, plan, e1, workspace, workspace_bytes, st);
   if (rc) return rc;
   EpiParams e2;
   e2.out = yw;
@@ -602,7 +561,7 @@ int mb200_moe_grouped_ffn(const void* xs, const void* const* w13_host, const voi
     MB_CHECK_ARG(comm->peer_yw[r] != nullptr, "moe_grouped_ffn: peer buffer %d missing", r);
     e2.peer_out[r] = comm->peer_yw[r];
   }
-  rc = launch_grouped<EPI_MOE_SCALE>(g, rows_cap, hidden, dim, w2_host, (int)n_experts, est, tile_rows, plan, e2, workspace, workspace_bytes, kWsHeader, st);
+  rc = launch_grouped<EPI_MOE_SCALE>(g, rows_cap, hidden, dim, w2_host, (int)n_experts, est, tile_rows, plan, e2, workspace, workspace_bytes, st);
   if (rc) return rc;
   MoeCombineParams c;
   c.yw = (const uint4*)yw;
@@ -709,29 +668,15 @@ int mb200_decode_step(const mb200_layer_desc* layers_dev, const int32_t* windows
   p.eps = eps;
   p.n_stages = plan.n_stages;
   p.xs_bytes = (int)plan.xs_bytes;
-  {
-    static int cap = -1;
-    if (cap < 0) {
-      const char* e = getenv("MB200_MK_INFLIGHT");
-      cap = e ? atoi(e) : 5;  // stages in flight per producer; MB200_MK_INFLIGHT=2..8 overrides
-    }
-    p.inflight_cap = cap < 2 ? 2 : (cap > 8 ? 8 : cap);
-    static int kvu = -1;
-    if (kvu < 0) {
-      const char* e2 = getenv("MB200_MK_KV_UNCAPPED");
-      kvu = e2 ? atoi(e2) : 0;
-    }
-    p.kv_uncapped = kvu;
-  }
   const size_t smem = plan.smem;
   // global scratch: header words + activations + per-slice attention partials
+  MB_CHECK_ARG((size_t)sms * sizeof(unsigned long long) <= kWsMkArgmaxSlots.bytes, "decode_step: %d SMs exceed the argmax slots", sms);
   uint8_t* ws = (uint8_t*)workspace;
-  p.attn_counters = (int*)(ws + 8192);
-  p.argmax_counter = (int*)(ws + 12288);
-  p.argmax_slots = (unsigned long long*)(ws + 32768);  // sms x 8 B
-  p.bar_flags = (unsigned*)(ws + 16384);
-  p.bar_epoch = (unsigned*)(ws + 20480);
-  p.done_counter = (int*)(ws + 20480 + 128);
+  p.argmax_counter = (int*)(ws + kWsMkArgmaxCounter.offset);
+  p.argmax_slots = (unsigned long long*)(ws + kWsMkArgmaxSlots.offset);
+  p.bar_flags = (unsigned*)(ws + kWsMkBarFlags.offset);
+  p.bar_epoch = (unsigned*)(ws + kWsMkBarEpoch.offset);
+  p.done_counter = (int*)(ws + kWsMkDoneCounter.offset);
   const DecodeScratch sc = decode_scratch(dim, hidden, n_heads, n_experts, top_k, sms);
   p.xbuf = (bf16*)(ws + sc.xbuf);
   p.hbuf = (bf16*)(ws + sc.hbuf);
@@ -797,7 +742,8 @@ int mb200_decode_step_supported(int64_t dim, int64_t hidden, int64_t n_heads, in
   return decode_plan(dim, hidden, n_heads, n_kv_heads, head_dim, vocab, n_experts, top_k, smem_optin, &plan);
 }
 
-// Debug: device buffer of n_layers*12 uint64 that CTA 0 of the decode megakernel fills with %globaltimer stamps (NULL = off).
+// Debug: device buffer of [8][n_layers][16] uint64 that 8 sampled CTAs of the decode megakernel fill with %globaltimer stamps
+// (NULL = off; see mk_stamp).
 int mb200_debug_set_decode_timeline(void* device_buffer) {
   g_mk_prof = (unsigned long long*)device_buffer;
   return MB200_OK;

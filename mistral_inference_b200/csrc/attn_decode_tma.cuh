@@ -1,24 +1,38 @@
 // GQA decode attention over the rotating KV cache for batched decode (B >= 2): TMA-staged K/V tiles, tensor-core scores.
 //
-// Roofline: HBM.  Algorithmic bytes per (sequence, layer) = 2 (K, V) * kv_len * KV * hd * 2 B.  The plain-load kernel
-// (attn_decode.cuh) keeps only what its registers can hold in flight (~28 KB per SM at batch 32: 37 % of the HBM rate measured on
+// Roofline: HBM.  Algorithmic bytes per (sequence, layer) = 2 (K, V) * kv_len * KV * hd * 2 B.  A kernel that loads K/V rows
+// into registers keeps only what its registers can hold in flight (~28 KB per SM at batch 32: 37 % of the HBM rate measured on
 // Nemo-12B shapes); here the bytes in flight are decoupled from the math: one producer thread per CTA streams [64 keys x 128 dims]
 // K and V tiles of one (sequence, kv head) into a 3-stage shared-memory ring with cp.async.bulk.tensor (two 128B-swizzled
 // [64 x 64] boxes per tile; the ring rows are 2 KB apart in the [max_batch * W, KV * hd] cache -- strided rows are the TMA
 // engine's job, not 256-byte requests from the SM), 96 KB in flight per CTA, two CTAs per SM.
-// CTA = (split s, kv head g, sequence b) like the plain kernel: ring slots [s*C, (s+1)*C) of that head, all H/KV query heads of
-// the group served from the same bytes (no repeat_kv, transformer_layers.py:84).  Four consumer warps take 16 keys each of every
-// tile:  S[16 x 16] = Q K^T with the REP query heads as MMA rows (mma.sync m16n8k16; the tiles are tiny and softmax lives in
-// the fragments), online softmax in fp32, P rounded to bf16, O[16 x 128] += P V.  Warps are merged through shared memory, splits
-// by the last CTA to arrive per (b, g) -- both exactly as in attn_decode.cuh.  Slots >= kv_len are uninitialised memory in the
-// reference (cache.py:166): their scores are masked by index and their V rows are zeroed in shared memory before the PV product.
+// CTA = (split s, kv head g, sequence b): it owns ring slots [s*C, (s+1)*C) of that head, C = ceil(kv_len / S), and serves all
+// H/KV query heads of the group from the same bytes (no repeat_kv, transformer_layers.py:84).  Softmax over the ring is
+// order-free (RoPE was applied with absolute positions before caching), so slots are consumed in slot order like the
+// reference's padded-keys mask (cache.py:250-254).  Four consumer warps take 16 keys each of every tile:  S[16 x 16] = Q K^T
+// with the REP query heads as MMA rows (mma.sync m16n8k16; the tiles are tiny and softmax lives in the fragments), online
+// softmax in fp32, P rounded to bf16, O[16 x 128] += P V.  Warps are merged through shared memory; with S > 1 each split
+// publishes its (m, l, acc) partial and the last CTA to arrive per (b, g) merges them.  Slots >= kv_len are uninitialised
+// memory in the reference (cache.py:166): their scores are masked by index and their V rows are zeroed in shared memory before
+// the PV product.
 #pragma once
-#include "attn_decode.cuh"
 #include "decode_megakernel.cuh"  // mbarrier helpers with the watchdog
 #include "gemm_mma.cuh"
 #include "gemm_wgmma.cuh"         // tma_load_2d, tensor-map encoder
 
 namespace mb200 {
+
+struct AttnDecodeParams {
+  const bf16* q;        // [B, H*hd]
+  const bf16* cache_k;  // [max_batch, W, KV, hd]
+  const bf16* cache_v;
+  const int32_t* kv_len;  // [B]
+  bf16* out;              // [B, H*hd]
+  float* partial;         // [B, KV, S, REP, hd + 2] (m, l, acc) when S > 1
+  int* counters;          // [B, KV] zero-initialised once; self-resetting
+  int B, W, H, KV, S;
+  float scale;
+};
 
 constexpr int ADT_KT = 64;                                 // keys per tile
 constexpr int ADT_STAGES = 3;

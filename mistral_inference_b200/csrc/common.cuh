@@ -62,6 +62,7 @@ inline void note_launch(const char* fmt, ...) {
 typedef __nv_bfloat16 bf16;
 
 constexpr int kHeadDim = 128;
+constexpr float kLog2e = 1.4426950408889634f;  // softmax runs in the exp2 domain
 
 // ---- bf16 <-> fp32 ---------------------------------------------------------------------------
 // A bf16 is the top half of an fp32: widening is a shift, exact.

@@ -24,7 +24,6 @@
 // is needed; every slice publishes (m, l, acc) per head and phase 2b merges the slices with all loads in flight at once.
 // Only the row of the token being decoded (written in phase 1 by other CTAs) is read from global memory after the barrier.
 #pragma once
-#include "attn_decode.cuh"
 #include "common.cuh"
 #include "gemm_mma.cuh"
 
@@ -32,20 +31,8 @@ namespace mb200 {
 
 constexpr int MK_CONSUMER_WARPS = 8;
 constexpr int MK_CONSUMERS = MK_CONSUMER_WARPS * 32;
-#ifndef MB200_MK_PRODUCERS
-#define MB200_MK_PRODUCERS 2
-#endif
-constexpr int MK_PRODUCER_WARPS = MB200_MK_PRODUCERS;  // one issuing thread each, stages dealt round-robin (a single thread is ~700 cycles per stage: the stage period)
-#ifndef MB200_MK_WG
-#define MB200_MK_WG 0
-#endif
-#if MB200_MK_WG
-// Experiment (round 2): producers in their own warpgroup so that setmaxnreg can move registers to the consumers (384 threads launch
-// with 168 registers; the pool a CTA can re-acquire is only what it released: (168 - 120) x 128 = (192 - 168) x 256).
-constexpr int MK_THREADS = MK_CONSUMERS + 128;
-#else
+constexpr int MK_PRODUCER_WARPS = 2;  // one issuing thread each, stages dealt round-robin (a single thread is ~700 cycles per stage: the stage period)
 constexpr int MK_THREADS = MK_CONSUMERS + 32 * MK_PRODUCER_WARPS;
-#endif
 constexpr int MK_WEIGHT_STAGE_BYTES = 16 * 1024;   // a weight stage: 2 rows x KC elements x 2 B
 constexpr int MK_MAX_KC = MK_WEIGHT_STAGE_BYTES / 4;  // elements per row chunk
 constexpr int MK_KV_PAD = 16;                      // K/V position rows are laid out with a 16-byte pad (ldmatrix bank spread)
@@ -87,13 +74,10 @@ struct MkParams {
   int dim, hidden, H, KV, vocab;
   float eps;
   int n_stages, xs_bytes;
-  int inflight_cap;  // max ring stages with outstanding bulk copies (< n_stages)
-  int kv_uncapped;
   // scratch (global)
   unsigned* bar_flags;  // grid barrier counter (monotonic, never reset)
   unsigned* bar_epoch;  // device word: number of barriers completed by previous launches (published by the last CTA to finish)
   int* done_counter;    // self-resetting: CTAs that have finished this launch
-  int* attn_counters;   // [KV]
   bf16* xbuf;           // [2][dim] residual stream ping-pong
   bf16* hbuf;           // [dim]
   bf16* qbuf;           // [H*hd]
@@ -101,7 +85,7 @@ struct MkParams {
   bf16* gbuf;           // [hidden]
   float* partial;       // [KV][splits][REP][hd+2]
   unsigned long long* prof_bar;  // optional [gridDim][n_layers][6][2] arrive/leave %globaltimer of every CTA at every barrier
-  unsigned long long* prof;  // optional [n_layers][12] globaltimer stamps written by CTA 0 (debug timeline), or null
+  unsigned long long* prof;  // optional [8][n_layers][16] globaltimer stamps of 8 sampled CTAs (debug timeline, see mk_stamp), or null
 };
 
 // debug timeline: 8 sampled CTAs (every 21st) record %globaltimer at each phase boundary: prof[sample][layer][16] (12..15: inside attention)
@@ -183,7 +167,7 @@ __device__ __forceinline__ unsigned ld_acquire_u32(const unsigned* p) {
 // x gridDim), so nothing has to be read or reset on the device.
 // (Measured alternatives on 148 CTAs: counter + generation word with fences 5 us; one flag per CTA polled by 148 threads of
 // every CTA 1.5 us when arrivals are spread out but 4-5 us when all CTAs arrive together -- 22 K simultaneous polls.)
-// Arrivals are spread over MK_BAR_WORDS counters on different 128-byte lines (CTA c -> word c % 8): when all CTAs arrive
+// Arrivals are spread over MK_BAR_WORDS counters on different 128-byte lines (bar_word_of below): when all CTAs arrive
 // within ~0.5 us (after the short wo / down phases) 148 same-address atomics serialise at one L2 slice (~3 us measured).
 constexpr int MK_BAR_WORDS = 8;
 __device__ __forceinline__ void st_release_u32(unsigned* p, unsigned v) {
@@ -193,14 +177,14 @@ __device__ __forceinline__ void red_add_release_u32(unsigned* p, unsigned v) {
   asm volatile("red.release.gpu.global.add.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
 }
 __device__ __forceinline__ void bar_stamp(const MkParams& p, int tid, int layer, int which, int leave) {
-  if (p.prof_bar != nullptr && tid == 0 && layer >= 0) {
+  if (p.prof_bar != nullptr && tid == 0) {
     unsigned long long t;
     asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t));
     p.prof_bar[(((int64_t)blockIdx.x * p.n_layers + layer) * 6 + which) * 2 + leave] = t;
   }
 }
-// Word j collects the arrivals of a CONTIGUOUS range of CTAs (c -> c * 8 / gridDim), which lets a phase whose input chunk was
-// produced by a known CTA range wait for just that range (see the down projection).
+// Word j collects the arrivals of a CONTIGUOUS range of CTAs (c -> c * 8 / gridDim).  Waiting for one range only, so that a
+// phase could start on the input chunks of the CTAs that have finished, was tried and dropped (see the down projection).
 __device__ __forceinline__ int bar_word_of(int cta) { return (cta * MK_BAR_WORDS) / (int)gridDim.x; }
 __device__ __forceinline__ unsigned bar_word_count(int j) {  // number of CTAs mapping to word j
   const int G = (int)gridDim.x;
@@ -208,15 +192,13 @@ __device__ __forceinline__ unsigned bar_word_count(int j) {  // number of CTAs m
   const int lo = (j * G + MK_BAR_WORDS - 1) / MK_BAR_WORDS, hi = ((j + 1) * G + MK_BAR_WORDS - 1) / MK_BAR_WORDS;
   return (unsigned)(hi - lo);
 }
-__device__ __forceinline__ void grid_arrive(const MkParams& p, int tid, unsigned& epoch, int layer = -1, int which = 0) {
+__device__ __forceinline__ void grid_barrier(const MkParams& p, int tid, unsigned& epoch, int layer, int which) {
   ++epoch;  // number of barriers completed once this one is
   bar_stamp(p, tid, layer, which, 0);
   consumer_sync();  // every consumer thread's global writes of this phase happen-before thread 0's release below
   if (tid == 0) red_add_release_u32(p.bar_flags + bar_word_of(blockIdx.x) * 32, 1u);
-}
-// wait until every CTA in words [w_lo, w_hi] has arrived at barrier number `epoch`
-__device__ __forceinline__ void grid_wait(const MkParams& p, int tid, unsigned epoch, int w_lo, int w_hi) {
-  if (tid >= w_lo && tid <= w_hi) {
+  // thread j < 8 waits until every CTA of word j has arrived at barrier number `epoch`
+  if (tid < MK_BAR_WORDS) {
     const unsigned target = epoch * bar_word_count(tid);
     unsigned spins = 0;
     while ((int)(ld_acquire_u32(p.bar_flags + tid * 32) - target) < 0) {
@@ -228,10 +210,6 @@ __device__ __forceinline__ void grid_wait(const MkParams& p, int tid, unsigned e
     }
   }
   consumer_sync();
-}
-__device__ __forceinline__ void grid_barrier(const MkParams& p, int tid, unsigned& epoch, int layer = -1, int which = 0) {
-  grid_arrive(p, tid, epoch, layer, which);
-  grid_wait(p, tid, epoch, 0, MK_BAR_WORDS - 1);
   bar_stamp(p, tid, layer, which, 1);
 }
 
@@ -297,6 +275,15 @@ __device__ __forceinline__ void bulk_g2s_hint(void* smem_dst, const void* gsrc, 
                : "memory");
 }
 
+// In-flight cap: stage `it` is only issued once stage it - cap has LANDED.  All n_stages slots still buffer data through the
+// phase boundaries, but the SM never has more than `cap` stages of read requests queued: right after a short phase the
+// consumers have drained the whole ring, and an uncapped producer then fires 12 x 16 KB at once -- the grid barrier's own
+// atomic / polls queue behind that burst in the SM's memory request path (measured: barrier latency 4 us after the wo
+// phase vs 1.5 us in steady state).  The bandwidth-delay product of one SM's HBM share is only ~3 stages.  The cap applies to
+// every stage, K/V slice stages included.
+constexpr int MK_INFLIGHT_CAP = 5;
+static_assert(MK_INFLIGHT_CAP <= MK_CONSUMER_WARPS, "below the smallest ring decode_plan accepts (n_stages > MK_CONSUMER_WARPS)");
+
 struct Producer {
   uint8_t* ring;
   uint64_t* full;
@@ -304,17 +291,9 @@ struct Producer {
   int n_stages;
   uint32_t it;
   uint64_t policy;  // L2 evict-first: weights and old K/V rows are read exactly once per token
-
-  // In-flight cap: stage `it` is only issued once stage it - cap has LANDED.  All n_stages slots still buffer data through the
-  // phase boundaries, but the SM never has more than `cap` stages of read requests queued: right after a short phase the
-  // consumers have drained the whole ring, and an uncapped producer then fires 12 x 16 KB at once -- the grid barrier's own
-  // atomic / polls queue behind that burst in the SM's memory request path (measured: barrier latency 4 us after the wo
-  // phase vs 1.5 us in steady state).  The bandwidth-delay product of one SM's HBM share is only ~3 stages.
-  int cap;
-  int me, n_prod;          // this producer issues the stages with it % n_prod == me
-  bool kv_uncapped;        // K/V slice stages ignore the in-flight cap (they are needed at once in phase 2a)
+  int me;                  // this producer issues the stages with it % MK_PRODUCER_WARPS == me
   uint32_t slot, par;      // ring slot / parity of stage `it`, kept incrementally (no division in the issue loop)
-  uint32_t cslot, cpar;    // same for stage it - cap
+  uint32_t cslot, cpar;    // same for stage it - MK_INFLIGHT_CAP
 
   __device__ __forceinline__ void advance() {
     ++it;
@@ -322,18 +301,18 @@ struct Producer {
       slot = 0;
       par ^= 1;
     }
-    if (it > (uint32_t)cap && ++cslot == (uint32_t)n_stages) {
+    if (it > (uint32_t)MK_INFLIGHT_CAP && ++cslot == (uint32_t)n_stages) {
       cslot = 0;
       cpar ^= 1;
     }
   }
   // returns the slot's buffer (and its full barrier, armed for `bytes`) or nullptr when the stage belongs to another producer
-  __device__ __forceinline__ uint8_t* acquire(uint32_t bytes, uint64_t*& bar, bool capped = true) {
-    if ((int)(it % (uint32_t)n_prod) != me) {
+  __device__ __forceinline__ uint8_t* acquire(uint32_t bytes, uint64_t*& bar) {
+    if ((int)(it % (uint32_t)MK_PRODUCER_WARPS) != me) {
       advance();
       return nullptr;
     }
-    if (capped && it >= (uint32_t)cap) mbar_wait(&full[cslot], cpar, 7, it);  // stage it - cap has landed (its slot cannot have been refilled yet)
+    if (it >= (uint32_t)MK_INFLIGHT_CAP) mbar_wait(&full[cslot], cpar, 7, it);  // stage it - cap has landed (its slot cannot have been refilled yet)
     mbar_wait(&empty[slot], par ^ 1, 1, it);
     bar = &full[slot];
     mbar_arrive_expect_tx(bar, bytes);
@@ -342,51 +321,40 @@ struct Producer {
     return dst;
   }
 
+  // one stage of a matrix slice: K-chunk `ch` of rows 2 * pair and 2 * pair + 1 of W [N, K]
+  __device__ __forceinline__ void pair_stage(const bf16* W, int K, const MatCut& c, int pair, int ch) {
+    const uint32_t row_bytes = (uint32_t)c.kc * 2;
+    const bf16* r0 = W + (int64_t)(2 * pair) * K;
+    uint64_t* bar;
+    uint8_t* dst = acquire(2 * row_bytes, bar);
+    if (dst == nullptr) return;
+    if (c.nch == 1) {
+      bulk_g2s_hint(dst, r0, 2 * row_bytes, bar, policy);  // the two rows are contiguous
+    } else {
+      bulk_g2s_hint(dst, r0 + ch * c.kc, row_bytes, bar, policy);
+      bulk_g2s_hint(dst + row_bytes, r0 + K + ch * c.kc, row_bytes, bar, policy);
+    }
+  }
+
   // this CTA's slice of one [N, K] weight matrix, in the stage order consume_matrix expects
   __device__ __forceinline__ void matrix(const bf16* W, int N, int K) {
     const MatCut c = cut_matrix(N, K);
-    const uint32_t row_bytes = (uint32_t)c.kc * 2;
     for (int g0 = c.p0; g0 < c.p1; g0 += MK_CONSUMER_WARPS) {
       const int g = min(MK_CONSUMER_WARPS, c.p1 - g0);
-      for (int ch = 0; ch < c.nch; ++ch) {
-        for (int w = 0; w < g; ++w) {
-          const bf16* r0 = W + (int64_t)(2 * (g0 + w)) * K;
-          uint64_t* bar;
-          uint8_t* dst = acquire(2 * row_bytes, bar);
-          if (dst == nullptr) continue;
-          if (c.nch == 1) {
-            bulk_g2s_hint(dst, r0, 2 * row_bytes, bar, policy);  // the two rows are contiguous
-          } else {
-            bulk_g2s_hint(dst, r0 + ch * c.kc, row_bytes, bar, policy);
-            bulk_g2s_hint(dst + row_bytes, r0 + K + ch * c.kc, row_bytes, bar, policy);
-          }
-        }
-      }
+      for (int ch = 0; ch < c.nch; ++ch)
+        for (int w = 0; w < g; ++w) pair_stage(W, K, c, g0 + w, ch);
     }
   }
 
   // expert down projections of one MoE layer: per group of 8 pairs expert-major, chunk-major (see consume_moe_down)
   __device__ __forceinline__ void moe_down(const bf16* const* w2, const int* sel, int top_k, int N, int K) {
     const MatCut c = cut_matrix(N, K);
-    const uint32_t row_bytes = (uint32_t)c.kc * 2;
     for (int g0 = c.p0; g0 < c.p1; g0 += MK_CONSUMER_WARPS) {
       const int g = min(MK_CONSUMER_WARPS, c.p1 - g0);
       for (int j = 0; j < top_k; ++j) {
         const bf16* W = w2[sel[j]];
-        for (int ch = 0; ch < c.nch; ++ch) {
-          for (int w = 0; w < g; ++w) {
-            const bf16* r0 = W + (int64_t)(2 * (g0 + w)) * K;
-            uint64_t* bar;
-            uint8_t* dst = acquire(2 * row_bytes, bar);
-            if (dst == nullptr) continue;
-            if (c.nch == 1) {
-              bulk_g2s_hint(dst, r0, 2 * row_bytes, bar, policy);
-            } else {
-              bulk_g2s_hint(dst, r0 + ch * c.kc, row_bytes, bar, policy);
-              bulk_g2s_hint(dst + row_bytes, r0 + K + ch * c.kc, row_bytes, bar, policy);
-            }
-          }
-        }
+        for (int ch = 0; ch < c.nch; ++ch)
+          for (int w = 0; w < g; ++w) pair_stage(W, K, c, g0 + w, ch);
       }
     }
   }
@@ -405,7 +373,7 @@ struct Producer {
 #pragma unroll
       for (int kv = 0; kv < 2; ++kv) {
         uint64_t* bar;
-        uint8_t* dst = acquire((uint32_t)rows * row_bytes, bar, !kv_uncapped);
+        uint8_t* dst = acquire((uint32_t)rows * row_bytes, bar);
         if (dst == nullptr) continue;
         const bf16* src = (kv ? vbase : kbase) + (int64_t)k0 * row_elems;
         for (int r = 0; r < rows; ++r) bulk_g2s_hint(dst + r * (row_bytes + MK_KV_PAD), src + (int64_t)r * row_elems, row_bytes, bar, policy);
@@ -422,10 +390,7 @@ __device__ __forceinline__ void producer_main(const MkParams& p, uint8_t* ring, 
   pr.empty = empty;
   pr.n_stages = p.n_stages;
   pr.it = 0;
-  pr.cap = p.inflight_cap;
   pr.me = me;
-  pr.n_prod = MK_PRODUCER_WARPS;
-  pr.kv_uncapped = p.kv_uncapped != 0;
   pr.slot = pr.par = pr.cslot = pr.cpar = 0;
   asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pr.policy));
   const int q_dim = p.H * kHeadDim, kv_dim = p.KV * kHeadDim;
@@ -450,58 +415,58 @@ __device__ __forceinline__ void producer_main(const MkParams& p, uint8_t* ring, 
   pr.matrix(p.w_out, p.vocab, p.dim);
 }
 
+// ---- consumers: one weight stage of a pair -----------------------------------------------------------------------------
+// Waits for ring stage `it`, adds this lane's share of (row 0 . xc) to a0 and of (row 1 . xc) to a1 (kc8 16-byte chunks per row,
+// 32 lanes x 16 B per step, unrolled -> plenty of ILP) and releases the slot: the calling warp is its only reader (empty
+// barriers count MK_CONSUMER_WARPS arrivals, all from that warp).
+__device__ __forceinline__ void consume_pair_stage(const uint8_t* ring, uint64_t* full, uint64_t* empty, int n_stages, uint32_t it,
+                                                   const uint4* xc, int kc8, int lane, float& a0, float& a1) {
+  const uint32_t slot = it % n_stages, par = (it / n_stages) & 1;
+  // Guard (tests/test_megakernel_protocol.py): bulk copies land out of order, so this warp may get here before the
+  // slot's PREVIOUS fill (owned by another warp) has landed; `full` would then still be one phase behind and a
+  // parity wait would alias and pass early.  Waiting first until that previous fill has been CONSUMED (same
+  // condition the producer waits for before refilling) pins `full` to phase {r, r+1} when it is tested.
+  mbar_wait(&empty[slot], par ^ 1, 2, it);
+  mbar_wait(&full[slot], par, 3, it);
+  const uint4* w0 = reinterpret_cast<const uint4*>(ring + (size_t)slot * MK_STAGE_BYTES);
+  const uint4* w1 = w0 + kc8;
+#pragma unroll 4
+  for (int i = lane; i < kc8; i += 32) {
+    const uint4 a = w0[i], b = w1[i], x = xc[i];
+    const uint32_t aw[4] = {a.x, a.y, a.z, a.w}, bw[4] = {b.x, b.y, b.z, b.w}, xw[4] = {x.x, x.y, x.z, x.w};
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const float xl = bf16lo(xw[j]), xh = bf16hi(xw[j]);
+      a0 = fmaf(bf16lo(aw[j]), xl, a0);
+      a0 = fmaf(bf16hi(aw[j]), xh, a0);
+      a1 = fmaf(bf16lo(bw[j]), xl, a1);
+      a1 = fmaf(bf16hi(bw[j]), xh, a1);
+    }
+  }
+  __syncwarp();
+  if (lane == 0) mbar_arrive_n(&empty[slot], MK_CONSUMER_WARPS);
+}
+
 // ---- consumers: y[pair] = W[pair rows] . xs, epilogue(pair, acc0, acc1) on one lane ----------------
-// Warp-per-pair inside a group: warp w owns pair g0+w and consumes its `nch` stages by itself (32 lanes x 16 B per step,
-// unrolled -> plenty of ILP); only the owning warp releases a slot (empty barriers have arrival count 1).  One block
-// barrier per GROUP keeps all warps within a group of each other (see the stage-order note above).
+// Warp-per-pair inside a group: warp w owns pair g0+w and consumes its `nch` stages by itself.  One block barrier per GROUP
+// keeps all warps within a group of each other (see the stage-order note above).
 // `pre(n)` runs on the finishing lane BEFORE the pair's stages are consumed and its result is handed to `epi`: loads the
 // epilogue needs (the residual) are then off the critical path of the phase's last pair (an L2 round trip right before the
 // barrier's release store: measured 3.2-4.2 us barrier latency after wo / down vs 1.75 us after gate/up, which loads nothing).
-// `ready(ch)` is called by ALL consumer threads before K-chunk `ch` of the FIRST group is touched: a phase can then stage its
-// input chunk by chunk as the CTAs that produce it finish (pass a no-op when the input was staged up front).
-template <class Ready, class Pre, class Epi>
+template <class Pre, class Epi>
 __device__ __forceinline__ void consume_matrix(int N, int K, const uint8_t* ring, uint64_t* full, uint64_t* empty, int n_stages, RingState& rs,
-                                               const uint4* xs, int tid, Ready ready, Pre pre, Epi epi) {
+                                               const uint4* xs, int tid, Pre pre, Epi epi) {
   const MatCut c = cut_matrix(N, K);
   const int lane = tid & 31, warp = tid >> 5;
   const int kc8 = c.kc >> 3;  // 16-byte chunks per row chunk
   for (int g0 = c.p0; g0 < c.p1; g0 += MK_CONSUMER_WARPS) {
     const int g = min(MK_CONSUMER_WARPS, c.p1 - g0);
-    float a0 = 0.f, a1 = 0.f;
-    uint2 prefetched = make_uint2(0u, 0u);
-    if (warp < g && lane == 0) prefetched = pre(2 * (g0 + warp));
-    for (int ch = 0; ch < c.nch; ++ch) {
-      if (g0 == c.p0) ready(ch);
-      if (warp < g) {
-        const uint32_t it = rs.it + (uint32_t)(ch * g + warp);
-        const uint32_t slot = it % n_stages, par = (it / n_stages) & 1;
-        // Guard (tests/test_megakernel_protocol.py): bulk copies land out of order, so this warp may get here before the
-        // slot's PREVIOUS fill (owned by another warp) has landed; `full` would then still be one phase behind and a
-        // parity wait would alias and pass early.  Waiting first until that previous fill has been CONSUMED (same
-        // condition the producer waits for before refilling) pins `full` to phase {r, r+1} when it is tested.
-        mbar_wait(&empty[slot], par ^ 1, 2, it);
-        mbar_wait(&full[slot], par, 3, it);
-        const uint4* w0 = reinterpret_cast<const uint4*>(ring + (size_t)slot * MK_STAGE_BYTES);
-        const uint4* w1 = w0 + kc8;
-        const uint4* xc = xs + ch * kc8;
-#pragma unroll 4
-        for (int i = lane; i < kc8; i += 32) {
-          const uint4 a = w0[i], b = w1[i], x = xc[i];
-          const uint32_t aw[4] = {a.x, a.y, a.z, a.w}, bw[4] = {b.x, b.y, b.z, b.w}, xw[4] = {x.x, x.y, x.z, x.w};
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            const float xl = bf16lo(xw[j]), xh = bf16hi(xw[j]);
-            a0 = fmaf(bf16lo(aw[j]), xl, a0);
-            a0 = fmaf(bf16hi(aw[j]), xh, a0);
-            a1 = fmaf(bf16lo(bw[j]), xl, a1);
-            a1 = fmaf(bf16hi(bw[j]), xh, a1);
-          }
-        }
-        __syncwarp();
-        if (lane == 0) mbar_arrive_n(&empty[slot], MK_CONSUMER_WARPS);  // this warp is the only reader of the slot
-      }
-    }
     if (warp < g) {
+      uint2 prefetched = make_uint2(0u, 0u);
+      if (lane == 0) prefetched = pre(2 * (g0 + warp));
+      float a0 = 0.f, a1 = 0.f;
+      for (int ch = 0; ch < c.nch; ++ch)
+        consume_pair_stage(ring, full, empty, n_stages, rs.it + (uint32_t)(ch * g + warp), xs + ch * kc8, kc8, lane, a0, a1);
       a0 = warp_sum(a0);
       a1 = warp_sum(a1);
       if (lane == 0) epi(2 * (g0 + warp), a0, a1, prefetched);
@@ -848,30 +813,9 @@ __device__ __forceinline__ void consume_moe_down(const MkParams& p, const MoeRou
       float r0 = 0.f, r1 = 0.f;
       for (int j = 0; j < p.top_k; ++j) {
         float a0 = 0.f, a1 = 0.f;
-        for (int ch = 0; ch < c.nch; ++ch) {
-          const uint32_t it = rs.it + (uint32_t)((j * c.nch + ch) * g + warp);
-          const uint32_t slot = it % n_stages, par = (it / n_stages) & 1;
-          mbar_wait(&empty[slot], par ^ 1, 2, it);
-          mbar_wait(&full[slot], par, 3, it);
-          const uint4* w0 = reinterpret_cast<const uint4*>(ring + (size_t)slot * MK_STAGE_BYTES);
-          const uint4* w1 = w0 + kc8;
-          const uint4* xc = xs + j * hid8 + ch * kc8;
-#pragma unroll 4
-          for (int i = lane; i < kc8; i += 32) {
-            const uint4 a = w0[i], b = w1[i], x = xc[i];
-            const uint32_t aw[4] = {a.x, a.y, a.z, a.w}, bw[4] = {b.x, b.y, b.z, b.w}, xw[4] = {x.x, x.y, x.z, x.w};
-#pragma unroll
-            for (int q = 0; q < 4; ++q) {
-              const float xl = bf16lo(xw[q]), xh = bf16hi(xw[q]);
-              a0 = fmaf(bf16lo(aw[q]), xl, a0);
-              a0 = fmaf(bf16hi(aw[q]), xh, a0);
-              a1 = fmaf(bf16lo(bw[q]), xl, a1);
-              a1 = fmaf(bf16hi(bw[q]), xh, a1);
-            }
-          }
-          __syncwarp();
-          if (lane == 0) mbar_arrive_n(&empty[slot], MK_CONSUMER_WARPS);
-        }
+        for (int ch = 0; ch < c.nch; ++ch)
+          consume_pair_stage(ring, full, empty, n_stages, rs.it + (uint32_t)((j * c.nch + ch) * g + warp), xs + j * hid8 + ch * kc8, kc8,
+                             lane, a0, a1);
         a0 = warp_sum(a0);
         a1 = warp_sum(a1);
         const float t0 = round_bf16(rt.w[j] * round_bf16(a0)), t1 = round_bf16(rt.w[j] * round_bf16(a1));
@@ -914,24 +858,14 @@ __global__ void __launch_bounds__(MK_THREADS, 1) decode_megakernel(const MkParam
 
   if (tid >= MK_CONSUMERS) {
     // ================= producers (one thread per producer warp; weights and old K/V rows never wait for activations) =================
-#if MB200_MK_WG
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 120;");
-    if ((tid & 31) == 0 && ((tid - MK_CONSUMERS) >> 5) < MK_PRODUCER_WARPS)
-#else
-    if ((tid & 31) == 0)
-#endif
-      producer_main(p, ring, full, empty, (tid - MK_CONSUMERS) >> 5, route, route_bar);
+    if ((tid & 31) == 0) producer_main(p, ring, full, empty, (tid - MK_CONSUMERS) >> 5, route, route_bar);
     return;
   }
-#if MB200_MK_WG
-  asm volatile("setmaxnreg.inc.sync.aligned.u32 192;");
-#endif
 
   // ================= consumer warps =================
   // barriers completed by previous launches on this workspace.  Nobody writes the word until every CTA of this launch has
   // finished (see the end of the kernel), and launches are stream ordered, so this read cannot race.
   unsigned epoch = ld_acquire_u32(p.bar_epoch);
-  const unsigned epoch0 = epoch;
   const int64_t token = *p.token;
   for (int l = 0; l < p.n_layers; ++l) {
     const MkLayer L = p.layers[l];
@@ -948,7 +882,7 @@ __global__ void __launch_bounds__(MK_THREADS, 1) decode_megakernel(const MkParam
       const float* rope_row = p.rope + (int64_t)p.pos * (kHeadDim / 2) * 2;
       bf16* ck = L.cache_k + (int64_t)slot_row * kv_dim;
       bf16* cv = L.cache_v + (int64_t)slot_row * kv_dim;
-      consume_matrix(q_dim + 2 * kv_dim, p.dim, ring, full, empty, p.n_stages, rs, xs, tid, [&](int) {},
+      consume_matrix(q_dim + 2 * kv_dim, p.dim, ring, full, empty, p.n_stages, rs, xs, tid,
                      [&](int n) { return *reinterpret_cast<const uint2*>(rope_row + ((n & (kHeadDim - 1)) >> 1) * 2); },
                      [&](int n, float a0, float a1, uint2 pf) {
         const float y0 = round_bf16(a0), y1 = round_bf16(a1);
@@ -985,7 +919,7 @@ __global__ void __launch_bounds__(MK_THREADS, 1) decode_megakernel(const MkParam
 
     // ---- phase 3: wo + residual ----
     stage_x(xs, p.abuf, nullptr, q_dim, 0.f, red, tid);
-    consume_matrix(p.dim, q_dim, ring, full, empty, p.n_stages, rs, xs, tid, [&](int) {}, [&](int n) { return make_uint2(ldcg_u32(x_in + n), 0u); }, [&](int n, float a0, float a1, uint2 pf) {
+    consume_matrix(p.dim, q_dim, ring, full, empty, p.n_stages, rs, xs, tid, [&](int n) { return make_uint2(ldcg_u32(x_in + n), 0u); }, [&](int n, float a0, float a1, uint2 pf) {
       const uint32_t r = pf.x;
       *reinterpret_cast<uint32_t*>(p.hbuf + n) = pack_bf16x2(round_bf16(a0) + bf16lo(r), round_bf16(a1) + bf16hi(r));
     });
@@ -996,7 +930,7 @@ __global__ void __launch_bounds__(MK_THREADS, 1) decode_megakernel(const MkParam
     if (p.n_experts == 0) {
     // ---- phase 4: RMSNorm + gate/up + SiLU*mul ----
       stage_x(xs, p.hbuf, L.ffn_norm, p.dim, p.eps, red, tid);
-      consume_matrix(2 * p.hidden, p.dim, ring, full, empty, p.n_stages, rs, xs, tid, [&](int) {}, [&](int) { return make_uint2(0u, 0u); }, [&](int n, float a0, float a1, uint2) {
+      consume_matrix(2 * p.hidden, p.dim, ring, full, empty, p.n_stages, rs, xs, tid, [&](int) { return make_uint2(0u, 0u); }, [&](int n, float a0, float a1, uint2) {
         const float s = round_bf16(ref_silu(round_bf16(a0)));
         p.gbuf[n >> 1] = __float2bfloat16_rn(s * round_bf16(a1));
       });
@@ -1006,10 +940,10 @@ __global__ void __launch_bounds__(MK_THREADS, 1) decode_megakernel(const MkParam
 
       // ---- phase 5: down + residual ----
       // (Tried: no full barrier here -- stage g chunk by chunk as the barrier words of the CTA range that produced each K-chunk
-      //  complete, via grid_arrive / grid_wait + the `ready` hook.  Correct, but 4 polling rounds + 4 block syncs cost more than
-      //  the ~5 us gate/up arrival skew they hide: 345 vs 351 tok/s.)
+      //  complete, waiting on those words only.  Correct, but 4 polling rounds + 4 block syncs cost more than the ~5 us gate/up
+      //  arrival skew they hide: 345 vs 351 tok/s.)
       stage_x(xs, p.gbuf, nullptr, p.hidden, 0.f, red, tid);
-      consume_matrix(p.dim, p.hidden, ring, full, empty, p.n_stages, rs, xs, tid, [&](int) {}, [&](int n) { return make_uint2(ldcg_u32(p.hbuf + n), 0u); },
+      consume_matrix(p.dim, p.hidden, ring, full, empty, p.n_stages, rs, xs, tid, [&](int n) { return make_uint2(ldcg_u32(p.hbuf + n), 0u); },
                      [&](int n, float a0, float a1, uint2 pf) {
                        const uint32_t r = pf.x;
                        *reinterpret_cast<uint32_t*>(x_out + n) = pack_bf16x2(round_bf16(a0) + bf16lo(r), round_bf16(a1) + bf16hi(r));
@@ -1021,7 +955,7 @@ __global__ void __launch_bounds__(MK_THREADS, 1) decode_megakernel(const MkParam
       const MoeRoute rt = *route;
       for (int j = 0; j < p.top_k; ++j) {
         bf16* gj = p.gbuf + (size_t)j * p.hidden;
-        consume_matrix(2 * p.hidden, p.dim, ring, full, empty, p.n_stages, rs, xs, tid, [&](int) {}, [&](int) { return make_uint2(0u, 0u); },
+        consume_matrix(2 * p.hidden, p.dim, ring, full, empty, p.n_stages, rs, xs, tid, [&](int) { return make_uint2(0u, 0u); },
                        [&](int n, float a0, float a1, uint2) {
                          const float sv = round_bf16(ref_silu(round_bf16(a0)));
                          gj[n >> 1] = __float2bfloat16_rn(sv * round_bf16(a1));
@@ -1052,7 +986,7 @@ __global__ void __launch_bounds__(MK_THREADS, 1) decode_megakernel(const MkParam
     u = (u & 0x80000000u) ? ~u : (u | 0x80000000u);
     return ((unsigned long long)u << 32) | (unsigned)(0x7fffffff - idx);
   };
-  consume_matrix(p.vocab, p.dim, ring, full, empty, p.n_stages, rs, xs, tid, [&](int) {}, [&](int) { return make_uint2(0u, 0u); },
+  consume_matrix(p.vocab, p.dim, ring, full, empty, p.n_stages, rs, xs, tid, [&](int) { return make_uint2(0u, 0u); },
                  [&](int n, float a0, float a1, uint2) {
                    const float y0 = round_bf16(a0), y1 = round_bf16(a1);
                    *reinterpret_cast<float2*>(p.logits + n) = make_float2(y0, y1);
@@ -1091,7 +1025,6 @@ __global__ void __launch_bounds__(MK_THREADS, 1) decode_megakernel(const MkParam
       st_release_u32(p.bar_epoch, epoch);
     }
   }
-  (void)epoch0;
 }
 
 }  // namespace mb200

@@ -23,13 +23,12 @@
 // tiles (expert segments of <= TA rows) come from the device-side plan of csrc/moe.cuh, each with its own weight tensor map.
 #pragma once
 #include "gemm_wgmma.cuh"
+#include "workspace.cuh"
 
 namespace mb200 {
 
 constexpr int SK_BN = 128;
-constexpr int SK_MAX_CTAS = 160;
-constexpr size_t SK_PARTIAL_BYTES = (size_t)SK_MAX_CTAS * 128 * SK_BN * sizeof(float);  // one [128 x 128] fp32 slot per CTA
-constexpr size_t SK_FLAGS_OFFSET = 24576;  // inside the zero-initialised workspace header: uint32 flags[SK_MAX_CTAS]
+static_assert(SK_PARTIAL_BYTES == (size_t)SK_MAX_CTAS * 128 * SK_BN * sizeof(float), "one [128 x SK_BN] fp32 slot per CTA");
 
 // -DMB200_SK_TRACE: every CTA of the dense kernel stamps %globaltimer / %clock64 at eight points of its life into a device ring
 // (scripts/trace_streamk.py reads it through mb200_debug_sk_trace) -- how the microseconds between dependent launches are spent.
@@ -244,15 +243,15 @@ inline bool streamk_eligible(int64_t T, int64_t N, int64_t K) {
   return T >= 1 && T <= 128 && N % SK_BN == 0 && K % TG_BK == 0;
 }
 
-// workspace: partial slots at `ws + header`, flags in the header (both overlap scratch of other, stream-ordered entry points)
+// workspace: partial slots and flags where workspace.cuh puts them (both overlap scratch of other, stream-ordered entry points)
 template <int MODE, int TA>
-int launch_streamk_ta(const GemmParams& g, void* workspace, size_t workspace_bytes, size_t header, cudaStream_t stream) {
+int launch_streamk_ta(const GemmParams& g, void* workspace, size_t workspace_bytes, cudaStream_t stream) {
   using Cfg = TgCfg<SK_BN, TA>;
   int dev = 0, sms = 0;
   MB_CHECK_CUDA(cudaGetDevice(&dev));
   MB_CHECK_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   if (sms > SK_MAX_CTAS) sms = SK_MAX_CTAS;
-  if (workspace == nullptr || workspace_bytes < header + SK_PARTIAL_BYTES) return fail(MB200_E_WORKSPACE, "stream-K gemm: workspace %zu < %zu", workspace_bytes, header + SK_PARTIAL_BYTES);
+  if (workspace == nullptr || workspace_bytes < kWsSkPartials.end()) return fail(MB200_E_WORKSPACE, "stream-K gemm: workspace %zu < %zu", workspace_bytes, kWsSkPartials.end());
   CUtensorMap map_a, map_w;
   int rc = make_tensor_map_2d(&map_a, g.a, g.T, g.K, TA);
   if (rc) return rc;
@@ -263,8 +262,8 @@ int launch_streamk_ta(const GemmParams& g, void* workspace, size_t workspace_byt
   p.N = g.N;
   p.K = g.K;
   p.epi = g.epi;
-  p.partials = reinterpret_cast<float*>((uint8_t*)workspace + header);
-  p.flags = reinterpret_cast<unsigned*>((uint8_t*)workspace + SK_FLAGS_OFFSET);
+  p.partials = reinterpret_cast<float*>((uint8_t*)workspace + kWsSkPartials.offset);
+  p.flags = reinterpret_cast<unsigned*>((uint8_t*)workspace + kWsSkFlags.offset);
   const long long units = (long long)(g.N / SK_BN) * (g.K / TG_BK);
   const int grid = (int)(units < sms ? units : sms);
   MB_CHECK_CUDA(cudaFuncSetAttribute(gemm_streamk_kernel<MODE, TA>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmem));
@@ -274,10 +273,10 @@ int launch_streamk_ta(const GemmParams& g, void* workspace, size_t workspace_byt
 }
 
 template <int MODE>
-int launch_streamk(const GemmParams& g, void* workspace, size_t workspace_bytes, size_t header, cudaStream_t stream) {
-  if (g.T <= 32) return launch_streamk_ta<MODE, 32>(g, workspace, workspace_bytes, header, stream);
-  if (g.T <= 64) return launch_streamk_ta<MODE, 64>(g, workspace, workspace_bytes, header, stream);
-  return launch_streamk_ta<MODE, 128>(g, workspace, workspace_bytes, header, stream);
+int launch_streamk(const GemmParams& g, void* workspace, size_t workspace_bytes, cudaStream_t stream) {
+  if (g.T <= 32) return launch_streamk_ta<MODE, 32>(g, workspace, workspace_bytes, stream);
+  if (g.T <= 64) return launch_streamk_ta<MODE, 64>(g, workspace, workspace_bytes, stream);
+  return launch_streamk_ta<MODE, 128>(g, workspace, workspace_bytes, stream);
 }
 
 }  // namespace mb200

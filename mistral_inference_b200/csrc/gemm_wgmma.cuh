@@ -316,14 +316,8 @@ inline int make_tensor_map_2d(CUtensorMap* map, const void* base, int64_t rows, 
   return MB200_OK;
 }
 
-// MB200_GEMM=mma forces the mma.sync kernel (A/B comparisons, debugging)
 inline bool wgmma_gemm_eligible(int64_t T, int64_t N, int64_t K) {
-  static int forced_mma = -1;
-  if (forced_mma < 0) {
-    const char* e = getenv("MB200_GEMM");
-    forced_mma = (e != nullptr && e[0] == 'm') ? 1 : 0;
-  }
-  if (forced_mma || K % TG_BK != 0) return false;
+  if (K % TG_BK != 0) return false;
   if (T >= TG_BM) return N % 128 == 0 || N % 192 == 0;
   return N % 32 == 0;  // small-batch weight-streaming variant (T <= 64 uses short A boxes; 65..127 the 128-row box)
 }

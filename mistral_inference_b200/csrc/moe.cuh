@@ -397,10 +397,10 @@ int launch_grouped_bn(const void* a, int64_t rows_cap, int64_t K, int64_t N, con
 // decode-sized calls: the stream-K weight-streaming kernel over (expert segment, n tile, k block) units
 template <int MODE, int TA>
 int launch_grouped_streamk(const void* a, int64_t rows_cap, int64_t K, int64_t N, const void* const* w_host, int E, const int32_t* plan,
-                           const EpiParams& epi, void* workspace, size_t workspace_bytes, size_t header, int sms, cudaStream_t stream) {
+                           const EpiParams& epi, void* workspace, size_t workspace_bytes, int sms, cudaStream_t stream) {
   using Cfg = TgCfg<SK_BN, TA>;
   if (sms > SK_MAX_CTAS) sms = SK_MAX_CTAS;
-  if (workspace == nullptr || workspace_bytes < header + SK_PARTIAL_BYTES) return fail(MB200_E_WORKSPACE, "grouped stream-K gemm: workspace %zu < %zu", workspace_bytes, header + SK_PARTIAL_BYTES);
+  if (workspace == nullptr || workspace_bytes < kWsSkPartials.end()) return fail(MB200_E_WORKSPACE, "grouped stream-K gemm: workspace %zu < %zu", workspace_bytes, kWsSkPartials.end());
   CUtensorMap map_a;
   MoeWeightMaps maps;
   int rc = make_tensor_map_2d(&map_a, a, rows_cap, K, TA);
@@ -419,8 +419,8 @@ int launch_grouped_streamk(const void* a, int64_t rows_cap, int64_t K, int64_t N
   p.N = (int)N;
   p.K = (int)K;
   p.epi = epi;
-  p.partials = reinterpret_cast<float*>((uint8_t*)workspace + header);
-  p.flags = reinterpret_cast<unsigned*>((uint8_t*)workspace + SK_FLAGS_OFFSET);
+  p.partials = reinterpret_cast<float*>((uint8_t*)workspace + kWsSkPartials.offset);
+  p.flags = reinterpret_cast<unsigned*>((uint8_t*)workspace + kWsSkFlags.offset);
   MB_CHECK_CUDA(cudaFuncSetAttribute(gemm_streamk_grouped_kernel<MODE, TA>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmem));
   MB_CHECK_CUDA(launch_pdl(gemm_streamk_grouped_kernel<MODE, TA>, dim3((unsigned)sms), dim3(Cfg::kThreads), (size_t)Cfg::kSmem, stream, map_a, maps, p, plan));
   return MB200_OK;
@@ -428,14 +428,14 @@ int launch_grouped_streamk(const void* a, int64_t rows_cap, int64_t K, int64_t N
 
 template <int MODE>
 int launch_grouped(const void* a, int64_t rows_cap, int64_t K, int64_t N, const void* const* w_host, int E, int est_mtiles, int tile_rows,
-                   const int32_t* plan, const EpiParams& epi, void* workspace, size_t workspace_bytes, size_t header, cudaStream_t stream) {
+                   const int32_t* plan, const EpiParams& epi, void* workspace, size_t workspace_bytes, cudaStream_t stream) {
   int dev = 0, sms = 0;
   MB_CHECK_CUDA(cudaGetDevice(&dev));
   MB_CHECK_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   MB_CHECK_ARG(K % TG_BK == 0 && N % 32 == 0, "grouped gemm: K=%lld must be a multiple of 64, N=%lld of 32", (long long)K, (long long)N);
   if (tile_rows < 128 && streamk_eligible(tile_rows, N, K)) {
-    if (tile_rows == 32) return launch_grouped_streamk<MODE, 32>(a, rows_cap, K, N, w_host, E, plan, epi, workspace, workspace_bytes, header, sms, stream);
-    return launch_grouped_streamk<MODE, 64>(a, rows_cap, K, N, w_host, E, plan, epi, workspace, workspace_bytes, header, sms, stream);
+    if (tile_rows == 32) return launch_grouped_streamk<MODE, 32>(a, rows_cap, K, N, w_host, E, plan, epi, workspace, workspace_bytes, sms, stream);
+    return launch_grouped_streamk<MODE, 64>(a, rows_cap, K, N, w_host, E, plan, epi, workspace, workspace_bytes, sms, stream);
   }
   if (tile_rows == 128) {
     // enough rows per expert for vertically adjacent tile pairs: the 2-CTA cluster kernel (W tile multicast, 2/3 of the L2 -> SM traffic)

@@ -34,6 +34,13 @@ def test_header_symbols_exported(built):
     assert declared == set(_abi._SIGNATURES), declared ^ set(_abi._SIGNATURES)
 
 
+def test_workspace_header_size_matches_the_header():
+    header = (REPO / "include" / "mistral_b200.h").read_text()
+    m = re.search(r"#define MB200_WORKSPACE_HEADER_BYTES \((\d+) \* (\d+)\)", header)
+    assert m, "MB200_WORKSPACE_HEADER_BYTES not found in the form (a * b)"
+    assert _abi.WORKSPACE_HEADER_BYTES == int(m.group(1)) * int(m.group(2))
+
+
 def test_library_loads_and_reports_version(built):
     assert _abi.lib().mb200_abi_version() == _abi.ABI_VERSION
     assert _abi.workspace_bytes(16, 4096, 32, 8, 128, 14336, 32000, 1) > _abi.WORKSPACE_HEADER_BYTES

@@ -1,12 +1,12 @@
 """Attention kernels at tile, window and split edges: which keys each query sees, and how they are weighted.
 
-Four kernels are checked against tables computed here from the mask definition of oracle/attention_ref.py (query at absolute
+Three kernels are checked against tables computed here from the mask definition of oracle/attention_ref.py (query at absolute
 position P sees keys in (P - W, P], bottom-right aligned; a ring slot holds position pos % W; decode sees slots [0, kv_len)):
 attn_prefill_wgmma_kernel (first prefill), attn_prefill_kernel (ring + chunk, the cache-less mode, and first prefill under
-MB200_ATTN=mma), attn_decode_tma_kernel<REP> (default decode) and attn_decode_kernel<REP> (MB200_ATTN_DECODE=plain), every
-compiled head ratio REP = H / KV of 1, 2, 4, 6, 8.  Every GPU test asserts, from the library's launch log, which kernel ran.
+MB200_ATTN=mma) and attn_decode_tma_kernel<REP> (decode), every compiled head ratio REP = H / KV of 1, 2, 4, 6, 8.  Every GPU
+test asserts, from the library's launch log, which kernel ran.
 
-Visible sets (exact).  With q = 0 every score is 0 and every P is exactly 1 in all four kernels (exp2 of 0), so l counts the
+Visible sets (exact).  With q = 0 every score is 0 and every P is exactly 1 in all three kernels (exp2 of 0), so l counts the
 visible keys and P.V sums exact integers in fp32.  V encodes the key's absolute position: dims 0..63 hold
 one-hot((j + a) mod 64), dims 64..127 one-hot((j div 64 + c) mod 64), both scaled by s = 1 or 2, where a, c and s depend on the
 KV head g and the sequence b.  The output is then O[i, h, d] = count_d / n_i, and the kernel's count * fl(1 / n) (or fl(count / n))
@@ -38,8 +38,7 @@ HD = 128
 KV = 2  # small KV counts keep the larger head ratios cheap
 REPS = [1, 2, 4, 6, 8]
 ATTN = r"attn_\w+_kernel"
-KERNEL = {"wgmma": r"attn_prefill_wgmma_kernel\b", "mma": r"attn_prefill_kernel\b", "tma": r"attn_decode_tma_kernel<{rep}>",
-          "plain": r"attn_decode_kernel<{rep}>"}
+KERNEL = {"wgmma": r"attn_prefill_wgmma_kernel\b", "mma": r"attn_prefill_kernel\b", "tma": r"attn_decode_tma_kernel<{rep}>"}
 
 
 class Case(NamedTuple):
@@ -249,11 +248,8 @@ def ws():
 
 def select_kernel(kernel: str, monkeypatch):
     monkeypatch.delenv("MB200_ATTN", raising=False)
-    monkeypatch.delenv("MB200_ATTN_DECODE", raising=False)
     if kernel == "mma":
         monkeypatch.setenv("MB200_ATTN", "mma")  # first prefill would take the wgmma kernel
-    if kernel == "plain":
-        monkeypatch.setenv("MB200_ATTN_DECODE", "plain")
 
 
 def run(case: Case, q: torch.Tensor, K, V, rep: int, ws) -> torch.Tensor:
@@ -346,9 +342,9 @@ def test_cacheless_visible_sets(rep, ws, monkeypatch):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("rep", REPS)
-@pytest.mark.parametrize("kernel", ["tma", "plain"])
+@pytest.mark.parametrize("kernel", ["tma"])
 def test_decode_visible_sets(kernel, rep, ws, monkeypatch):
-    """Both decode kernels: kv_len around the 64-key tile and at the window, more splits than keys, B = 5 on a cache with
+    """The decode kernel: kv_len around the 64-key tile and at the window, more splits than keys, B = 5 on a cache with
     max_batch 6, and on one workspace S = 64 then S = 7 (the split counters reset themselves between launches)."""
     check_visible_sets(decode_cases(), kernel, rep, ws, monkeypatch)
 
@@ -358,7 +354,6 @@ SOFTMAX_CASES = {
     "wgmma": Case("prefill", (0, 0), (300, 129), 200),
     "mma": Case("prefill", (150, 37), (130, 65), 200),
     "tma": Case("decode", (300, 129, 64, 1, 200), (), 300, 7),
-    "plain": Case("decode", (300, 129, 64, 1, 200), (), 300, 7),
 }
 LOG2E = 1.4426950408889634
 SCORE_LOG2_PER_UNIT = HD * HD ** -0.5 * LOG2E  # q = k = all-ones vectors: score in log2 units
@@ -412,7 +407,7 @@ def reference64(case: Case, q: torch.Tensor, K, V, rep: int):
 @pytest.mark.gpu
 @pytest.mark.parametrize("pattern", ["rising", "dominant", "wide"])
 @pytest.mark.parametrize("rep", [1, 4, 8])
-@pytest.mark.parametrize("kernel", ["wgmma", "mma", "tma", "plain"])
+@pytest.mark.parametrize("kernel", ["wgmma", "mma", "tma"])
 def test_softmax_weighting_vs_float64(kernel, rep, pattern, ws, monkeypatch):
     """Online softmax under stress: maxima that grow in every key tile and split, one dominant key at the first / last / tile-edge
     / window-edge position, and scores spanning +-60 in log2 units.  Bound derived in the module docstring."""

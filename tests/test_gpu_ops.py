@@ -224,10 +224,9 @@ def _oracle_decode(q, ck, cv, kv_len, H, KV):
     (4, 300, [300, 299, 17, 150], 9),
 ])
 @pytest.mark.parametrize("H,KV", [(32, 8), (4, 2), (48, 8)])
-@pytest.mark.parametrize("kernel", ["tma", "plain"])
-def test_attn_decode(B, W, lens, S, H, KV, kernel, ws, monkeypatch):
-    """Both decode attention kernels: the TMA-staged tensor-core one (default) and the register-staged one (MB200_ATTN_DECODE=plain)."""
-    monkeypatch.setenv("MB200_ATTN_DECODE", kernel)
+@pytest.mark.parametrize("kernel", ["tma"])
+def test_attn_decode(B, W, lens, S, H, KV, kernel, ws):
+    """The decode attention kernel: TMA-staged K/V tiles, tensor-core scores."""
     if (H, KV) != (32, 8) and W == 4096:
         pytest.skip("long ring: 7B head layout only")
     q = rnd(B, H * 128, seed=20)
@@ -242,10 +241,8 @@ def test_attn_decode(B, W, lens, S, H, KV, kernel, ws, monkeypatch):
     for _ in range(2):  # twice: the split counters must self-reset
         out.zero_()
         _abi.attn_decode(q.to(DEV), ck_d, cv_d, kv_len.to(DEV), out, H, KV, 128, S, ws)
-        if kernel == "plain":
-            assert_bf16_close(out, want, max_ulp=1, min_exact=0.9, atol=2e-3, what="decode attention")
-        else:  # P is rounded to bf16 for the tensor-core PV product, like the prefill kernels (and any tensor-core attention)
-            assert_bf16_close(out, want, max_ulp=2, min_exact=0.5, atol=4e-3, what="decode attention (tma)")
+        # P is rounded to bf16 for the tensor-core PV product, like the prefill kernels (and any tensor-core attention)
+        assert_bf16_close(out, want, max_ulp=2, min_exact=0.5, atol=4e-3, what="decode attention (tma)")
 
 
 def _oracle_prefill(q, k_new, v_new, ck, cv, seqlens, seqpos, W, H, KV):
