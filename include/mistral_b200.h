@@ -330,9 +330,11 @@ int mb200_decode_step(const mb200_layer_desc* layers_dev, const int32_t* windows
  * for tensor-map encoding.  mb200_last_error() is thread-local. */
 #define MB200_WORKSPACE_HEADER_BYTES (64 * 1024)
 
-/* Debug: a device buffer of [8][n_layers][16] uint64 that mb200_decode_step fills with %globaltimer stamps at every phase
- * boundary of 8 sampled CTAs (0, 21, ..., 147: every 21st CTA of a grid of up to 168 SMs); NULL switches it off.  Used by
- * scripts/mk_timeline.py to see where a decode step spends time. */
+/* Debug: a device buffer of [8][n_layers][24] uint64 for 8 sampled CTAs (0, 21, ..., 147: every 21st CTA of a grid of up to
+ * 168 SMs); NULL switches it off.  Per CTA and layer, words 0..15 are %globaltimer stamps at the phase boundaries and words
+ * 16..21 the nanoseconds the weight producers spent blocked (ADDED to the buffer: zero-fill it before the step).  The layout is
+ * spelled out next to mk_stamp in csrc/decode_megakernel.cuh.  Used by scripts/mk_timeline.py to see where a decode step spends
+ * time. */
 int mb200_debug_set_decode_timeline(void* device_buffer);
 /* Debug: [n_sm][n_layers][6][2] uint64 arrive/leave stamps of every CTA at every grid barrier (NULL = off). */
 int mb200_debug_set_barrier_timeline(void* device_buffer);

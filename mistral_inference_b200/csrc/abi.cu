@@ -742,8 +742,8 @@ int mb200_decode_step_supported(int64_t dim, int64_t hidden, int64_t n_heads, in
   return decode_plan(dim, hidden, n_heads, n_kv_heads, head_dim, vocab, n_experts, top_k, smem_optin, &plan);
 }
 
-// Debug: device buffer of [8][n_layers][16] uint64 that 8 sampled CTAs of the decode megakernel fill with %globaltimer stamps
-// (NULL = off; see mk_stamp).
+// Debug: device buffer of [8][n_layers][MK_PROF_WORDS] uint64 that 8 sampled CTAs of the decode megakernel fill with phase
+// stamps and producer blocked times (NULL = off; layout next to mk_stamp).
 int mb200_debug_set_decode_timeline(void* device_buffer) {
   g_mk_prof = (unsigned long long*)device_buffer;
   return MB200_OK;

@@ -6,14 +6,14 @@
 // Here one CTA per SM lives for the whole token:
 //   * a PRODUCER warp walks the CTA's static weight schedule for the whole model (every layer's QKV / wo /
 //     gate-up / down slice and the lm-head slice are contiguous row ranges known up front) and streams it with
-//     cp.async.bulk (TMA bulk copies, completion on mbarriers) through a ~176 KB shared-memory ring.  Weights do
-//     not depend on activations, so the producer never waits for a phase boundary: while the consumers sit in a
-//     grid barrier the ring keeps filling, and HBM stays busy across all ~160 dependencies.
+//     cp.async.bulk (TMA bulk copies, completion on mbarriers) through a shared-memory ring (12 x 16 KB on an H100).
+//     Weights do not depend on activations, so the producer never waits for a phase boundary: while the consumers sit
+//     in a grid barrier the ring keeps filling, and HBM stays busy across all ~190 dependencies.
 //   * 8 CONSUMER warps do the math out of shared memory (fp32 FMA on bf16 pairs; batch 1 is ~0.1 flop/byte, far
 //     below the CUDA-core roof, tensor cores would not help), with the same fused prologues/epilogues as the
 //     per-op kernels (RMSNorm, RoPE + ring scatter, SiLU*mul, residual adds) and the same rounding points as the
 //     reference (SURVEY.md Appendix A).
-//   * phases are separated by a self-resetting sense-reversing grid barrier (5 per layer).
+//   * phases are separated by a grid barrier on monotonic counters (6 per layer, see grid_barrier).
 // Row pairs (2 rows = one RoPE pair / one gate-up pair) are dealt to CTAs as contiguous ranges:
 // CTA c owns pairs [c*P/G, (c+1)*P/G) of each matrix, so its slice of every weight matrix is one contiguous byte
 // range and load imbalance is at most one pair.
@@ -85,15 +85,24 @@ struct MkParams {
   bf16* gbuf;           // [hidden]
   float* partial;       // [KV][splits][REP][hd+2]
   unsigned long long* prof_bar;  // optional [gridDim][n_layers][6][2] arrive/leave %globaltimer of every CTA at every barrier
-  unsigned long long* prof;  // optional [8][n_layers][16] globaltimer stamps of 8 sampled CTAs (debug timeline, see mk_stamp), or null
+  unsigned long long* prof;  // optional [8][n_layers][MK_PROF_WORDS] debug timeline of 8 sampled CTAs (see mk_stamp), or null
 };
 
-// debug timeline: 8 sampled CTAs (every 21st) record %globaltimer at each phase boundary: prof[sample][layer][16] (12..15: inside attention)
+// Debug timeline of 8 sampled CTAs (every 21st): prof[sample][layer][MK_PROF_WORDS] uint64.
+//   words 0..15   %globaltimer when consumer thread 0 passes a phase boundary (mk_stamp; 12..15: inside attention)
+//   words 16..21  ns the producers spent blocked in the stages of that layer (the lm head counts to the last layer), ADDED
+//                 to the buffer, which the caller zero-fills: 16 + producer = waiting for a free slot (ring full),
+//                 18 + producer = waiting on the in-flight cap, 20 + producer = the ring-full waits of MK_PROF_LONG_NS or
+//                 more: the ring stayed full through a consumer stall, so the SM's share of HBM went idle
+//   words 22..23  unused
+constexpr int MK_PROF_STAMPS = 16;
+constexpr int MK_PROF_WORDS = 24;
+constexpr unsigned long long MK_PROF_LONG_NS = 1000;
 __device__ __forceinline__ void mk_stamp(const MkParams& p, int tid, int layer, int idx) {
   if (p.prof != nullptr && tid == 0 && blockIdx.x % 21 == 0) {
     unsigned long long t;
     asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t));
-    p.prof[((blockIdx.x / 21) * p.n_layers + layer) * 16 + idx] = t;
+    p.prof[((blockIdx.x / 21) * p.n_layers + layer) * MK_PROF_WORDS + idx] = t;
   }
 }
 
@@ -261,22 +270,165 @@ __device__ __forceinline__ AttnSlice attn_slice(const MkParams& p, int W) {
   return a;
 }
 
-// ---- producer (one thread) ---------------------------------------------------------------------------------------------
+// ---- producer (one thread per producer warp) ---------------------------------------------------------------------------
 // The CTA's whole schedule (every layer: QKV slice, K/V slice, wo, gate/up, down slices; then the lm-head slice) is a pure
-// function of (blockIdx, shapes, pos), so the producer simply walks it, blocking only on free ring slots.  Its per-stage
-// budget is ~350 cycles (5.5 stages/us per SM at the HBM share of one SM): keep these loops lean -- a generic "schedule
-// iterator" version (needed for a second, L2-prefetch cursor) cost 5 % end to end on its own.
-// Experiment on record (DESIGN.md): running cp.async.bulk.prefetch.L2 D stages ahead to use the L2 as a second-level ring
-// measured slower when this kernel was tuned: the prefetched lines do not survive until the copy.
+// function of (blockIdx, shapes, pos) and, on MoE layers, of the layer's routing decision.  A `Walk` is a position in it: the
+// producer steps it once per stage and blocks only on free ring slots, the in-flight cap and MoE route gates.
+// Per-stage budget: a 16 KB stage lasts ~1,300 cycles at one SM's share of HBM on an H100 (~25 GB/s; ~2,600 cycles per issuing
+// thread), so a few integer divisions per stage are free.  Measured on an H100 80GB HBM3 at a 400 W power limit (Mistral-7B,
+// batch 1, 4k context): this walk decodes at 172.6-173.0 tok/s where the nested loops it replaced ran at 168.5-168.9 (on a
+// B200, at ~350 cycles per stage, a schedule iterator had cost 5 %).
+// Experiment on record: an L2 look-ahead -- a second Walk issuing cp.async.bulk.prefetch.L2 for the stages up to D past the
+// copy cursor while the producer is blocked, so that HBM keeps streaming when a consumer stall outlasts the ring -- measured
+// slower on the same H100: 171.3-171.8 tok/s at D = 8, 16 or 24 stages, 170.2-171.6 with an evict-first hint on the
+// prefetches (on a B200 the prefetched lines did not survive until the copy), although the debug timeline shows the ring
+// staying full through consumer stalls for ~9.5 us of a 167 us layer (DESIGN.md section 3.1): the prefetches are issued by
+// the same producer threads through the same bulk-copy path as the copies, and cost more than the idle time they cover.
+// Each stage is one or more bulk copies that land in the stage's ring slot: `count` pieces of `bytes`, `src_step` elements
+// apart in global memory and `dst_step` bytes apart in the slot.
+struct StageCopy {
+  const bf16* src;
+  int64_t src_step;
+  uint32_t bytes, dst_step;
+  int count;
+};
+
+enum : int { SEG_QKV, SEG_KV, SEG_WO, SEG_UP, SEG_DOWN };  // segments of a layer, in stream order (SEG_UP once per expert)
+
+struct Walk {
+  uint32_t it;              // running stage number (the consumers' RingState::it of the same stage)
+  int layer, seg, e, s, n;  // layer (n_layers: the lm head), segment, gate/up expert of a MoE layer, stage s of the segment's n
+  MatCut c;                 // matrix: its cut (row length c.kc * c.nch)
+  int k_begin, k_end, pps;  // K/V slice: positions and positions per stage (attn_slice)
+  const bf16* W;            // matrix (unused in a MoE down segment: one per routed expert), or the K rows of the K/V slice
+  const bf16* V;            // V rows of the K/V slice
+
+  __device__ __forceinline__ bool done(const MkParams& p) const { return layer > p.n_layers; }
+  // the gate/up segment of a MoE layer whose routing decision the producer does not hold yet: expert weights are unknown
+  __device__ __forceinline__ bool gated(const MkParams& p, int routed) const {
+    return p.n_experts != 0 && layer < p.n_layers && seg == SEG_UP && e == 0 && routed != layer;
+  }
+  __device__ __forceinline__ void matrix(const bf16* w, int N, int K) {
+    W = w;
+    c = cut_matrix(N, K);
+    n = (c.p1 - c.p0) * c.nch;
+  }
+  // experts interleaved per group of pairs: the routed ones in the down segment of a MoE layer, else 1
+  __device__ __forceinline__ int experts(const MkParams& p) const { return (seg == SEG_DOWN && p.n_experts) ? p.top_k : 1; }
+  // shape of the current segment; `sel` packs the routed experts of the current MoE layer, 8 bits each, ascending
+  __device__ __forceinline__ void setup(const MkParams& p, uint32_t sel) {
+    const int q_dim = p.H * kHeadDim, kv_dim = p.KV * kHeadDim;
+    s = 0;
+    if (layer == p.n_layers) {
+      matrix(p.w_out, p.vocab, p.dim);
+      return;
+    }
+    const MkLayer& L = p.layers[layer];
+    if (seg == SEG_QKV) {
+      matrix(L.wqkv, q_dim + 2 * kv_dim, p.dim);
+    } else if (seg == SEG_KV) {
+      const int win = p.windows[layer];
+      const AttnSlice a = attn_slice(p, win);
+      k_begin = a.k_begin;
+      k_end = a.k_end;
+      pps = a.pps;
+      n = 2 * a.n_kvst;  // alternating K / V stages
+      W = L.cache_k + ((int64_t)p.batch_row * win) * kv_dim;
+      V = L.cache_v + ((int64_t)p.batch_row * win) * kv_dim;
+    } else if (seg == SEG_WO) {
+      matrix(L.wo, p.dim, q_dim);
+    } else if (seg == SEG_UP) {
+      matrix(p.n_experts ? p.moe_w13[layer * p.n_experts + ((sel >> (8 * e)) & 0xff)] : L.w13, 2 * p.hidden, p.dim);
+    } else {
+      matrix(L.w2, p.dim, p.hidden);
+      n *= experts(p);
+    }
+  }
+  __device__ __forceinline__ void next_segment(const MkParams& p) {
+    if (layer == p.n_layers) {
+      ++layer;
+      return;
+    }
+    if (seg == SEG_UP && ++e < (p.n_experts ? p.top_k : 1)) return;
+    e = 0;
+    if (++seg > SEG_DOWN) {
+      seg = SEG_QKV;
+      ++layer;
+    }
+  }
+  // moves to the first stage at or after the current segment (skipping segments with no stage on this CTA); stops with n = 0
+  // at the end of the schedule or at a route gate
+  __device__ __forceinline__ void settle(const MkParams& p, uint32_t sel, int routed) {
+    for (;;) {
+      n = 0;
+      if (done(p) || gated(p, routed)) return;
+      setup(p, sel);
+      if (n > 0) return;
+      next_segment(p);
+    }
+  }
+  __device__ __forceinline__ void next(const MkParams& p, uint32_t sel, int routed) {
+    ++it;
+    if (++s < n) return;
+    next_segment(p);
+    settle(p, sel, routed);
+  }
+
+  // the copies of stage s, in the order the consumers expect: a matrix slice in groups of up to 8 pairs, inside a group
+  // expert-major, then chunk-major (stage (j, ch, w) holds K-chunk ch of pair g0 + w of expert j); the K/V slice alternates
+  // K and V stages of `pps` position rows, one copy per row so that rows sit (row bytes + MK_KV_PAD) apart in the slot
+  // (8 consecutive rows then cover all 32 banks for ldmatrix)
+  __device__ __forceinline__ StageCopy stage(const MkParams& p, uint32_t sel) const {
+    StageCopy sc;
+    if (seg == SEG_KV) {
+      const int64_t row_elems = (int64_t)p.KV * kHeadDim;
+      const int k0 = k_begin + (s >> 1) * pps;
+      sc.src = ((s & 1) ? V : W) + (int64_t)k0 * row_elems;
+      sc.src_step = row_elems;
+      sc.bytes = (uint32_t)row_elems * 2;
+      sc.dst_step = sc.bytes + MK_KV_PAD;
+      sc.count = min(pps, k_end - k0);
+      return sc;
+    }
+    const int ne = experts(p), K = c.kc * c.nch;
+    const int per_group = MK_CONSUMER_WARPS * c.nch * ne;
+    const int gi = s / per_group, r = s - gi * per_group;
+    const int g0 = c.p0 + gi * MK_CONSUMER_WARPS, g = min(MK_CONSUMER_WARPS, c.p1 - g0);
+    const int j = r / (c.nch * g), r2 = r - j * (c.nch * g);
+    const int ch = r2 / g, w = r2 - ch * g;
+    const bf16* m = (seg == SEG_DOWN && p.n_experts) ? p.moe_w2[layer * p.n_experts + ((sel >> (8 * j)) & 0xff)] : W;
+    const bf16* r0 = m + (int64_t)(2 * (g0 + w)) * K;
+    sc.bytes = (uint32_t)c.kc * 2;
+    if (c.nch == 1) {  // the two rows are contiguous
+      sc.src = r0;
+      sc.src_step = 0;
+      sc.bytes *= 2;
+      sc.dst_step = 0;
+      sc.count = 1;
+    } else {
+      sc.src = r0 + ch * c.kc;
+      sc.src_step = K;
+      sc.dst_step = sc.bytes;
+      sc.count = 2;
+    }
+    return sc;
+  }
+};
+
 __device__ __forceinline__ void bulk_g2s_hint(void* smem_dst, const void* gsrc, uint32_t bytes, uint64_t* bar, uint64_t policy) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;" ::"r"(
                    smem_u32(smem_dst)),
                "l"(gsrc), "r"(bytes), "r"(smem_u32(bar)), "l"(policy)
                : "memory");
 }
+__device__ __forceinline__ unsigned long long globaltimer() {
+  unsigned long long t;
+  asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t));
+  return t;
+}
 
 // In-flight cap: stage `it` is only issued once stage it - cap has LANDED.  All n_stages slots still buffer data through the
-// phase boundaries, but the SM never has more than `cap` stages of read requests queued: right after a short phase the
+// phase boundaries, but the SM never has more than `cap` stages of copies queued: right after a short phase the
 // consumers have drained the whole ring, and an uncapped producer then fires 12 x 16 KB at once -- the grid barrier's own
 // atomic / polls queue behind that burst in the SM's memory request path (measured: barrier latency 4 us after the wo
 // phase vs 1.5 us in steady state).  The bandwidth-delay product of one SM's HBM share is only ~3 stages.  The cap applies to
@@ -289,96 +441,57 @@ struct Producer {
   uint64_t* full;
   uint64_t* empty;
   int n_stages;
-  uint32_t it;
   uint64_t policy;  // L2 evict-first: weights and old K/V rows are read exactly once per token
   int me;                  // this producer issues the stages with it % MK_PRODUCER_WARPS == me
-  uint32_t slot, par;      // ring slot / parity of stage `it`, kept incrementally (no division in the issue loop)
+  uint32_t slot, par;      // ring slot / parity of the copy cursor's stage, kept incrementally (no division in the issue loop)
   uint32_t cslot, cpar;    // same for stage it - MK_INFLIGHT_CAP
+  uint32_t sel;            // routed experts of MoE layer `routed`, 8 bits each (ascending)
+  int routed;
+  unsigned long long* prof;  // this CTA's rows of the debug timeline, or null
 
-  __device__ __forceinline__ void advance() {
-    ++it;
+  __device__ __forceinline__ bool owns(uint32_t it) const { return (int)(it % (uint32_t)MK_PRODUCER_WARPS) == me; }
+  __device__ __forceinline__ void advance(uint32_t it) {  // ring position of stage it + 1 (`it` = the stage just passed)
     if (++slot == (uint32_t)n_stages) {
       slot = 0;
       par ^= 1;
     }
-    if (it > (uint32_t)MK_INFLIGHT_CAP && ++cslot == (uint32_t)n_stages) {
+    if (it + 1 > (uint32_t)MK_INFLIGHT_CAP && ++cslot == (uint32_t)n_stages) {
       cslot = 0;
       cpar ^= 1;
     }
   }
-  // returns the slot's buffer (and its full barrier, armed for `bytes`) or nullptr when the stage belongs to another producer
-  __device__ __forceinline__ uint8_t* acquire(uint32_t bytes, uint64_t*& bar) {
-    if ((int)(it % (uint32_t)MK_PRODUCER_WARPS) != me) {
-      advance();
-      return nullptr;
+
+  // fills the ring slot of the copy cursor's stage once stage it - cap has landed (its slot cannot have been refilled yet) and
+  // the slot is free.  With the timeline on, the time blocked on either condition is added to the producer's words of the
+  // copy cursor's layer.
+  __device__ __forceinline__ void copy(const MkParams& p, const Walk& cp) {
+    bool landed = cp.it < (uint32_t)MK_INFLIGHT_CAP || mbar_try_wait(&full[cslot], cpar);
+    if (!landed || !mbar_try_wait(&empty[slot], par ^ 1)) {
+      const unsigned long long t0 = prof != nullptr ? globaltimer() : 0ull;
+      unsigned long long t_landed = t0;
+      for (uint32_t spins = 0;;) {
+        if (!landed && mbar_try_wait(&full[cslot], cpar)) {
+          landed = true;
+          if (prof != nullptr) t_landed = globaltimer();
+        }
+        if (landed && mbar_try_wait(&empty[slot], par ^ 1)) break;
+        // the watchdog traps without the printf: a call in this loop makes ptxas spill around it (+256 B of spill loads); a
+        // stuck producer still shows as consumers stuck on `full` in their own watchdog reports
+        if (++spins == MB200_WATCHDOG_SPINS) __trap();
+      }
+      if (prof != nullptr) {
+        const unsigned long long full_ns = globaltimer() - t_landed;
+        unsigned long long* row = prof + (int64_t)min(cp.layer, p.n_layers - 1) * MK_PROF_WORDS + MK_PROF_STAMPS;
+        row[me] += full_ns;
+        row[2 + me] += t_landed - t0;
+        if (full_ns >= MK_PROF_LONG_NS) row[4 + me] += full_ns;
+      }
     }
-    if (it >= (uint32_t)MK_INFLIGHT_CAP) mbar_wait(&full[cslot], cpar, 7, it);  // stage it - cap has landed (its slot cannot have been refilled yet)
-    mbar_wait(&empty[slot], par ^ 1, 1, it);
-    bar = &full[slot];
-    mbar_arrive_expect_tx(bar, bytes);
+    const StageCopy sc = cp.stage(p, sel);
+    uint64_t* bar = &full[slot];
+    mbar_arrive_expect_tx(bar, sc.bytes * (uint32_t)sc.count);
     uint8_t* dst = ring + (size_t)slot * MK_STAGE_BYTES;
-    advance();
-    return dst;
-  }
-
-  // one stage of a matrix slice: K-chunk `ch` of rows 2 * pair and 2 * pair + 1 of W [N, K]
-  __device__ __forceinline__ void pair_stage(const bf16* W, int K, const MatCut& c, int pair, int ch) {
-    const uint32_t row_bytes = (uint32_t)c.kc * 2;
-    const bf16* r0 = W + (int64_t)(2 * pair) * K;
-    uint64_t* bar;
-    uint8_t* dst = acquire(2 * row_bytes, bar);
-    if (dst == nullptr) return;
-    if (c.nch == 1) {
-      bulk_g2s_hint(dst, r0, 2 * row_bytes, bar, policy);  // the two rows are contiguous
-    } else {
-      bulk_g2s_hint(dst, r0 + ch * c.kc, row_bytes, bar, policy);
-      bulk_g2s_hint(dst + row_bytes, r0 + K + ch * c.kc, row_bytes, bar, policy);
-    }
-  }
-
-  // this CTA's slice of one [N, K] weight matrix, in the stage order consume_matrix expects
-  __device__ __forceinline__ void matrix(const bf16* W, int N, int K) {
-    const MatCut c = cut_matrix(N, K);
-    for (int g0 = c.p0; g0 < c.p1; g0 += MK_CONSUMER_WARPS) {
-      const int g = min(MK_CONSUMER_WARPS, c.p1 - g0);
-      for (int ch = 0; ch < c.nch; ++ch)
-        for (int w = 0; w < g; ++w) pair_stage(W, K, c, g0 + w, ch);
-    }
-  }
-
-  // expert down projections of one MoE layer: per group of 8 pairs expert-major, chunk-major (see consume_moe_down)
-  __device__ __forceinline__ void moe_down(const bf16* const* w2, const int* sel, int top_k, int N, int K) {
-    const MatCut c = cut_matrix(N, K);
-    for (int g0 = c.p0; g0 < c.p1; g0 += MK_CONSUMER_WARPS) {
-      const int g = min(MK_CONSUMER_WARPS, c.p1 - g0);
-      for (int j = 0; j < top_k; ++j) {
-        const bf16* W = w2[sel[j]];
-        for (int ch = 0; ch < c.nch; ++ch)
-          for (int w = 0; w < g; ++w) pair_stage(W, K, c, g0 + w, ch);
-      }
-    }
-  }
-
-  // this CTA's K and V slice: alternating K / V stages of `pps` positions; one copy per position row so that rows sit
-  // (row_bytes + 16) apart in shared memory (8 consecutive rows then cover all 32 banks for ldmatrix)
-  __device__ __forceinline__ void kv_slice(const MkParams& p, const MkLayer& L, int W) {
-    const AttnSlice a = attn_slice(p, W);
-    const int64_t row_elems = (int64_t)p.KV * kHeadDim;
-    const uint32_t row_bytes = (uint32_t)row_elems * 2;
-    const bf16* kbase = L.cache_k + ((int64_t)p.batch_row * W) * row_elems;
-    const bf16* vbase = L.cache_v + ((int64_t)p.batch_row * W) * row_elems;
-    for (int j = 0; j < a.n_kvst; ++j) {
-      const int k0 = a.k_begin + j * a.pps;
-      const int rows = min(a.pps, a.k_end - k0);
-#pragma unroll
-      for (int kv = 0; kv < 2; ++kv) {
-        uint64_t* bar;
-        uint8_t* dst = acquire((uint32_t)rows * row_bytes, bar);
-        if (dst == nullptr) continue;
-        const bf16* src = (kv ? vbase : kbase) + (int64_t)k0 * row_elems;
-        for (int r = 0; r < rows; ++r) bulk_g2s_hint(dst + r * (row_bytes + MK_KV_PAD), src + (int64_t)r * row_elems, row_bytes, bar, policy);
-      }
-    }
+    for (int r = 0; r < sc.count; ++r) bulk_g2s_hint(dst + r * sc.dst_step, sc.src + r * sc.src_step, sc.bytes, bar, policy);
   }
 };
 
@@ -389,30 +502,32 @@ __device__ __forceinline__ void producer_main(const MkParams& p, uint8_t* ring, 
   pr.full = full;
   pr.empty = empty;
   pr.n_stages = p.n_stages;
-  pr.it = 0;
   pr.me = me;
   pr.slot = pr.par = pr.cslot = pr.cpar = 0;
+  pr.sel = 0;
+  pr.routed = -1;
+  pr.prof = (p.prof != nullptr && blockIdx.x % 21 == 0) ? p.prof + (int64_t)(blockIdx.x / 21) * p.n_layers * MK_PROF_WORDS : nullptr;
   asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pr.policy));
-  const int q_dim = p.H * kHeadDim, kv_dim = p.KV * kHeadDim;
-  for (int l = 0; l < p.n_layers; ++l) {
-    const MkLayer L = p.layers[l];
-    pr.matrix(L.wqkv, q_dim + 2 * kv_dim, p.dim);
-    pr.kv_slice(p, L, p.windows[l]);
-    pr.matrix(L.wo, p.dim, q_dim);
-    if (p.n_experts == 0) {
-      pr.matrix(L.w13, 2 * p.hidden, p.dim);
-      pr.matrix(L.w2, p.dim, p.hidden);
-    } else {
-      // expert weights are data dependent: wait for this layer's routing decision (the only point where the weight stream
-      // cannot run ahead of the activations)
-      mbar_wait(route_bar, (uint32_t)(l & 1), 8, (uint32_t)l);
-      int sel[MK_MAX_TOPK];
-      for (int j = 0; j < p.top_k; ++j) sel[j] = route->e[j];
-      for (int j = 0; j < p.top_k; ++j) pr.matrix(p.moe_w13[l * p.n_experts + sel[j]], 2 * p.hidden, p.dim);
-      pr.moe_down(p.moe_w2 + l * p.n_experts, sel, p.top_k, p.dim, p.hidden);
+  Walk cp;
+  cp.it = 0;
+  cp.layer = cp.seg = cp.e = 0;
+  cp.settle(p, pr.sel, pr.routed);
+  while (!cp.done(p)) {
+    if (cp.n == 0) {
+      // a MoE layer's route gate: expert weights are data dependent, so wait for the layer's routing decision (the only
+      // point where the weight stream cannot run ahead of the activations)
+      mbar_wait(route_bar, (uint32_t)(cp.layer & 1), 8, (uint32_t)cp.layer);
+      uint32_t sel = 0;
+      for (int j = 0; j < p.top_k; ++j) sel |= (uint32_t)route->e[j] << (8 * j);
+      pr.sel = sel;
+      pr.routed = cp.layer;
+      cp.settle(p, pr.sel, pr.routed);
+      continue;
     }
+    if (pr.owns(cp.it)) pr.copy(p, cp);
+    pr.advance(cp.it);
+    cp.next(p, pr.sel, pr.routed);
   }
-  pr.matrix(p.w_out, p.vocab, p.dim);
 }
 
 // ---- consumers: one weight stage of a pair -----------------------------------------------------------------------------
