@@ -338,7 +338,7 @@ int mb200_decode_step(const mb200_layer_desc* layers_dev, const int32_t* windows
 int mb200_debug_set_decode_timeline(void* device_buffer);
 /* Debug: [n_sm][n_layers][6][2] uint64 arrive/leave stamps of every CTA at every grid barrier (NULL = off). */
 int mb200_debug_set_barrier_timeline(void* device_buffer);
-/* Debug, per calling thread: the attention, dense GEMM and vision data-movement kernels launched since the last call, one line each, named like the
+/* Debug, per calling thread: the attention, dense GEMM, mixture-of-experts and vision data-movement kernels launched since the last call, one line each, named like the
  * kernel with its template arguments (e.g. "attn_decode_tma_kernel<8>", "gemm_wgmma_kernel<0, 1, 32, 64>").  Copies the log
  * into `out` (NUL-terminated; NULL discards it), clears it, and switches recording on (enable != 0) or off.  MB200_E_INVALID
  * when `out` is too small or launches were dropped because the log filled up.  Tests use it to check which kernel a call chose. */

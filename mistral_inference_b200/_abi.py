@@ -402,7 +402,7 @@ def set_barrier_timeline(buf: Optional[torch.Tensor]) -> None:
 
 
 def launch_log(enable: bool) -> list:
-    """Names of the attention / dense GEMM kernels launched from this thread since the last call (empty while recording is off);
+    """Names of the attention / GEMM / MoE kernels launched from this thread since the last call (empty while recording is off);
     clears the log and switches recording on or off (include/mistral_b200.h)."""
     buf = ctypes.create_string_buffer(32768)
     _check(lib().mb200_debug_launch_log(int(enable), ctypes.cast(buf, c_void_p), len(buf)), "mb200_debug_launch_log")

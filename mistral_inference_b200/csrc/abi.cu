@@ -515,15 +515,18 @@ int mb200_moe_route(const void* hn, const void* gate_w, int64_t T, int64_t dim, 
   }
 #undef MB_ROUTE
   MB_CHECK_LAUNCH("moe_route_kernel");
+  note_launch("moe_route_kernel<%d, %s>", (int)n_experts, wide ? "true" : "false");
   const int tile_rows = moe_tile_rows(T);
   const int64_t pairs = T * top_k, cap = moe_tile_cap(pairs, n_experts, tile_rows);
   const size_t plan_smem = ((size_t)n_experts * MP_THREADS + 2 * n_experts + 1) * sizeof(int32_t);
   MB_CHECK_CUDA(cudaFuncSetAttribute(moe_plan_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)plan_smem));
   moe_plan_kernel<<<1, MP_THREADS, plan_smem, st>>>(sel, (int)pairs, (int)n_experts, tile_rows, (int)shard_rank, (int)shard_world, (int)cap, slot, plan);
   MB_CHECK_LAUNCH("moe_plan_kernel");
+  note_launch("moe_plan_kernel<%s>", pairs <= 512 ? "short" : "scan");  // the kernel's own switch: a thread per expert, or the 1024-thread scan
   moe_gather_kernel<<<(unsigned)ceil_div(pairs, 8), 256, 0, st>>>((const uint4*)hn, sel, (const bf16*)wts, slot, (int)pairs, (int)top_k, (int)(dim / 8),
                                                                   (int)shard_rank, (int)shard_world, (uint4*)xs, (bf16*)row_w);
   MB_CHECK_LAUNCH("moe_gather_kernel");
+  note_launch("moe_gather_kernel");
   return MB200_OK;
 }
 
@@ -589,6 +592,7 @@ int mb200_moe_grouped_ffn(const void* xs, const void* const* w13_host, const voi
   }
   moe_combine_kernel<<<(unsigned)T, 128, 0, st>>>(c);
   MB_CHECK_LAUNCH("moe_combine_kernel");
+  note_launch("moe_combine_kernel");
   return MB200_OK;
 }
 

@@ -373,6 +373,7 @@ int launch_grouped_bn(const void* a, int64_t rows_cap, int64_t K, int64_t N, con
   if (CL == 1) {
     gemm_wgmma_grouped_kernel<MODE, CL, BN, TA><<<sms, Cfg::kThreads, Cfg::kSmem, stream>>>(map_a, maps, p, plan);
     MB_CHECK_LAUNCH("gemm_wgmma_grouped_kernel");
+    note_launch("gemm_wgmma_grouped_kernel<%d, %d, %d, %d>", MODE, CL, BN, TA);
     return MB200_OK;
   }
   cudaLaunchConfig_t cfg = {};
@@ -389,6 +390,7 @@ int launch_grouped_bn(const void* a, int64_t rows_cap, int64_t K, int64_t N, con
   cfg.numAttrs = 1;
   MB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, gemm_wgmma_grouped_kernel<MODE, CL, BN, TA>, map_a, maps, p, plan));
   MB_CHECK_LAUNCH("gemm_wgmma_grouped_kernel<cluster 2>");
+  note_launch("gemm_wgmma_grouped_kernel<%d, %d, %d, %d>", MODE, CL, BN, TA);
   return MB200_OK;
 }
 
@@ -423,6 +425,7 @@ int launch_grouped_streamk(const void* a, int64_t rows_cap, int64_t K, int64_t N
   p.flags = reinterpret_cast<unsigned*>((uint8_t*)workspace + kWsSkFlags.offset);
   MB_CHECK_CUDA(cudaFuncSetAttribute(gemm_streamk_grouped_kernel<MODE, TA>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmem));
   MB_CHECK_CUDA(launch_pdl(gemm_streamk_grouped_kernel<MODE, TA>, dim3((unsigned)sms), dim3(Cfg::kThreads), (size_t)Cfg::kSmem, stream, map_a, maps, p, plan));
+  note_launch("gemm_streamk_grouped_kernel<%d, %d>", MODE, TA);
   return MB200_OK;
 }
 

@@ -79,7 +79,7 @@ def assert_bf16_close(got: torch.Tensor, want: torch.Tensor, max_ulp: int = 1, m
 
 # ----------------------------------------------------------------------------- which kernels a call launched
 def launched_kernels(fn) -> List[str]:
-    """Runs `fn()` and returns the attention and dense GEMM kernels libmb200 launched for it, in order, named like the kernels
+    """Runs `fn()` and returns the attention, GEMM and MoE kernels libmb200 launched for it, in order, named like the kernels
     with their template arguments ("attn_decode_tma_kernel<8>").  The library records each launch next to the launch statement
     (mb200_debug_launch_log), so the record does not depend on a profiler being able to attach."""
     from mistral_inference_b200 import _abi
