@@ -270,6 +270,30 @@ int mb200_moe_grouped_ffn(const void* xs, const void* const* w13_host, const voi
                           int64_t hidden, int64_t n_experts, int64_t top_k, const mb200_moe_comm* comm, void* workspace,
                           size_t workspace_bytes, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * FP8 (e4m3) expert weights.  A storage format with an exact definition: per row n of an expert matrix W [N, K] (bf16),
+ *     s[n] = fp32(amax_k |W[n, k]| / 448)  (IEEE division; s[n] = 1 for an all-zero row)
+ *     q[n, k] = e4m3fn_rn(clamp(fp32(W[n, k] / s[n]), -448, 448))  (IEEE division, round to nearest even)
+ *     W'[n, k] = bf16_rn(fp32(float(q[n, k]) * s[n]))
+ * and the FP8 model computes exactly what the bf16 model computes with expert weights W': every rounding after the weights is the
+ * bf16 path's.
+ *
+ * mb200_quantize_e4m3_rows: q and s of a bf16 matrix w [rows, K] (K a multiple of 8).  Row n of q starts at q + n * q_row_stride
+ *     bytes, its scale is scale[n * scale_stride]: with q_row_stride = 2 * K and scale_stride = 2, w1 and w3 (offset by one row
+ *     and one scale) fill the interleaved rows of the packed gate/up matrix (row 2i = w1[i], row 2i + 1 = w3[i]).
+ * mb200_moe_grouped_ffn_fp8: mb200_moe_grouped_ffn with e4m3 experts: w13_host / w2_host are HOST arrays of E device pointers to
+ *     q (packed gate/up [2*hidden, dim] and down [dim, hidden], one byte per element), w13_scale_host / w2_scale_host HOST arrays
+ *     of E device pointers to their fp32 row scales ([2*hidden] and [dim]); NULL for experts of other ranks.  The grouped GEMMs
+ *     load the e4m3 tiles and convert them to W' in shared memory; tile rows, tile width and the stream-K partition are those of
+ *     mb200_moe_grouped_ffn for the same plan, except that 128-row calls never run as 2-CTA clusters.
+ */
+int mb200_quantize_e4m3_rows(const void* w, int64_t rows, int64_t K, void* q, int64_t q_row_stride, float* scale, int64_t scale_stride,
+                             void* stream);
+int mb200_moe_grouped_ffn_fp8(const void* xs, const void* const* w13_host, const float* const* w13_scale_host, const void* const* w2_host,
+                              const float* const* w2_scale_host, const int32_t* plan, const void* row_w, const int32_t* slot,
+                              const void* residual, void* g, void* yw, void* out, int64_t T, int64_t dim, int64_t hidden, int64_t n_experts,
+                              int64_t top_k, const mb200_moe_comm* comm, void* workspace, size_t workspace_bytes, void* stream);
+
 /* Buffers that other ranks (one process per GPU) can write: plain cudaMalloc + CUDA IPC.  alloc zero-fills and synchronises;
  * export writes the 64-byte IPC handle to pass to the other processes (e.g. torch.distributed.all_gather_object); open maps a
  * peer's buffer into this process (peer access over NVLink is enabled lazily).  These are the only entry points that allocate. */

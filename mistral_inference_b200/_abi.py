@@ -56,6 +56,9 @@ _SIGNATURES = {
                                 c_void_p, c_void_p, c_void_p]),
     "mb200_moe_grouped_ffn": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64,
                                       c_int64, c_int64, c_int64, c_int64, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "mb200_quantize_e4m3_rows": (c_int, [c_void_p, c_int64, c_int64, c_void_p, c_int64, c_void_p, c_int64, c_void_p]),
+    "mb200_moe_grouped_ffn_fp8": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                          c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int64, c_int64, c_void_p, c_void_p, c_size_t, c_void_p]),
     "mb200_comm_alloc": (c_int, [c_size_t, ctypes.POINTER(c_void_p)]),
     "mb200_comm_free": (c_int, [c_void_p]),
     "mb200_comm_export": (c_int, [c_void_p, c_void_p]),
@@ -347,6 +350,26 @@ def moe_grouped_ffn(b, w13_host, w2_host, residual: Optional[torch.Tensor], out:
                                        _ptr(b.slot), _ptr(residual), _ptr(b.g), b.yw_ptr, _ptr(out), T, dim, hidden, E, k,
                                        ctypes.cast(ctypes.pointer(comm), c_void_p) if comm is not None else None, ws.ptr, ws.nbytes, _stream()),
            "mb200_moe_grouped_ffn")
+
+
+def moe_grouped_ffn_fp8(b, w13_host, s13_host, w2_host, s2_host, residual: Optional[torch.Tensor], out: torch.Tensor, T: int, dim: int,
+                        hidden: int, E: int, k: int, comm: Optional[MoeCommStruct], ws: "Workspace") -> None:
+    """moe_grouped_ffn with e4m3 experts: host arrays of E device pointers to the weights and to their fp32 row scales."""
+    _check(lib().mb200_moe_grouped_ffn_fp8(_ptr(b.xs), ctypes.cast(w13_host, c_void_p), ctypes.cast(s13_host, c_void_p),
+                                           ctypes.cast(w2_host, c_void_p), ctypes.cast(s2_host, c_void_p), _ptr(b.plan), _ptr(b.row_w),
+                                           _ptr(b.slot), _ptr(residual), _ptr(b.g), b.yw_ptr, _ptr(out), T, dim, hidden, E, k,
+                                           ctypes.cast(ctypes.pointer(comm), c_void_p) if comm is not None else None, ws.ptr, ws.nbytes,
+                                           _stream()), "mb200_moe_grouped_ffn_fp8")
+
+
+def quantize_e4m3_rows(w: torch.Tensor, q: torch.Tensor, scale: torch.Tensor) -> None:
+    """q (uint8 [rows, K], rows may be strided) and scale (fp32 [rows], may be strided) of the bf16 matrix w [rows, K]."""
+    rows, K = w.shape
+    assert w.dtype == torch.bfloat16 and q.dtype == torch.uint8 and scale.dtype == torch.float32, (w.dtype, q.dtype, scale.dtype)
+    assert q.shape == (rows, K) and q.stride(1) == 1 and scale.shape == (rows,), (tuple(q.shape), tuple(scale.shape))
+    assert q.is_cuda and scale.is_cuda and w.device == q.device == scale.device
+    _check(lib().mb200_quantize_e4m3_rows(_ptr(w), rows, K, q.data_ptr(), q.stride(0), scale.data_ptr(), scale.stride(0), _stream()),
+           "mb200_quantize_e4m3_rows")
 
 
 def comm_alloc(nbytes: int) -> int:

@@ -530,9 +530,11 @@ int mb200_moe_route(const void* hn, const void* gate_w, int64_t T, int64_t dim, 
   return MB200_OK;
 }
 
-int mb200_moe_grouped_ffn(const void* xs, const void* const* w13_host, const void* const* w2_host, const int32_t* plan, const void* row_w,
-                          const int32_t* slot, const void* residual, void* g, void* yw, void* out, int64_t T, int64_t dim, int64_t hidden,
-                          int64_t n_experts, int64_t top_k, const mb200_moe_comm* comm, void* workspace, size_t workspace_bytes, void* stream) {
+// s13 / s2: NULL for bf16 experts; for FP8 ones the host arrays of per-row fp32 scale pointers next to the e4m3 weights
+static int moe_grouped_ffn(const void* xs, const void* const* w13_host, const void* const* w2_host, const float* const* s13_host,
+                           const float* const* s2_host, const int32_t* plan, const void* row_w, const int32_t* slot, const void* residual, void* g,
+                           void* yw, void* out, int64_t T, int64_t dim, int64_t hidden, int64_t n_experts, int64_t top_k, const mb200_moe_comm* comm,
+                           void* workspace, size_t workspace_bytes, void* stream) {
   MB_CHECK_ARG(xs && w13_host && w2_host && plan && row_w && slot && g && yw && out, "moe_grouped_ffn: null pointer");
   MB_CHECK_ARG(T >= 1 && top_k >= 1 && top_k <= MOE_MAX_TOPK && n_experts <= MOE_MAX_EXPERTS && dim % 64 == 0 && hidden % 64 == 0,
                "moe_grouped_ffn: T=%lld k=%lld E=%lld dim=%lld hidden=%lld", (long long)T, (long long)top_k, (long long)n_experts, (long long)dim,
@@ -553,7 +555,8 @@ int mb200_moe_grouped_ffn(const void* xs, const void* const* w13_host, const voi
   EpiParams e1;
   e1.out = g;
   e1.ld_out = hidden;
-  int rc = launch_grouped<EPI_SWIGLU>(xs, rows_cap, dim, 2 * hidden, w13_host, (int)n_experts, est, tile_rows, plan, e1, workspace, workspace_bytes, st);
+  int rc = launch_grouped<EPI_SWIGLU>(xs, rows_cap, dim, 2 * hidden, w13_host, (int)n_experts, est, tile_rows, plan, e1, workspace, workspace_bytes, st,
+                                      s13_host);
   if (rc) return rc;
   EpiParams e2;
   e2.out = yw;
@@ -564,7 +567,8 @@ int mb200_moe_grouped_ffn(const void* xs, const void* const* w13_host, const voi
     MB_CHECK_ARG(comm->peer_yw[r] != nullptr, "moe_grouped_ffn: peer buffer %d missing", r);
     e2.peer_out[r] = comm->peer_yw[r];
   }
-  rc = launch_grouped<EPI_MOE_SCALE>(g, rows_cap, hidden, dim, w2_host, (int)n_experts, est, tile_rows, plan, e2, workspace, workspace_bytes, st);
+  rc = launch_grouped<EPI_MOE_SCALE>(g, rows_cap, hidden, dim, w2_host, (int)n_experts, est, tile_rows, plan, e2, workspace, workspace_bytes, st,
+                                     s2_host);
   if (rc) return rc;
   MoeCombineParams c;
   c.yw = (const uint4*)yw;
@@ -593,6 +597,35 @@ int mb200_moe_grouped_ffn(const void* xs, const void* const* w13_host, const voi
   moe_combine_kernel<<<(unsigned)T, 128, 0, st>>>(c);
   MB_CHECK_LAUNCH("moe_combine_kernel");
   note_launch("moe_combine_kernel");
+  return MB200_OK;
+}
+
+int mb200_moe_grouped_ffn(const void* xs, const void* const* w13_host, const void* const* w2_host, const int32_t* plan, const void* row_w,
+                          const int32_t* slot, const void* residual, void* g, void* yw, void* out, int64_t T, int64_t dim, int64_t hidden,
+                          int64_t n_experts, int64_t top_k, const mb200_moe_comm* comm, void* workspace, size_t workspace_bytes, void* stream) {
+  return moe_grouped_ffn(xs, w13_host, w2_host, nullptr, nullptr, plan, row_w, slot, residual, g, yw, out, T, dim, hidden, n_experts, top_k, comm,
+                         workspace, workspace_bytes, stream);
+}
+
+int mb200_moe_grouped_ffn_fp8(const void* xs, const void* const* w13_host, const float* const* w13_scale_host, const void* const* w2_host,
+                              const float* const* w2_scale_host, const int32_t* plan, const void* row_w, const int32_t* slot, const void* residual,
+                              void* g, void* yw, void* out, int64_t T, int64_t dim, int64_t hidden, int64_t n_experts, int64_t top_k,
+                              const mb200_moe_comm* comm, void* workspace, size_t workspace_bytes, void* stream) {
+  MB_CHECK_ARG(w13_scale_host && w2_scale_host, "moe_grouped_ffn_fp8: null scale table");
+  return moe_grouped_ffn(xs, w13_host, w2_host, w13_scale_host, w2_scale_host, plan, row_w, slot, residual, g, yw, out, T, dim, hidden, n_experts,
+                         top_k, comm, workspace, workspace_bytes, stream);
+}
+
+int mb200_quantize_e4m3_rows(const void* w, int64_t rows, int64_t K, void* q, int64_t q_row_stride, float* scale, int64_t scale_stride, void* stream) {
+  MB_CHECK_ARG(w && q && scale, "quantize_e4m3_rows: null pointer");
+  MB_CHECK_ARG(rows >= 1 && rows <= 0x7fffffff && K >= 8 && K % 8 == 0 && K <= (1 << 24), "quantize_e4m3_rows: rows=%lld K=%lld (K a multiple of 8)",
+               (long long)rows, (long long)K);
+  MB_CHECK_ARG(q_row_stride >= K && q_row_stride % 8 == 0 && scale_stride >= 1, "quantize_e4m3_rows: q_row_stride=%lld (>= K, multiple of 8) scale_stride=%lld",
+               (long long)q_row_stride, (long long)scale_stride);
+  MB_CHECK_ARG(((uintptr_t)w & 15) == 0 && ((uintptr_t)q & 7) == 0 && ((uintptr_t)scale & 3) == 0, "quantize_e4m3_rows: misaligned pointer");
+  quantize_e4m3_rows_kernel<<<(unsigned)rows, 256, 0, (cudaStream_t)stream>>>((const uint4*)w, (int)K, (uint8_t*)q, q_row_stride, scale, scale_stride);
+  MB_CHECK_LAUNCH("quantize_e4m3_rows_kernel");
+  note_launch("quantize_e4m3_rows_kernel");
   return MB200_OK;
 }
 

@@ -55,14 +55,19 @@ struct SkParams {
   unsigned* flags;  // [gridDim], zero between launches
 };
 
-template <int MODE, int TA, bool GROUPED>
-__device__ __forceinline__ void sk_gemm_body(const CUtensorMap& map_a, const CUtensorMap* map_w_base, const SkParams& p, const int32_t* plan) {
-  using Cfg = TgCfg<SK_BN, TA>;
+// W8 (grouped only): FP8 expert weights, converted per stage by warps 1-3 exactly as in tc_gemm_body (gemm_wgmma.cuh).  The
+// partition into (tile, k-block) units is the bf16 kernel's, so an FP8 call splits and sums every tile the same way.
+template <int MODE, int TA, bool GROUPED, bool W8 = false>
+__device__ __forceinline__ void sk_gemm_body(const CUtensorMap& map_a, const CUtensorMap* map_w_base, const SkParams& p, const int32_t* plan,
+                                             const MoeWeightScales* scales = nullptr) {
+  static_assert(!W8 || GROUPED, "FP8 weights: grouped variant only");
+  using Cfg = TgCfg<SK_BN, TA, W8>;
   constexpr int STAGES = Cfg::kStages, STAGE_BYTES = Cfg::kStageBytes, A_BYTES = Cfg::kABytes, NCONS = 128 * Cfg::kWG;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES + Cfg::kSlack);
   uint64_t* empty = full + STAGES;
+  uint64_t* raw = empty + STAGES;  // W8 only
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int G = (int)gridDim.x, cta = (int)blockIdx.x;
@@ -78,8 +83,9 @@ __device__ __forceinline__ void sk_gemm_body(const CUtensorMap& map_a, const CUt
 
   if (threadIdx.x == 0) {
     for (int i = 0; i < STAGES; ++i) {
-      mbar_init(&full[i], 1);
+      mbar_init(&full[i], W8 ? 1 + W8_CONVERTERS : 1);
       mbar_init(&empty[i], Cfg::kWG);
+      if (W8) mbar_init(&raw[i], 1);
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&map_a) : "memory");
@@ -110,7 +116,12 @@ __device__ __forceinline__ void sk_gemm_body(const CUtensorMap& map_a, const CUt
         if (do_w) {
           const int n0 = (tile / num_m) * SK_BN;
           const CUtensorMap* wmap = GROUPED ? map_w_base + tile_expert[tile % num_m] : map_w_base;
-          tma_load_2d(sa + A_BYTES, wmap, &full[s], kb * TG_BK, n0);
+          if (W8) {
+            mbar_arrive_expect_tx(&raw[s], Cfg::kRawBytes);
+            tma_load_2d(sa + A_BYTES + Cfg::kBBytes, wmap, &raw[s], kb * TG_BK, n0);
+          } else {
+            tma_load_2d(sa + A_BYTES, wmap, &full[s], kb * TG_BK, n0);
+          }
         }
         if (do_a) tma_load_2d(sa, &map_a, &full[s], kb * TG_BK, GROUPED ? tile_row0[tile % num_m] : 0);
       };
@@ -125,10 +136,22 @@ __device__ __forceinline__ void sk_gemm_body(const CUtensorMap& map_a, const CUt
       for (uint32_t it = head; it < n_it; ++it) {
         const uint32_t s = it % STAGES, par = (it / STAGES) & 1;
         mbar_wait_quiet(&empty[s], par ^ 1);
-        mbar_arrive_expect_tx(&full[s], STAGE_BYTES);
+        mbar_arrive_expect_tx(&full[s], W8 ? A_BYTES : STAGE_BYTES);
         issue(it, true, true);
       }
       SK_STAMP(3);  // last tile requested
+    }
+  } else if (W8 && warp < 4) {
+    // ================= FP8: e4m3 -> bf16 W' tile of every stage, in the producer's order =================
+    const int ct = (int)threadIdx.x - 32;
+    const uint32_t n_it = (uint32_t)(u_end - u_begin);
+    for (uint32_t it = 0; it < n_it; ++it) {
+      const int tile = (int)(((uint32_t)u_begin + it) / (uint32_t)num_k);
+      const uint32_t s = it % STAGES, par = (it / STAGES) & 1;
+      mbar_wait_quiet(&raw[s], par);
+      uint8_t* sa = smem + s * STAGE_BYTES;
+      convert_w8_tile<SK_BN>(sa + A_BYTES + Cfg::kBBytes, sa + A_BYTES, scales->s[tile_expert[tile % num_m]] + (tile / num_m) * SK_BN, ct);
+      mbar_arrive(&full[s]);
     }
   } else if (warp >= 4) {
     // ================= consumer warpgroups: rows 64 * wg .. + 63 of the [TA x 128] tile =================
@@ -235,6 +258,13 @@ __global__ void __launch_bounds__(TgCfg<SK_BN, TA>::kThreads, 1)
     gemm_streamk_grouped_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ MoeWeightMaps maps_w, const SkParams p,
                                 const int32_t* __restrict__ plan) {
   sk_gemm_body<MODE, TA, true>(map_a, maps_w.m, p, plan);
+}
+
+template <int MODE, int TA>
+__global__ void __launch_bounds__(TgCfg<SK_BN, TA, true>::kThreads, 1)
+    gemm_streamk_grouped_fp8_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ MoeWeightMaps maps_w,
+                                    const __grid_constant__ MoeWeightScales scales, const SkParams p, const int32_t* __restrict__ plan) {
+  sk_gemm_body<MODE, TA, true, true>(map_a, maps_w.m, p, plan, &scales);
 }
 
 inline bool streamk_eligible(int64_t T, int64_t N, int64_t K) {

@@ -13,6 +13,8 @@
 // Tiles are walked m-fastest so that the CTAs that share a W tile run together and hit it in L2.
 #pragma once
 #include <cuda.h>
+#include <cuda_fp16.h>
+#include <cuda_fp8.h>
 
 #include <cstdlib>
 
@@ -32,11 +34,14 @@ constexpr int TG_BM = 128, TG_BN = 256, TG_BK = 64;
 // it in the stage -- accumulator row i depends on A row i only, and rows >= TA are never stored.  The stage shrinks to
 // (TA + BN) * 128 bytes, so the ring gets deep enough to keep a whole SM's share of HBM bandwidth in flight: those launches are
 // weight-streaming GEMMs, bound by HBM, with BN chosen by the launcher to give every SM at most one (equal) tile per round.
-template <int BN, int TA = 128>
+// W8 (FP8 expert weights, csrc/moe.cuh): a stage also holds the e4m3 [BN x 64] W tile as TMA delivered it (kRawBytes, unswizzled)
+// next to the bf16 tile the MMAs read, which the producer warpgroup's three idle warps write from it (convert_w8_tile).
+template <int BN, int TA = 128, bool W8 = false>
 struct TgCfg {
   static constexpr int kABytes = TA * TG_BK * 2;
   static constexpr int kBBytes = BN * TG_BK * 2;
-  static constexpr int kStageBytes = kABytes + kBBytes;
+  static constexpr int kRawBytes = W8 ? BN * TG_BK : 0;
+  static constexpr int kStageBytes = kABytes + kBBytes + kRawBytes;
   static constexpr int kWG = TA > 64 ? 2 : 1;  // consumer warpgroups: 64 accumulator rows each
   static constexpr int kThreads = 128 * (1 + kWG);
   // A wgmma reads 64 rows (8 KB) from a stage's A base; in the LAST stage that must not run past the ring
@@ -44,10 +49,11 @@ struct TgCfg {
   static constexpr int kMaxStages = (227 * 1024 - 1024 - 512 - kSlack) / kStageBytes;
   // decode-sized variants: a ring of ~100 KB (80 KB of weights in flight per CTA, above the bandwidth-delay product of one SM's
   // share of HBM) instead of the whole 227 KB: a successor's CTA, which starts when the predecessor's CTA on its SM exits, has its
-  // first ring filled sooner, and other decode kernels' CTAs fit beside it.
-  static constexpr int kShortRingStages = (100 * 1024) / kStageBytes;
+  // first ring filled sooner, and other decode kernels' CTAs fit beside it.  W8: an e4m3 stage carries half the HBM bytes of a
+  // bf16 one and needs the bf16 tile beside it, so its ring is twice as long to keep the same bytes in flight.
+  static constexpr int kShortRingStages = ((W8 ? 200 : 100) * 1024) / kStageBytes;
   static constexpr int kStages = (TA < 128 || BN < 128) ? (kShortRingStages < 3 ? 3 : (kShortRingStages > kMaxStages ? kMaxStages : kShortRingStages))
-                                                        : (BN == 128 ? 6 : 4);
+                                                        : W8 ? kMaxStages : (BN == 128 ? 6 : 4);
   static constexpr int kSmem = kStages * kStageBytes + kSlack + 1024 /*align*/ + 512 /*barriers*/;
   static_assert(kSmem <= 227 * 1024, "shared memory plan exceeds the 227 KB of an sm_90 block");
 };
@@ -85,6 +91,36 @@ __device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta)
   uint32_t remote;
   asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(smem_u32(bar)), "r"(cta));
   asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(remote) : "memory");
+}
+
+// ---- FP8 expert weights: e4m3 tile -> the bf16 W' tile of the stage ----------------------------------------------------------
+// W'[n, k] = bf16_rn(fp32(float(q[n, k]) * s[n])): e4m3 -> f16 is exact (cvt.rn.f16x2.e4m3x2), f16 -> f32 exact, one IEEE fp32
+// multiply, one bf16 rounding -- the same bits as the CPU restatement in oracle/fp8.py.  The bf16 tile is written in the 128B-swizzled
+// layout TMA gives the bf16 kernels (16-byte chunk c of row r at chunk c ^ (r & 7)), so the wgmma descriptors are unchanged.
+// Thread ct of W8_CONVERTERS takes 16-byte e4m3 chunks ct, ct + W8_CONVERTERS, ...: consecutive threads read consecutive 16 bytes,
+// and each quarter warp's 16-byte stores hit 8 distinct chunk columns of two rows (no bank conflicts).
+constexpr int W8_CONVERTERS = 96;  // warps 1-3 of the producer warpgroup
+template <int BN>
+__device__ __forceinline__ void convert_w8_tile(const uint8_t* raw, uint8_t* wtile, const float* __restrict__ scale_rows, int ct) {
+#pragma unroll 2
+  for (int q = ct; q < BN * (TG_BK / 16); q += W8_CONVERTERS) {
+    const int row = q >> 2, c = q & 3;
+    const uint4 v = *reinterpret_cast<const uint4*>(raw + row * TG_BK + c * 16);
+    const float s = __ldg(scale_rows + row);
+    const uint32_t in[4] = {v.x, v.y, v.z, v.w};
+    uint32_t o[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const __half2_raw hr = __nv_cvt_fp8x2_to_halfraw2((__nv_fp8x2_storage_t)(in[j >> 1] >> (16 * (j & 1))), __NV_E4M3);
+      const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&hr));
+      const __nv_bfloat162 b = __floats2bfloat162_rn(__fmul_rn(f.x, s), __fmul_rn(f.y, s));
+      o[j] = *reinterpret_cast<const uint32_t*>(&b);
+    }
+    uint8_t* dst = wtile + row * (TG_BK * 2);
+    *reinterpret_cast<uint4*>(dst + (((2 * c) ^ (row & 7)) << 4)) = make_uint4(o[0], o[1], o[2], o[3]);
+    *reinterpret_cast<uint4*>(dst + (((2 * c + 1) ^ (row & 7)) << 4)) = make_uint4(o[4], o[5], o[6], o[7]);
+  }
+  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy stores -> the wgmma (async proxy) reads
 }
 
 // One consumer warpgroup's share of a k-block: the 64 tile rows starting at a_addr against the whole [BN x 64] W tile.
@@ -125,16 +161,24 @@ constexpr int MOE_MAX_EXPERTS = 16;  // tensor maps travel as kernel parameters 
 struct MoeWeightMaps {
   CUtensorMap m[MOE_MAX_EXPERTS];
 };
+struct MoeWeightScales {  // W8: per-row fp32 scales of each expert's matrix (null for experts of other ranks)
+  const float* s[MOE_MAX_EXPERTS];
+};
 
-template <int MODE, int CL, int BN, int TA, bool GROUPED>
-__device__ __forceinline__ void tc_gemm_body(const CUtensorMap& map_a, const CUtensorMap* map_w_base, const TcGemmParams& p, const int32_t* plan) {
+// W8 (grouped, single CTA only): the producer thread loads the e4m3 W tile into the stage's raw area on raw[s]; warps 1-3 wait on
+// raw[s], write the bf16 tile and arrive on full[s] (W8_CONVERTERS arrivals next to the producer's expect_tx for the A tile).
+template <int MODE, int CL, int BN, int TA, bool GROUPED, bool W8 = false>
+__device__ __forceinline__ void tc_gemm_body(const CUtensorMap& map_a, const CUtensorMap* map_w_base, const TcGemmParams& p, const int32_t* plan,
+                                             const MoeWeightScales* scales = nullptr) {
   static_assert(TA == 128 || CL == 1, "small-batch variant is single-CTA");
-  using Cfg = TgCfg<BN, TA>;
+  static_assert(!W8 || (GROUPED && CL == 1), "FP8 weights: grouped single-CTA variant only");
+  using Cfg = TgCfg<BN, TA, W8>;
   constexpr int STAGES = Cfg::kStages, B_BYTES = Cfg::kBBytes, STAGE_BYTES = Cfg::kStageBytes, A_BYTES = Cfg::kABytes;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);  // SW128 wants 1024-B tiles
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES + Cfg::kSlack);
   uint64_t* empty = full + STAGES;
+  uint64_t* raw = empty + STAGES;  // W8 only
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int rank = CL > 1 ? (int)cluster_ctarank() : 0;
@@ -197,8 +241,9 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& map_a, const CUt
 
   if (threadIdx.x == 0) {
     for (int i = 0; i < STAGES; ++i) {
-      mbar_init(&full[i], 1);
+      mbar_init(&full[i], W8 ? 1 + W8_CONVERTERS : 1);
       mbar_init(&empty[i], CL * Cfg::kWG);
+      if (W8) mbar_init(&raw[i], 1);
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&map_a) : "memory");
@@ -222,8 +267,15 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& map_a, const CUt
         for (int kb = 0; kb < num_k; ++kb, ++it) {
           const uint32_t s = it % STAGES, par = (it / STAGES) & 1;
           mbar_wait_quiet(&empty[s], par ^ 1);
-          mbar_arrive_expect_tx(&full[s], STAGE_BYTES);  // A + both halves of W (the peer's half may land first: tx-count goes negative)
           uint8_t* sa = smem + s * STAGE_BYTES;
+          if constexpr (W8) {
+            mbar_arrive_expect_tx(&full[s], A_BYTES);
+            tma_load_2d(sa, &map_a, &full[s], kb * TG_BK, m0);
+            mbar_arrive_expect_tx(&raw[s], Cfg::kRawBytes);
+            tma_load_2d(sa + A_BYTES + B_BYTES, wmap, &raw[s], kb * TG_BK, n0);
+            continue;
+          }
+          mbar_arrive_expect_tx(&full[s], STAGE_BYTES);  // A + both halves of W (the peer's half may land first: tx-count goes negative)
           tma_load_2d(sa, &map_a, &full[s], kb * TG_BK, m0);
           if (CL > 1)
             tma_load_2d_multicast(sa + A_BYTES + rank * (B_BYTES / CL), wmap, &full[s], kb * TG_BK, n0 + rank * (BN / CL),
@@ -231,6 +283,22 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& map_a, const CUt
           else
             tma_load_2d(sa + A_BYTES, wmap, &full[s], kb * TG_BK, n0);
         }
+      }
+    }
+  } else if (W8 && warp < 4) {
+    // ================= FP8: e4m3 -> bf16 W' tile of every stage, in the producer's order =================
+    const int ct = (int)threadIdx.x - 32;
+    uint32_t it = 0;
+    for (int tile = cta; tile < num_tiles; tile += n_cta) {
+      int mu, nt;
+      tile_mn(tile, mu, nt);
+      const float* srows = scales->s[tile_expert[mu]] + nt * BN;
+      for (int kb = 0; kb < num_k; ++kb, ++it) {
+        const uint32_t s = it % STAGES, par = (it / STAGES) & 1;
+        mbar_wait_quiet(&raw[s], par);
+        uint8_t* sa = smem + s * STAGE_BYTES;
+        convert_w8_tile<BN>(sa + A_BYTES + B_BYTES, sa + A_BYTES, srows, ct);
+        mbar_arrive(&full[s]);
       }
     }
   } else if (warp >= 4) {
@@ -287,6 +355,14 @@ __global__ void __launch_bounds__(TgCfg<BN, TA>::kThreads, 1)
   tc_gemm_body<MODE, CL, BN, TA, true>(map_a, maps_w.m, p, plan);
 }
 
+// FP8 expert weights: maps_w are e4m3 [N, K] maps (box [BN x 64] bytes, no swizzle), scales the per-row fp32 scales.
+template <int MODE, int BN, int TA>
+__global__ void __launch_bounds__(TgCfg<BN, TA, true>::kThreads, 1)
+    gemm_wgmma_grouped_fp8_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ MoeWeightMaps maps_w,
+                                  const __grid_constant__ MoeWeightScales scales, const TcGemmParams p, const int32_t* __restrict__ plan) {
+  tc_gemm_body<MODE, 1, BN, TA, true, true>(map_a, maps_w.m, p, plan, &scales);
+}
+
 // ---- host: tensor maps (driver API through the runtime's entry-point lookup, no libcuda link dependency) ----
 typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
                                     const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
@@ -313,6 +389,20 @@ inline int make_tensor_map_2d(CUtensorMap* map, const void* base, int64_t rows, 
   const CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                          CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) return fail(MB200_E_CUDA, "cuTensorMapEncodeTiled failed (%d) rows=%lld K=%lld", (int)r, (long long)rows, (long long)K);
+  return MB200_OK;
+}
+
+// [rows, K] e4m3 (one byte per element), box = [box_rows x 64] bytes, unswizzled: the raw tile that convert_w8_tile reads
+inline int make_tensor_map_e4m3(CUtensorMap* map, const void* base, int64_t rows, int64_t K, int box_rows) {
+  PFN_encodeTiled enc = get_encode_tiled();
+  if (enc == nullptr) return fail(MB200_E_CUDA, "cuTensorMapEncodeTiled entry point not available");
+  const cuuint64_t dims[2] = {(cuuint64_t)K, (cuuint64_t)rows};
+  const cuuint64_t strides[1] = {(cuuint64_t)K};
+  const cuuint32_t box[2] = {(cuuint32_t)TG_BK, (cuuint32_t)box_rows};
+  const cuuint32_t estr[2] = {1, 1};
+  const CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                         CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) return fail(MB200_E_CUDA, "cuTensorMapEncodeTiled (e4m3) failed (%d) rows=%lld K=%lld", (int)r, (long long)rows, (long long)K);
   return MB200_OK;
 }
 

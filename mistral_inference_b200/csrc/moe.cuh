@@ -341,34 +341,98 @@ __global__ void __launch_bounds__(128) moe_combine_kernel(const MoeCombineParams
   }
 }
 
+// ---- FP8 expert weights: row-wise e4m3 quantiser, one CTA per row ----------------------------------------------------------------
+// s[n] = fp32(amax[n] / 448) (1 for an all-zero row), q[n, k] = e4m3_rn_satfinite(fp32(W[n, k] / s[n])): IEEE divisions (the library
+// is built without fast math), cvt.rn.satfinite.e4m3x2.f32 clamps to +-448 like the contract's clamp.  q rows land q_stride bytes
+// apart and scales scale_stride floats apart, so w1 / w3 fill the interleaved rows of the packed gate/up matrix directly.
+__global__ void __launch_bounds__(256) quantize_e4m3_rows_kernel(const uint4* __restrict__ w, int K, uint8_t* __restrict__ q, int64_t q_stride,
+                                                                 float* __restrict__ scale, int64_t scale_stride) {
+  const int n = blockIdx.x, chunks = K >> 3;
+  const uint4* row = w + (int64_t)n * chunks;
+  float amax = 0.f;
+  for (int c = threadIdx.x; c < chunks; c += 256) {
+    const uint4 v = row[c];
+    const uint32_t u[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+    for (int j = 0; j < 4; ++j) amax = fmaxf(amax, fmaxf(fabsf(bf16lo(u[j])), fabsf(bf16hi(u[j]))));
+  }
+  __shared__ float part[8];
+  amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, 16));
+  amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, 8));
+  amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, 4));
+  amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, 2));
+  amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, 1));
+  if ((threadIdx.x & 31) == 0) part[threadIdx.x >> 5] = amax;
+  __syncthreads();
+  amax = part[0];
+#pragma unroll
+  for (int i = 1; i < 8; ++i) amax = fmaxf(amax, part[i]);
+  const float s = amax == 0.f ? 1.f : __fdiv_rn(amax, 448.f);
+  if (threadIdx.x == 0) scale[(int64_t)n * scale_stride] = s;
+  uint2* qrow = reinterpret_cast<uint2*>(q + (int64_t)n * q_stride);
+  for (int c = threadIdx.x; c < chunks; c += 256) {
+    const uint4 v = row[c];
+    const uint32_t u[4] = {v.x, v.y, v.z, v.w};
+    uint32_t o[2] = {0u, 0u};
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const float2 f = make_float2(__fdiv_rn(bf16lo(u[j]), s), __fdiv_rn(bf16hi(u[j]), s));
+      o[j >> 1] |= (uint32_t)__nv_cvt_float2_to_fp8x2(f, __NV_SATFINITE, __NV_E4M3) << (16 * (j & 1));
+    }
+    qrow[c] = make_uint2(o[0], o[1]);
+  }
+}
+
 // ---- host side -------------------------------------------------------------------------------------------------------------
 inline int moe_tile_rows(int64_t T) { return T <= 32 ? 32 : (T <= 64 ? 64 : 128); }  // an expert gets at most one row per token: decode batches fit ONE short m tile
 inline int64_t moe_tile_cap(int64_t pairs, int64_t E, int tile_rows) { return (pairs + tile_rows - 1) / tile_rows + E; }
 inline int64_t moe_plan_words(int64_t pairs, int64_t E, int tile_rows) { return MOE_PLAN_HEADER + 4 * moe_tile_cap(pairs, E, tile_rows); }
 inline int64_t moe_row_cap(int64_t pairs, int64_t E, int tile_rows) { return moe_tile_cap(pairs, E, tile_rows) * tile_rows; }
 
+// Tensor maps of the experts' weights (bf16, or e4m3 when `scales` is given) and their scale table; an expert of another rank
+// (NULL) gets a placeholder that this rank's tiles never reference.
+inline int moe_weight_maps(MoeWeightMaps* maps, MoeWeightScales* sc, const CUtensorMap& placeholder, const void* const* w_host,
+                           const float* const* scales, int E, int64_t N, int64_t K, int box_rows) {
+  for (int e = 0; e < MOE_MAX_EXPERTS; ++e) {
+    const void* w = e < E && w_host[e] != nullptr ? w_host[e] : nullptr;
+    sc->s[e] = w != nullptr && scales != nullptr ? scales[e] : nullptr;
+    if (w == nullptr) {
+      maps->m[e] = placeholder;
+      continue;
+    }
+    if (scales != nullptr && scales[e] == nullptr) return fail(MB200_E_INVALID, "grouped gemm: expert %d has e4m3 weights but no scales", e);
+    const int rc = scales ? make_tensor_map_e4m3(&maps->m[e], w, N, K, box_rows) : make_tensor_map_2d(&maps->m[e], w, N, K, box_rows);
+    if (rc) return rc;
+  }
+  return MB200_OK;
+}
+
+// FP8 (`scales` given): gemm_wgmma_grouped_fp8_kernel, always one CTA per tile (CL = 1): in a cluster pair each CTA would have to
+// convert the whole multicast tile, and the e4m3 tile already halves the L2 -> SM bytes that the multicast saves a third of.
 template <int MODE, int BN, int TA, int CL = 1>
 int launch_grouped_bn(const void* a, int64_t rows_cap, int64_t K, int64_t N, const void* const* w_host, int E, const int32_t* plan, const EpiParams& epi,
-                      int sms, cudaStream_t stream) {
+                      int sms, cudaStream_t stream, const float* const* scales = nullptr) {
   using Cfg = TgCfg<BN, TA>;
   CUtensorMap map_a;
   MoeWeightMaps maps;
+  MoeWeightScales sc;
   int rc = make_tensor_map_2d(&map_a, a, rows_cap, K, TA);
   if (rc) return rc;
-  for (int e = 0; e < MOE_MAX_EXPERTS; ++e) {
-    const void* w = e < E && w_host[e] != nullptr ? w_host[e] : nullptr;
-    if (w == nullptr) {  // an expert of another rank: never referenced by this rank's tiles
-      maps.m[e] = map_a;
-      continue;
-    }
-    rc = make_tensor_map_2d(&maps.m[e], w, N, K, BN / CL);  // cluster pairs: each CTA fetches half of the W tile and multicasts it
-    if (rc) return rc;
-  }
+  rc = moe_weight_maps(&maps, &sc, map_a, w_host, scales, E, N, K, scales ? BN : BN / CL);  // cluster pairs: each CTA fetches half of the W tile and multicasts it
+  if (rc) return rc;
   TcGemmParams p;
   p.T = (int)rows_cap;
   p.N = (int)N;
   p.K = (int)K;
   p.epi = epi;
+  if (scales != nullptr) {
+    using Cfg8 = TgCfg<BN, TA, true>;
+    MB_CHECK_CUDA(cudaFuncSetAttribute(gemm_wgmma_grouped_fp8_kernel<MODE, BN, TA>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg8::kSmem));
+    gemm_wgmma_grouped_fp8_kernel<MODE, BN, TA><<<sms, Cfg8::kThreads, Cfg8::kSmem, stream>>>(map_a, maps, sc, p, plan);
+    MB_CHECK_LAUNCH("gemm_wgmma_grouped_fp8_kernel");
+    note_launch("gemm_wgmma_grouped_fp8_kernel<%d, 1, %d, %d>", MODE, BN, TA);
+    return MB200_OK;
+  }
   MB_CHECK_CUDA(cudaFuncSetAttribute(gemm_wgmma_grouped_kernel<MODE, CL, BN, TA>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmem));
   if (CL == 1) {
     gemm_wgmma_grouped_kernel<MODE, CL, BN, TA><<<sms, Cfg::kThreads, Cfg::kSmem, stream>>>(map_a, maps, p, plan);
@@ -399,23 +463,18 @@ int launch_grouped_bn(const void* a, int64_t rows_cap, int64_t K, int64_t N, con
 // decode-sized calls: the stream-K weight-streaming kernel over (expert segment, n tile, k block) units
 template <int MODE, int TA>
 int launch_grouped_streamk(const void* a, int64_t rows_cap, int64_t K, int64_t N, const void* const* w_host, int E, const int32_t* plan,
-                           const EpiParams& epi, void* workspace, size_t workspace_bytes, int sms, cudaStream_t stream) {
+                           const EpiParams& epi, void* workspace, size_t workspace_bytes, int sms, cudaStream_t stream,
+                           const float* const* scales = nullptr) {
   using Cfg = TgCfg<SK_BN, TA>;
   if (sms > SK_MAX_CTAS) sms = SK_MAX_CTAS;
   if (workspace == nullptr || workspace_bytes < kWsSkPartials.end()) return fail(MB200_E_WORKSPACE, "grouped stream-K gemm: workspace %zu < %zu", workspace_bytes, kWsSkPartials.end());
   CUtensorMap map_a;
   MoeWeightMaps maps;
+  MoeWeightScales sc;
   int rc = make_tensor_map_2d(&map_a, a, rows_cap, K, TA);
   if (rc) return rc;
-  for (int e = 0; e < MOE_MAX_EXPERTS; ++e) {
-    const void* w = e < E && w_host[e] != nullptr ? w_host[e] : nullptr;
-    if (w == nullptr) {
-      maps.m[e] = map_a;
-      continue;
-    }
-    rc = make_tensor_map_2d(&maps.m[e], w, N, K, SK_BN);
-    if (rc) return rc;
-  }
+  rc = moe_weight_maps(&maps, &sc, map_a, w_host, scales, E, N, K, SK_BN);
+  if (rc) return rc;
   SkParams p;
   p.T = (int)rows_cap;
   p.N = (int)N;
@@ -423,6 +482,14 @@ int launch_grouped_streamk(const void* a, int64_t rows_cap, int64_t K, int64_t N
   p.epi = epi;
   p.partials = reinterpret_cast<float*>((uint8_t*)workspace + kWsSkPartials.offset);
   p.flags = reinterpret_cast<unsigned*>((uint8_t*)workspace + kWsSkFlags.offset);
+  if (scales != nullptr) {
+    using Cfg8 = TgCfg<SK_BN, TA, true>;
+    MB_CHECK_CUDA(cudaFuncSetAttribute(gemm_streamk_grouped_fp8_kernel<MODE, TA>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg8::kSmem));
+    MB_CHECK_CUDA(launch_pdl(gemm_streamk_grouped_fp8_kernel<MODE, TA>, dim3((unsigned)sms), dim3(Cfg8::kThreads), (size_t)Cfg8::kSmem, stream, map_a, maps,
+                             sc, p, plan));
+    note_launch("gemm_streamk_grouped_fp8_kernel<%d, %d>", MODE, TA);
+    return MB200_OK;
+  }
   MB_CHECK_CUDA(cudaFuncSetAttribute(gemm_streamk_grouped_kernel<MODE, TA>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmem));
   MB_CHECK_CUDA(launch_pdl(gemm_streamk_grouped_kernel<MODE, TA>, dim3((unsigned)sms), dim3(Cfg::kThreads), (size_t)Cfg::kSmem, stream, map_a, maps, p, plan));
   note_launch("gemm_streamk_grouped_kernel<%d, %d>", MODE, TA);
@@ -431,23 +498,24 @@ int launch_grouped_streamk(const void* a, int64_t rows_cap, int64_t K, int64_t N
 
 template <int MODE>
 int launch_grouped(const void* a, int64_t rows_cap, int64_t K, int64_t N, const void* const* w_host, int E, int est_mtiles, int tile_rows,
-                   const int32_t* plan, const EpiParams& epi, void* workspace, size_t workspace_bytes, cudaStream_t stream) {
+                   const int32_t* plan, const EpiParams& epi, void* workspace, size_t workspace_bytes, cudaStream_t stream,
+                   const float* const* scales = nullptr) {
   int dev = 0, sms = 0;
   MB_CHECK_CUDA(cudaGetDevice(&dev));
   MB_CHECK_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   MB_CHECK_ARG(K % TG_BK == 0 && N % 32 == 0, "grouped gemm: K=%lld must be a multiple of 64, N=%lld of 32", (long long)K, (long long)N);
   if (tile_rows < 128 && streamk_eligible(tile_rows, N, K)) {
-    if (tile_rows == 32) return launch_grouped_streamk<MODE, 32>(a, rows_cap, K, N, w_host, E, plan, epi, workspace, workspace_bytes, sms, stream);
-    return launch_grouped_streamk<MODE, 64>(a, rows_cap, K, N, w_host, E, plan, epi, workspace, workspace_bytes, sms, stream);
+    if (tile_rows == 32) return launch_grouped_streamk<MODE, 32>(a, rows_cap, K, N, w_host, E, plan, epi, workspace, workspace_bytes, sms, stream, scales);
+    return launch_grouped_streamk<MODE, 64>(a, rows_cap, K, N, w_host, E, plan, epi, workspace, workspace_bytes, sms, stream, scales);
   }
   if (tile_rows == 128) {
     // enough rows per expert for vertically adjacent tile pairs: the 2-CTA cluster kernel (W tile multicast, 2/3 of the L2 -> SM traffic)
-    if (N % 256 == 0 && wgmma_cluster_enabled() && rows_cap >= (int64_t)E * 512)
-      return launch_grouped_bn<MODE, 256, 128, 2>(a, rows_cap, K, N, w_host, E, plan, epi, sms, stream);
-    if (N % 256 == 0) return launch_grouped_bn<MODE, 256, 128>(a, rows_cap, K, N, w_host, E, plan, epi, sms, stream);
-    if (N % 128 == 0) return launch_grouped_bn<MODE, 128, 128>(a, rows_cap, K, N, w_host, E, plan, epi, sms, stream);
-    if (N % 64 == 0) return launch_grouped_bn<MODE, 64, 128>(a, rows_cap, K, N, w_host, E, plan, epi, sms, stream);
-    return launch_grouped_bn<MODE, 32, 128>(a, rows_cap, K, N, w_host, E, plan, epi, sms, stream);
+    if (N % 256 == 0 && scales == nullptr && wgmma_cluster_enabled() && rows_cap >= (int64_t)E * 512)
+      return launch_grouped_bn<MODE, 256, 128, 2>(a, rows_cap, K, N, w_host, E, plan, epi, sms, stream, scales);
+    if (N % 256 == 0) return launch_grouped_bn<MODE, 256, 128>(a, rows_cap, K, N, w_host, E, plan, epi, sms, stream, scales);
+    if (N % 128 == 0) return launch_grouped_bn<MODE, 128, 128>(a, rows_cap, K, N, w_host, E, plan, epi, sms, stream, scales);
+    if (N % 64 == 0) return launch_grouped_bn<MODE, 64, 128>(a, rows_cap, K, N, w_host, E, plan, epi, sms, stream, scales);
+    return launch_grouped_bn<MODE, 32, 128>(a, rows_cap, K, N, w_host, E, plan, epi, sms, stream, scales);
   }
   int best = 32;
   double best_score = -1.0;
@@ -469,17 +537,17 @@ int launch_grouped(const void* a, int64_t rows_cap, int64_t K, int64_t N, const 
   }
   if (tile_rows == 64) {
     switch (best) {
-      case 256: return launch_grouped_bn<MODE, 256, 64>(a, rows_cap, K, N, w_host, E, plan, epi, sms, stream);
-      case 128: return launch_grouped_bn<MODE, 128, 64>(a, rows_cap, K, N, w_host, E, plan, epi, sms, stream);
-      case 64: return launch_grouped_bn<MODE, 64, 64>(a, rows_cap, K, N, w_host, E, plan, epi, sms, stream);
-      default: return launch_grouped_bn<MODE, 32, 64>(a, rows_cap, K, N, w_host, E, plan, epi, sms, stream);
+      case 256: return launch_grouped_bn<MODE, 256, 64>(a, rows_cap, K, N, w_host, E, plan, epi, sms, stream, scales);
+      case 128: return launch_grouped_bn<MODE, 128, 64>(a, rows_cap, K, N, w_host, E, plan, epi, sms, stream, scales);
+      case 64: return launch_grouped_bn<MODE, 64, 64>(a, rows_cap, K, N, w_host, E, plan, epi, sms, stream, scales);
+      default: return launch_grouped_bn<MODE, 32, 64>(a, rows_cap, K, N, w_host, E, plan, epi, sms, stream, scales);
     }
   }
   switch (best) {
-    case 256: return launch_grouped_bn<MODE, 256, 32>(a, rows_cap, K, N, w_host, E, plan, epi, sms, stream);
-    case 128: return launch_grouped_bn<MODE, 128, 32>(a, rows_cap, K, N, w_host, E, plan, epi, sms, stream);
-    case 64: return launch_grouped_bn<MODE, 64, 32>(a, rows_cap, K, N, w_host, E, plan, epi, sms, stream);
-    default: return launch_grouped_bn<MODE, 32, 32>(a, rows_cap, K, N, w_host, E, plan, epi, sms, stream);
+    case 256: return launch_grouped_bn<MODE, 256, 32>(a, rows_cap, K, N, w_host, E, plan, epi, sms, stream, scales);
+    case 128: return launch_grouped_bn<MODE, 128, 32>(a, rows_cap, K, N, w_host, E, plan, epi, sms, stream, scales);
+    case 64: return launch_grouped_bn<MODE, 64, 32>(a, rows_cap, K, N, w_host, E, plan, epi, sms, stream, scales);
+    default: return launch_grouped_bn<MODE, 32, 32>(a, rows_cap, K, N, w_host, E, plan, epi, sms, stream, scales);
   }
 }
 

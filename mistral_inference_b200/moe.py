@@ -37,6 +37,55 @@ class _GateView:
         return self._layer.gate_weight
 
 
+EXPERT_WEIGHTS = ("bf16", "fp8")
+
+
+class Fp8Expert(nn.Module):
+    """One expert with FP8 (e4m3) weights, the storage format of include/mistral_b200.h: `w13_q` [2*hidden, dim] (row 2i = w1[i],
+    row 2i + 1 = w3[i], like FeedForward.w13) and `w2_q` [dim, hidden] hold the e4m3 bit patterns as uint8, with one fp32 scale
+    per row.  The scales are stored as their int32 bit patterns (`w13_scale` / `w2_scale` are the fp32 views): `Module.to(dtype)`
+    casts every floating tensor, and these must keep their bits.  Weights arrive as bf16 and are quantised in place on the device."""
+
+    def __init__(self, dim: int, hidden_dim: int):
+        super().__init__()
+        self.dim = dim
+        self.hidden_dim = hidden_dim
+        self.w13_q = nn.Parameter(torch.empty(2 * hidden_dim, dim, dtype=torch.uint8), requires_grad=False)
+        self.w2_q = nn.Parameter(torch.empty(dim, hidden_dim, dtype=torch.uint8), requires_grad=False)
+        self.w13_scale_bits = nn.Parameter(torch.empty(2 * hidden_dim, dtype=torch.int32), requires_grad=False)
+        self.w2_scale_bits = nn.Parameter(torch.empty(dim, dtype=torch.int32), requires_grad=False)
+
+    @property
+    def w13_scale(self) -> torch.Tensor:
+        return self.w13_scale_bits.view(torch.float32)
+
+    @property
+    def w2_scale(self) -> torch.Tensor:
+        return self.w2_scale_bits.view(torch.float32)
+
+    def _slots(self, name: str) -> Tuple[torch.Tensor, torch.Tensor]:
+        """(q rows, scale entries) of the reference Linear `name` (w1, w2 or w3): zero-copy, strided for w1 / w3."""
+        h, d = self.hidden_dim, self.dim
+        if name in ("w1", "w3"):
+            seg = 0 if name == "w1" else 1
+            return self.w13_q.view(h, 2, d)[:, seg], self.w13_scale.view(h, 2)[:, seg]
+        if name == "w2":
+            return self.w2_q, self.w2_scale
+        raise ValueError(f"expert Linear {name!r}")
+
+    def weight_e4m3(self, name: str) -> torch.Tensor:
+        return self._slots(name)[0].view(torch.float8_e4m3fn)
+
+    def weight_scale(self, name: str) -> torch.Tensor:
+        return self._slots(name)[1]
+
+    def quantize_(self, name: str, w: torch.Tensor) -> None:
+        """Quantises the bf16 weight `w` of Linear `name` into place (one bf16 copy of `w` on the device while it runs)."""
+        q, s = self._slots(name)
+        assert tuple(w.shape) == tuple(q.shape), f"{name}: shape {tuple(w.shape)} != expected {tuple(q.shape)}"
+        _abi.quantize_e4m3_rows(w.to(device=q.device, dtype=torch.bfloat16).contiguous(), q, s)
+
+
 class MoeBuffers:
     """Row buffers of one MoE call for up to `T` tokens (shared by all layers of a model; sizes from mb200_moe_sizes)."""
 
@@ -138,18 +187,26 @@ class MoeLayer(nn.Module):
     def sharded(self) -> bool:
         return self.expert_shard[1] > 1
 
+    @property
+    def fp8(self) -> bool:
+        return isinstance(self.experts[str(self.local_expert_ids[0])], Fp8Expert)
+
     def _weight_tables(self):
-        """HOST arrays of E device pointers (NULL for experts of other ranks), rebuilt when a weight moved."""
+        """HOST arrays of E device pointers (NULL for experts of other ranks), rebuilt when a weight moved: (w13, w2), and for FP8
+        experts (w13_q, w13 scales, w2_q, w2 scales)."""
         E = self.args.num_experts
-        key = tuple((e, self.experts[str(e)].w13.data_ptr(), self.experts[str(e)].w2_weight.data_ptr()) for e in self.local_expert_ids)
+        if self.fp8:
+            tensors = lambda ex: (ex.w13_q, ex.w13_scale_bits, ex.w2_q, ex.w2_scale_bits)  # noqa: E731
+        else:
+            tensors = lambda ex: (ex.w13, ex.w2_weight)  # noqa: E731
+        key = tuple((e, *(t.data_ptr() for t in tensors(self.experts[str(e)]))) for e in self.local_expert_ids)
         if self._ptrs is None or self._ptrs[0] != key:
-            w13 = (ctypes.c_void_p * E)()
-            w2 = (ctypes.c_void_p * E)()
+            tables = [(ctypes.c_void_p * E)() for _ in key[0][1:]]
             for e in self.local_expert_ids:
-                w13[e] = self.experts[str(e)].w13.data_ptr()
-                w2[e] = self.experts[str(e)].w2_weight.data_ptr()
-            self._ptrs = (key, w13, w2)
-        return self._ptrs[1], self._ptrs[2]
+                for tab, t in zip(tables, tensors(self.experts[str(e)])):
+                    tab[e] = t.data_ptr()
+            self._ptrs = (key, tables)
+        return self._ptrs[1]
 
     def run(self, hn: torch.Tensor, residual: Optional[torch.Tensor], ws: "_abi.Workspace") -> torch.Tensor:
         """`hn` = ffn_norm(h) [T, dim]; returns residual + moe(hn) (or moe(hn) when residual is None)."""
@@ -157,7 +214,7 @@ class MoeLayer(nn.Module):
         first = self.experts[str(self.local_expert_ids[0])]
         E, k = self.args.num_experts, self.args.num_experts_per_tok
         out = torch.empty_like(hn)
-        w13, w2 = self._weight_tables()
+        tables = self._weight_tables()
         g, G = self.expert_shard
         for r0 in range(0, T, MOE_BLOCK_TOKENS):
             r1 = min(T, r0 + MOE_BLOCK_TOKENS)
@@ -166,8 +223,12 @@ class MoeLayer(nn.Module):
             b = ws.moe_buffers(n, dim, first.hidden_dim, E, k, hn.dtype, comm, self.layer_parity)
             assert comm is None or b.rows_cap <= comm.rows_cap
             _abi.moe_route(hn[r0:r1], self.gate_weight, E, k, g, G, b)
-            _abi.moe_grouped_ffn(b, w13, w2, residual[r0:r1] if residual is not None else None, out[r0:r1], n, dim, first.hidden_dim, E, k,
-                                 comm.struct(self.layer_parity) if comm is not None else None, ws)
+            res = residual[r0:r1] if residual is not None else None
+            cs = comm.struct(self.layer_parity) if comm is not None else None
+            if len(tables) == 4:
+                _abi.moe_grouped_ffn_fp8(b, *tables, res, out[r0:r1], n, dim, first.hidden_dim, E, k, cs, ws)
+            else:
+                _abi.moe_grouped_ffn(b, *tables, res, out[r0:r1], n, dim, first.hidden_dim, E, k, cs, ws)
         return out
 
     def forward(self, inputs: torch.Tensor, ws: Optional["_abi.Workspace"] = None) -> torch.Tensor:

@@ -18,6 +18,7 @@ from . import _abi
 from .args import PATCH_MERGE, TransformerArgs
 from .cache import BufferCache, CacheInputMetadata
 from .rope import precompute_freqs_cis
+from .moe import EXPERT_WEIGHTS, Fp8Expert
 from .transformer_layers import LoraAdapter, RMSNorm, TransformerBlock
 from .vision_encoder import PatchMerger, VisionLanguageAdapter, VisionTransformer
 
@@ -58,11 +59,18 @@ class _OutputView:
 
 class Transformer(nn.Module):
     def __init__(self, args: TransformerArgs, pipeline_rank: int = 0, num_pipeline_ranks: int = 1, softmax_fp32: bool = True,
-                 expert_parallel: Optional[Tuple[int, int]] = None, expert_group: Any = None):
+                 expert_parallel: Optional[Tuple[int, int]] = None, expert_group: Any = None, expert_weights: str = "bf16"):
         """Same signature as the reference (transformer.py:34-40) plus `expert_parallel = (rank, world)`: MoE experts sharded
         `e % world == rank` over the ranks of `expert_group` (default process group), everything else replicated, one
-        all-reduce of [T, dim] per MoE layer (SURVEY.md 8e)."""
+        all-reduce of [T, dim] per MoE layer (SURVEY.md 8e); and `expert_weights`: "bf16", or "fp8" to store every MoE expert
+        matrix as e4m3 with one fp32 scale per row (moe.Fp8Expert; the model then computes exactly what the bf16 model computes
+        with the dequantised weights W', see include/mistral_b200.h)."""
         super().__init__()
+        if expert_weights not in EXPERT_WEIGHTS:
+            raise ValueError(f"expert_weights={expert_weights!r}: expected one of {EXPERT_WEIGHTS}")
+        if expert_weights == "fp8" and args.moe is None:
+            raise ValueError("expert_weights='fp8' needs a mixture-of-experts model: only the grouped expert GEMMs read FP8 weights")
+        self.expert_weights = expert_weights
         if args.lora is not None and args.moe is not None:
             raise NotImplementedError("un-merged LoRA on mixture-of-experts layers is not built: the grouped expert GEMMs have no "
                                       "LoRA stage (merge the adapter instead: args.lora = None, then load_lora)")
@@ -109,7 +117,7 @@ class Transformer(nn.Module):
         self.layers = nn.ModuleDict({
             str(i): TransformerBlock(dim=args.dim, hidden_dim=args.hidden_dim, n_heads=args.n_heads, n_kv_heads=args.n_kv_heads,
                                      head_dim=args.head_dim, norm_eps=args.norm_eps, lora=args.lora, moe=args.moe,
-                                     expert_shard=self.expert_parallel, expert_group=expert_group)
+                                     expert_shard=self.expert_parallel, expert_group=expert_group, expert_weights=expert_weights)
             for i in range(offset, end)
         })
         self.n_local_layers = len(self.layers)
@@ -305,11 +313,12 @@ class Transformer(nn.Module):
                 and len(set(cache.cache_sizes)) <= 8)
 
     def _megakernel_ok(self, B: int) -> bool:
-        # the megakernel has no LoRA stage: with un-merged adapters batch 1 takes the per-layer graph path
+        # the megakernel has no LoRA stage and reads bf16 experts only: with un-merged adapters or FP8 experts batch 1 takes the
+        # per-layer graph path
         # the shape limits (head ratio, K chunking, KV <= 8, MoE sizes, a shared-memory ring of >= 9 stages next to the
         # activations) are the library's, asked once per model: a model it refuses takes the per-layer path
         if not (B == 1 and self.num_pipeline_ranks == 1 and self.expert_parallel[1] == 1 and self.args.lora is None
-                and os.environ.get("MB200_MEGAKERNEL", "1") != "0"):
+                and self.expert_weights == "bf16" and os.environ.get("MB200_MEGAKERNEL", "1") != "0"):
             return False
         if self._megakernel_refused is None:
             a, moe = self.args, self.args.moe
@@ -568,6 +577,12 @@ class Transformer(nn.Module):
                     return False  # an expert owned by another expert-parallel rank
                 ff = ff.experts[parts[2]]
                 parts = parts[2:]
+                if isinstance(ff, Fp8Expert):  # the reference's bf16 weight, quantised into place
+                    if parts[2:] != ["weight"] or parts[1] not in ("w1", "w2", "w3"):
+                        raise ValueError(f"Unexpected key {k}")
+                    name = parts[1]
+                    put(ff.weight_e4m3(name), lambda _seg, w: ff.quantize_(name, w))
+                    return True
             name = parts[1]
             if name == "w1":
                 put(ff.w13.view(ff.hidden_dim, 2, ff.dim)[:, 0])
@@ -644,7 +659,9 @@ class Transformer(nn.Module):
         adapters may be absent (they stay zero); the reference's post-hook clears every missing key (lora.py:66-69), this keeps
         the base weights strict."""
         if self.args.lora is None:
-            return set(self.reference_keys()) - set(loaded)
+            # an FP8 expert's `X.weight_e4m3` and `X.weight_scale` are both set by the reference's `X.weight`
+            have = set(loaded) | {k[: -len(".weight")] + sfx for k in loaded for sfx in (".weight_e4m3", ".weight_scale")}
+            return set(self.reference_keys()) - have
         have = set(loaded) | {k[: -len(".weight")] + ".linear.weight" for k in loaded}
         return {k for k in self.reference_keys() if k not in have and not k.endswith((".lora_A.weight", ".lora_B.weight"))}
 
@@ -687,7 +704,11 @@ class Transformer(nn.Module):
             out[p + "feed_forward.gate.weight"] = ff.gate_weight
             for e, ex in ff.experts.items():  # keyed by the global expert id; the local ones only when sharded
                 for n in ("w1", "w2", "w3"):
-                    out[p + f"feed_forward.experts.{e}.{n}.weight"] = getattr(ex, n).weight
+                    if isinstance(ex, Fp8Expert):  # the stored format itself: no dequantised copies
+                        out[p + f"feed_forward.experts.{e}.{n}.weight_e4m3"] = ex.weight_e4m3(n)
+                        out[p + f"feed_forward.experts.{e}.{n}.weight_scale"] = ex.weight_scale(n)
+                    else:
+                        out[p + f"feed_forward.experts.{e}.{n}.weight"] = getattr(ex, n).weight
         else:
             for n in ("w1", "w2", "w3"):
                 Transformer._linear_state(out, p, blk, "feed_forward." + n, getattr(ff, n).weight)
@@ -725,6 +746,9 @@ class Transformer(nn.Module):
         lora_dtype = lora_dtypes.pop()
         assert lora_dtype == self.dtype, f"LoRA weights dtype differs from model's dtype {lora_dtype} != {self.dtype}"
         assert all("lora" in key for key in lora_state_dict.keys())
+        if self.expert_weights == "fp8" and any(".experts." in key for key in lora_state_dict):
+            raise NotImplementedError("merging a LoRA adapter into FP8 expert weights is not built: the experts are stored quantised "
+                                      "(load the adapter into a bf16 model, or drop its expert Linears)")
         lora_state_dict = {k: v.to(self.device) for k, v in lora_state_dict.items()}
         if self.args.lora is not None:
             with torch.no_grad():
@@ -764,9 +788,11 @@ class Transformer(nn.Module):
     @staticmethod
     def from_folder(folder: Union[Path, str], max_batch_size: int = 1, num_pipeline_ranks: int = 1,
                     device: Union[torch.device, str] = "cuda", dtype: Optional[torch.dtype] = None,
-                    softmax_fp32: bool = True, expert_parallel: Optional[Tuple[int, int]] = None, expert_group: Any = None) -> "Transformer":
+                    softmax_fp32: bool = True, expert_parallel: Optional[Tuple[int, int]] = None, expert_group: Any = None,
+                    expert_weights: str = "bf16") -> "Transformer":
         """transformer.py:297-338.  Tensors stream from disk straight into the packed device buffers; with `expert_parallel`
-        the experts of other ranks are skipped (never read into device memory)."""
+        the experts of other ranks are skipped (never read into device memory).  With expert_weights="fp8" each bf16 expert
+        tensor is copied to the device and quantised into place: the peak is the FP8 model plus about one bf16 tensor."""
         with open(Path(folder) / "params.json", "r") as f:
             model_args = TransformerArgs.from_dict(json.load(f))
         model_args.max_batch_size = max_batch_size
@@ -785,7 +811,8 @@ class Transformer(nn.Module):
             # shapes on `meta`, storage allocated ONCE, directly in the target dtype on the target device (the reference builds
             # on meta and assigns, transformer.py:321-331; a fp32 build followed by .to(bf16) would need 3x the model's bytes)
             return Transformer.empty(model_args, dev, dtype or ck_dtype, pipeline_rank=pipeline_rank, num_pipeline_ranks=num_pipeline_ranks,
-                                     softmax_fp32=softmax_fp32, expert_parallel=expert_parallel, expert_group=expert_group)
+                                     softmax_fp32=softmax_fp32, expert_parallel=expert_parallel, expert_group=expert_group,
+                                     expert_weights=expert_weights)
 
         if pt_model_file.exists():
             loaded = torch.load(str(pt_model_file), mmap=True)

@@ -15,7 +15,7 @@ from torch import nn
 from . import _abi
 from .args import LoraArgs, MoeArgs
 from .cache import CacheView
-from .moe import MoeLayer
+from .moe import Fp8Expert, MoeLayer
 
 
 class _WeightView:
@@ -235,7 +235,8 @@ class TransformerBlock(nn.Module):
     """transformer_layers.py:123-169: pre-norm residual wiring; FeedForward or MoeLayer."""
 
     def __init__(self, dim: int, hidden_dim: int, n_heads: int, n_kv_heads: int, head_dim: int, norm_eps: float,
-                 lora: Optional[LoraArgs] = None, moe: Optional[MoeArgs] = None, expert_shard: Tuple[int, int] = (0, 1), expert_group=None):
+                 lora: Optional[LoraArgs] = None, moe: Optional[MoeArgs] = None, expert_shard: Tuple[int, int] = (0, 1), expert_group=None,
+                 expert_weights: str = "bf16"):
         super().__init__()
         if lora is not None and moe is not None:
             raise NotImplementedError("un-merged LoRA on mixture-of-experts layers is not built: the grouped expert GEMMs have no "
@@ -249,7 +250,8 @@ class TransformerBlock(nn.Module):
         self.feed_forward: nn.Module
         if moe is not None:
             g, G = expert_shard  # this rank allocates only the experts it owns (e % G == g): SURVEY.md 8(e)
-            self.feed_forward = MoeLayer(experts={e: FeedForward(dim=dim, hidden_dim=hidden_dim, lora=lora) for e in range(moe.num_experts) if e % G == g},
+            expert = (lambda: Fp8Expert(dim, hidden_dim)) if expert_weights == "fp8" else (lambda: FeedForward(dim=dim, hidden_dim=hidden_dim, lora=lora))
+            self.feed_forward = MoeLayer(experts={e: expert() for e in range(moe.num_experts) if e % G == g},
                                          gate_weight=nn.Parameter(torch.empty(moe.num_experts, dim), requires_grad=False), moe_args=moe,
                                          expert_shard=expert_shard, expert_group=expert_group)
         else:
