@@ -30,7 +30,7 @@
 extern "C" {
 #endif
 
-#define MB200_ABI_VERSION 1
+#define MB200_ABI_VERSION 2
 
 #define MB200_OK 0
 #define MB200_E_INVALID (-1)   /* bad argument / unsupported shape */
@@ -109,6 +109,40 @@ int mb200_attn_decode(const void* q, const void* cache_k, const void* cache_v, c
 int mb200_attn_prefill(const void* q, const void* k_new, const void* v_new, const void* cache_k, const void* cache_v,
                        const int32_t* q_start, const int32_t* seqpos, void* out, int64_t T, int64_t B, int64_t max_seqlen,
                        int64_t W, int64_t n_heads, int64_t n_kv_heads, int64_t head_dim, int causal, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * FP8 (e4m3) KV cache (Python: BufferCache(..., kv_cache="fp8"), Transformer(..., kv_cache="fp8")).  A storage format with an
+ * exact definition, not a new numeric path.  Per layer the ring holds, for each (slot, kv head) row x of hd = 128 bf16 values,
+ * 128 e4m3 bytes q in cache_k / cache_v [max_batch, W, KV, hd] and one int8 exponent e in exp_k / exp_v [max_batch, W, KV]:
+ *   e    = max(-124, smallest integer with amax|x| <= 448 * 2^e)      (all-zero row: -124)
+ *   q[i] = e4m3fn_rn(fp32(x[i]) * 2^-e)                               (2^-e scales exactly; one rounding, |q| <= 448)
+ *   x'   = q * 2^e                                                    (exact in bf16; -0 stays -0)
+ * The FP8-cache model is the bf16 model with k <- k', v <- v' inserted right after RoPE in every forward that has a cache:
+ * attention sees only k' and v', from the ring in decode, from the chunk in first prefill, from both in chunked prefill.
+ * The -124 clamp makes the smallest e4m3 subnormal (2^-9) times 2^e the smallest bf16 subnormal, so every x' is a bf16 value.
+ * Rows with |x| >= 2^127 are outside the format (their amax can round up to 2^128).  Projection: quantising x' again returns x'
+ * (the bytes may differ: a largest |q| of exactly 224 re-quantises as e - 1 and 2q), so prefill quantises k / v in place before
+ * attention and writes the ring from k' / v' afterwards.  The readers rebuild the bf16 bits of x' exactly, so
+ * mb200_attn_decode_fp8 and mb200_attn_prefill_fp8 are bit-identical to mb200_attn_decode / mb200_attn_prefill on a bf16 ring
+ * that holds x'.  head_dim 128 only.
+ *
+ * mb200_kv_quantize: k, v [T, KV*hd] bf16.  write_back != 0: k, v <- k', v' in place.  cache_rows [T] int32 (or NULL): for
+ *   cache_rows[t] >= 0, (q, e) of token t go to ring row cache_rows[t] (slot + b*W, as mb200_kv_ring_write).  Decode: ring only;
+ *   prefill: in place before attention, then ring only from k' / v' after it.
+ * mb200_attn_decode_fp8: mb200_attn_decode reading the e4m3 ring and its exponents.  Workspace: as mb200_attn_decode (the
+ *   e4m3 ring needs no scratch of its own, so mb200_workspace_bytes is unchanged).
+ * mb200_attn_prefill_fp8: mb200_attn_prefill (causal 1 or 2) reading old keys from the e4m3 ring; k_new / v_new must already
+ *   hold k' / v'.  causal = 2 reads no ring row and runs the bf16 kernels.
+ */
+int mb200_kv_quantize(void* k, void* v, int write_back, void* cache_k, void* cache_v, int8_t* exp_k, int8_t* exp_v,
+                      const int32_t* cache_rows, int64_t T, int64_t n_kv_heads, int64_t head_dim, void* stream);
+int mb200_attn_decode_fp8(const void* q, const void* cache_k, const void* cache_v, const int8_t* exp_k, const int8_t* exp_v,
+                          const int32_t* kv_len, void* out, int64_t B, int64_t W, int64_t n_heads, int64_t n_kv_heads,
+                          int64_t head_dim, int64_t n_splits, void* workspace, size_t workspace_bytes, void* stream);
+int mb200_attn_prefill_fp8(const void* q, const void* k_new, const void* v_new, const void* cache_k, const void* cache_v,
+                           const int8_t* exp_k, const int8_t* exp_v, const int32_t* q_start, const int32_t* seqpos, void* out,
+                           int64_t T, int64_t B, int64_t max_seqlen, int64_t W, int64_t n_heads, int64_t n_kv_heads,
+                           int64_t head_dim, int causal, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * out = residual + bf16( x @ W^T )   (bf16 add, one more rounding).

@@ -15,7 +15,7 @@ import torch
 _LIB_PATH = Path(os.environ.get("MB200_LIB_PATH") or Path(__file__).resolve().parent / "libmb200.so")  # override: A/B builds of experiments
 _lib: Optional[ctypes.CDLL] = None
 
-ABI_VERSION = 1
+ABI_VERSION = 2
 SKINNY_MAX_T = 4
 WORKSPACE_HEADER_BYTES = 64 * 1024
 
@@ -32,6 +32,11 @@ _SIGNATURES = {
                                   c_int64, c_void_p, c_size_t, c_void_p]),
     "mb200_attn_prefill": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64,
                                    c_int64, c_int64, c_int64, c_int64, c_int64, c_int, c_void_p]),
+    "mb200_kv_quantize": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_void_p]),
+    "mb200_attn_decode_fp8": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int64,
+                                      c_int64, c_int64, c_void_p, c_size_t, c_void_p]),
+    "mb200_attn_prefill_fp8": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                       c_int64, c_int64, c_int64, c_int64, c_int64, c_int64, c_int64, c_int, c_void_p]),
     "mb200_linear_residual": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_void_p, c_size_t, c_void_p]),
     "mb200_linear_bias": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int, c_void_p, c_size_t, c_void_p]),
     "mb200_vision_patchify": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int64, c_int64, c_void_p]),
@@ -211,6 +216,28 @@ def attn_prefill(q, k_new, v_new, cache_k, cache_v, q_start, seqpos, out, B, max
     _check(lib().mb200_attn_prefill(_ptr(q), _ptr(k_new), _ptr(v_new), _ptr(cache_k), _ptr(cache_v), _ptr(q_start), _ptr(seqpos),
                                     _ptr(out), q.shape[0], B, max_seqlen, W, n_heads, n_kv_heads, head_dim, (2 if first_prefill else 1) if causal else 0,
                                     _stream()), "mb200_attn_prefill")
+
+
+def kv_quantize(k, v, write_back: bool, cache_k=None, cache_v=None, exp_k=None, exp_v=None, cache_rows=None) -> None:
+    """FP8 KV cache (include/mistral_b200.h): k, v [T, KV*hd] bf16 <- k', v' when `write_back`; (q, e) of each token t with
+    cache_rows[t] >= 0 into the e4m3 ring cache_k / cache_v [.., KV, hd] and its int8 exponents exp_k / exp_v [.., KV]."""
+    KV = exp_k.shape[-1] if exp_k is not None else k.shape[1] // 128
+    _check(lib().mb200_kv_quantize(_ptr(k), _ptr(v), int(write_back), _ptr(cache_k), _ptr(cache_v), _ptr(exp_k), _ptr(exp_v), _ptr(cache_rows),
+                                   k.shape[0], KV, k.shape[1] // KV, _stream()), "mb200_kv_quantize")
+
+
+def attn_decode_fp8(q, cache_k, cache_v, exp_k, exp_v, kv_len, out, n_heads, n_kv_heads, head_dim, n_splits, ws: Workspace) -> None:
+    B = q.shape[0]
+    W = cache_k.shape[1]
+    _check(lib().mb200_attn_decode_fp8(_ptr(q), _ptr(cache_k), _ptr(cache_v), _ptr(exp_k), _ptr(exp_v), _ptr(kv_len), _ptr(out), B, W, n_heads,
+                                       n_kv_heads, head_dim, n_splits, ws.ptr, ws.nbytes, _stream()), "mb200_attn_decode_fp8")
+
+
+def attn_prefill_fp8(q, k_new, v_new, cache_k, cache_v, exp_k, exp_v, q_start, seqpos, out, B, max_seqlen, W, n_heads, n_kv_heads, head_dim,
+                     first_prefill: bool = False) -> None:
+    _check(lib().mb200_attn_prefill_fp8(_ptr(q), _ptr(k_new), _ptr(v_new), _ptr(cache_k), _ptr(cache_v), _ptr(exp_k), _ptr(exp_v), _ptr(q_start),
+                                        _ptr(seqpos), _ptr(out), q.shape[0], B, max_seqlen, W, n_heads, n_kv_heads, head_dim,
+                                        2 if first_prefill else 1, _stream()), "mb200_attn_prefill_fp8")
 
 
 def linear_residual(x, w, residual, out, ws: Workspace) -> None:

@@ -15,6 +15,7 @@ import numpy as np
 import torch
 
 SlidingWindow = Union[None, int, List[Optional[int]]]
+KV_CACHE_FORMATS = ("bf16", "fp8")
 
 
 def get_cache_sizes(n_layers: int, max_seq_len: int, sliding_window: SlidingWindow) -> List[int]:
@@ -48,9 +49,12 @@ class CacheInputMetadata:
 class CacheView:
     """cache.py:70-137: one layer's ring plus the metadata of this forward."""
 
-    def __init__(self, cache_k: torch.Tensor, cache_v: torch.Tensor, metadata: CacheInputMetadata, kv_seqlens_host: List[int]):
+    def __init__(self, cache_k: torch.Tensor, cache_v: torch.Tensor, metadata: CacheInputMetadata, kv_seqlens_host: List[int],
+                 cache_k_exp: Optional[torch.Tensor] = None, cache_v_exp: Optional[torch.Tensor] = None):
         self.cache_k = cache_k
         self.cache_v = cache_v
+        self.cache_k_exp = cache_k_exp  # FP8 cache: int8 exponents [max_batch, W, KV] of the e4m3 rows (None for bf16)
+        self.cache_v_exp = cache_v_exp
         self.metadata = metadata
         self.kv_seqlens_host = kv_seqlens_host
 
@@ -70,12 +74,25 @@ class CacheView:
     def prefill(self) -> bool:
         return self.metadata.prefill
 
+    @property
+    def fp8(self) -> bool:
+        return self.cache_k_exp is not None
+
 
 class BufferCache:
-    """Rectangular rotating cache; constructor and methods as cache.py:140-195."""
+    """Rectangular rotating cache; constructor and methods as cache.py:140-195.
+
+    kv_cache="fp8" stores every row as e4m3 codes with one int8 power-of-two exponent per (slot, kv head): `cache_k[i]` /
+    `cache_v[i]` are torch.float8_e4m3fn [max_batch, W, KV, hd] and `cache_k_exp[i]` / `cache_v_exp[i]` int8 [max_batch, W, KV]
+    (format: include/mistral_b200.h, mb200_kv_quantize).  Half the bytes of the bf16 cache plus 1/128 for the exponents."""
 
     def __init__(self, n_layers: int, max_batch_size: int, max_seq_len: int, n_kv_heads: int, head_dim: int,
-                 sliding_window: SlidingWindow = None):
+                 sliding_window: SlidingWindow = None, kv_cache: str = "bf16"):
+        if kv_cache not in KV_CACHE_FORMATS:
+            raise ValueError(f"kv_cache={kv_cache!r}: expected one of {KV_CACHE_FORMATS}")
+        if kv_cache == "fp8" and head_dim != 128:
+            raise ValueError(f"kv_cache='fp8' needs head_dim 128 (got {head_dim})")
+        self.kv_cache = kv_cache
         self.max_seq_len = max_seq_len
         self.n_kv_heads = n_kv_heads
         self.head_dim = head_dim
@@ -85,16 +102,25 @@ class BufferCache:
         assert len(self.cache_sizes) == n_layers, f"Expected {n_layers} cache sizes, got {len(self.cache_sizes)}"
         self.cache_k: Dict[int, torch.Tensor] = {}
         self.cache_v: Dict[int, torch.Tensor] = {}
+        self.cache_k_exp: Dict[int, torch.Tensor] = {}
+        self.cache_v_exp: Dict[int, torch.Tensor] = {}
         for i, cache_size in enumerate(self.cache_sizes):
-            self.cache_k[i] = torch.empty((max_batch_size, cache_size, n_kv_heads, head_dim))
-            self.cache_v[i] = torch.empty((max_batch_size, cache_size, n_kv_heads, head_dim))
+            if kv_cache == "fp8":
+                self.cache_k[i] = torch.empty((max_batch_size, cache_size, n_kv_heads, head_dim), dtype=torch.float8_e4m3fn)
+                self.cache_v[i] = torch.empty((max_batch_size, cache_size, n_kv_heads, head_dim), dtype=torch.float8_e4m3fn)
+                self.cache_k_exp[i] = torch.empty((max_batch_size, cache_size, n_kv_heads), dtype=torch.int8)
+                self.cache_v_exp[i] = torch.empty((max_batch_size, cache_size, n_kv_heads), dtype=torch.int8)
+            else:
+                self.cache_k[i] = torch.empty((max_batch_size, cache_size, n_kv_heads, head_dim))
+                self.cache_v[i] = torch.empty((max_batch_size, cache_size, n_kv_heads, head_dim))
         # host copy of the valid length per batch element (the reference keeps it on the device and syncs, cache.py:217)
         self._kv_seqlens_host: Optional[List[int]] = None
 
     # -- reference API --------------------------------------------------------------------------
     def get_view(self, layer_id: int, metadata: CacheInputMetadata) -> CacheView:
         assert self._kv_seqlens_host is not None
-        return CacheView(self.cache_k[layer_id], self.cache_v[layer_id], metadata, self._kv_seqlens_host)
+        return CacheView(self.cache_k[layer_id], self.cache_v[layer_id], metadata, self._kv_seqlens_host,
+                         self.cache_k_exp.get(layer_id), self.cache_v_exp.get(layer_id))
 
     def reset(self) -> None:
         self._kv_seqlens_host = None
@@ -113,10 +139,23 @@ class BufferCache:
         return self.cache_k[0].device
 
     def to(self, device: torch.device, dtype: torch.dtype) -> "BufferCache":
+        """Moves the cache; a bf16 cache takes `dtype`, an FP8 cache keeps its element format (e4m3 codes, int8 exponents)."""
         for i in range(self.n_layers):
-            self.cache_k[i] = self.cache_k[i].to(device=device, dtype=dtype)
-            self.cache_v[i] = self.cache_v[i].to(device=device, dtype=dtype)
+            if self.kv_cache == "fp8":
+                self.cache_k[i] = self.cache_k[i].to(device=device)
+                self.cache_v[i] = self.cache_v[i].to(device=device)
+                self.cache_k_exp[i] = self.cache_k_exp[i].to(device=device)
+                self.cache_v_exp[i] = self.cache_v_exp[i].to(device=device)
+            else:
+                self.cache_k[i] = self.cache_k[i].to(device=device, dtype=dtype)
+                self.cache_v[i] = self.cache_v[i].to(device=device, dtype=dtype)
         return self
+
+    @property
+    def nbytes(self) -> int:
+        """Bytes of every ring (and, for an FP8 cache, its exponents)."""
+        tensors = list(self.cache_k.values()) + list(self.cache_v.values()) + list(self.cache_k_exp.values()) + list(self.cache_v_exp.values())
+        return sum(t.numel() * t.element_size() for t in tensors)
 
     def update_seqlens(self, seqlens: List[int]) -> None:
         assert self._kv_seqlens_host is not None

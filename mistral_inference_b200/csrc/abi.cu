@@ -12,6 +12,7 @@
 #include "gemm_mma.cuh"
 #include "gemm_streamk.cuh"
 #include "gemm_wgmma.cuh"
+#include "kv_fp8.cuh"
 #include "lora.cuh"
 #include "moe.cuh"
 #include "sampling.cuh"
@@ -343,6 +344,111 @@ int mb200_attn_prefill(const void* q, const void* k_new, const void* v_new, cons
   attn_prefill_kernel<<<grid, AP_THREADS, AP_SMEM, (cudaStream_t)stream>>>(p);
   note_launch("attn_prefill_kernel");
   MB_CHECK_LAUNCH("attn_prefill_kernel");
+  return MB200_OK;
+}
+
+int mb200_kv_quantize(void* k, void* v, int write_back, void* cache_k, void* cache_v, int8_t* exp_k, int8_t* exp_v, const int32_t* cache_rows,
+                      int64_t T, int64_t n_kv_heads, int64_t head_dim, void* stream) {
+  MB_CHECK_ARG(k && v, "kv_quantize: null pointer");
+  MB_CHECK_ARG(head_dim == kHeadDim, "kv_quantize: head_dim=%lld unsupported (128 only)", (long long)head_dim);
+  MB_CHECK_ARG(cache_rows == nullptr || (cache_k && cache_v && exp_k && exp_v), "kv_quantize: cache_rows without ring pointers");
+  MB_CHECK_ARG(T >= 0 && n_kv_heads >= 1 && T * n_kv_heads * 2 <= 0x7fffffff, "kv_quantize: T=%lld KV=%lld", (long long)T, (long long)n_kv_heads);
+  MB_CHECK_ARG(((uintptr_t)k & 7) == 0 && ((uintptr_t)v & 7) == 0 && ((uintptr_t)cache_k & 3) == 0 && ((uintptr_t)cache_v & 3) == 0,
+               "kv_quantize: misaligned pointer");
+  if (T == 0 || (!write_back && cache_rows == nullptr)) return MB200_OK;
+  KvQuantParams p;
+  p.k = (bf16*)k;
+  p.v = (bf16*)v;
+  p.cache_k = (uint8_t*)cache_k;
+  p.cache_v = (uint8_t*)cache_v;
+  p.exp_k = exp_k;
+  p.exp_v = exp_v;
+  p.rows = cache_rows;
+  p.T = (int)T;
+  p.KV = (int)n_kv_heads;
+  p.write_back = write_back ? 1 : 0;
+  const int64_t warps = T * n_kv_heads * 2;
+  MB_CHECK_CUDA(launch_pdl(kv_quantize_kernel, dim3((unsigned)ceil_div(warps, 4)), dim3(128), 0, (cudaStream_t)stream, p));
+  note_launch("kv_quantize_kernel");
+  return MB200_OK;
+}
+
+int mb200_attn_decode_fp8(const void* q, const void* cache_k, const void* cache_v, const int8_t* exp_k, const int8_t* exp_v, const int32_t* kv_len,
+                          void* out, int64_t B, int64_t W, int64_t n_heads, int64_t n_kv_heads, int64_t head_dim, int64_t n_splits,
+                          void* workspace, size_t workspace_bytes, void* stream) {
+  MB_CHECK_ARG(q && cache_k && cache_v && exp_k && exp_v && kv_len && out, "attn_decode_fp8: null pointer");
+  MB_CHECK_ARG(head_dim == kHeadDim, "attn_decode_fp8: head_dim=%lld unsupported (128 only)", (long long)head_dim);
+  MB_CHECK_ARG(n_kv_heads >= 1 && n_heads % n_kv_heads == 0, "attn_decode_fp8: H %% KV != 0");
+  const int rep = (int)(n_heads / n_kv_heads);
+  MB_CHECK_ARG(n_splits >= 1 && n_splits <= 64, "attn_decode_fp8: n_splits=%lld out of [1, 64]", (long long)n_splits);
+  MB_CHECK_ARG((size_t)B * n_kv_heads * sizeof(int) <= kWsSplitKvCounters.bytes, "attn_decode_fp8: B*KV too large for the counter block");
+  AttnDecodeFp8Params fp;
+  AttnDecodeParams& p = fp.a;
+  p.q = (const bf16*)q;
+  p.cache_k = (const bf16*)cache_k;
+  p.cache_v = (const bf16*)cache_v;
+  p.kv_len = kv_len;
+  p.out = (bf16*)out;
+  p.B = (int)B;
+  p.W = (int)W;
+  p.H = (int)n_heads;
+  p.KV = (int)n_kv_heads;
+  p.S = (int)n_splits;
+  p.scale = 0.08838834764831845f;  // as mb200_attn_decode
+  p.partial = nullptr;
+  p.counters = nullptr;
+  fp.exp_k = exp_k;
+  fp.exp_v = exp_v;
+  if (n_splits > 1) {
+    const WsRegion pr = ws_splitkv_partials(B, n_kv_heads, n_splits, rep);
+    if (workspace == nullptr || workspace_bytes < pr.end()) return fail(MB200_E_WORKSPACE, "attn_decode_fp8: workspace %zu < %zu", workspace_bytes, pr.end());
+    p.counters = (int*)((uint8_t*)workspace + kWsSplitKvCounters.offset);
+    p.partial = (float*)((uint8_t*)workspace + pr.offset);
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  switch (rep) {
+    case 1: return launch_attn_decode_tma_fp8<1>(fp, B * W, st);
+    case 2: return launch_attn_decode_tma_fp8<2>(fp, B * W, st);
+    case 4: return launch_attn_decode_tma_fp8<4>(fp, B * W, st);
+    case 6: return launch_attn_decode_tma_fp8<6>(fp, B * W, st);
+    case 8: return launch_attn_decode_tma_fp8<8>(fp, B * W, st);
+    default: return fail(MB200_E_INVALID, "attn_decode_fp8: H/KV=%d unsupported (1,2,4,6,8)", rep);
+  }
+}
+
+int mb200_attn_prefill_fp8(const void* q, const void* k_new, const void* v_new, const void* cache_k, const void* cache_v, const int8_t* exp_k,
+                           const int8_t* exp_v, const int32_t* q_start, const int32_t* seqpos, void* out, int64_t T, int64_t B, int64_t max_seqlen,
+                           int64_t W, int64_t n_heads, int64_t n_kv_heads, int64_t head_dim, int causal, void* stream) {
+  MB_CHECK_ARG(causal == 1 || causal == 2, "attn_prefill_fp8: causal=%d (1 or 2; the cache-less forward has no ring)", causal);
+  MB_CHECK_ARG(head_dim == kHeadDim, "attn_prefill_fp8: head_dim=%lld unsupported (128 only)", (long long)head_dim);
+  MB_CHECK_ARG(exp_k && exp_v, "attn_prefill_fp8: null pointer");
+  // first prefill reads no ring row: the bf16 kernels run it on the chunk's k' / v'
+  if (causal == 2) return mb200_attn_prefill(q, k_new, v_new, cache_k, cache_v, q_start, seqpos, out, T, B, max_seqlen, W, n_heads, n_kv_heads, head_dim, 2, stream);
+  MB_CHECK_ARG(q && k_new && v_new && out && cache_k && cache_v && q_start && seqpos, "attn_prefill_fp8: null pointer");
+  MB_CHECK_ARG(n_kv_heads >= 1 && n_heads % n_kv_heads == 0, "attn_prefill_fp8: H %% KV != 0");
+  if (T == 0) return MB200_OK;
+  AttnPrefillParams p;
+  p.q = (const bf16*)q;
+  p.k_new = (const bf16*)k_new;
+  p.v_new = (const bf16*)v_new;
+  p.cache_k = (const bf16*)cache_k;
+  p.cache_v = (const bf16*)cache_v;
+  p.q_start = q_start;
+  p.seqpos = seqpos;
+  p.out = (bf16*)out;
+  p.T = (int)T;
+  p.B = (int)B;
+  p.W = (int)W;
+  p.H = (int)n_heads;
+  p.KV = (int)n_kv_heads;
+  p.causal = 1;
+  p.scale_log2 = 0.08838834764831845f * 1.4426950408889634f;
+  const KvFp8Exps ex{exp_k, exp_v};
+  const dim3 grid((unsigned)ceil_div(max_seqlen, AP_BQ), (unsigned)n_heads, (unsigned)B);
+  MB_CHECK_CUDA(cudaFuncSetAttribute(attn_prefill_fp8_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, AP_SMEM));
+  attn_prefill_fp8_kernel<<<grid, AP_THREADS, AP_SMEM, (cudaStream_t)stream>>>(p, ex);
+  note_launch("attn_prefill_fp8_kernel");
+  MB_CHECK_LAUNCH("attn_prefill_fp8_kernel");
   return MB200_OK;
 }
 

@@ -47,6 +47,88 @@ __device__ __forceinline__ uint32_t adt_off(int row, int C) {
   return (uint32_t)((C >> 3) * ADT_HALF_BYTES + row * 128 + (((C & 7) ^ (row & 7)) << 4));
 }
 
+// The end of a decode CTA, after every warp has published its (m, l, acc) in sm_m / sm_l / sm_acc and the block has synchronised:
+// merge the consumer warps and, with S > 1, the splits (the last CTA of a (b, g) to arrive combines them).  Shared by
+// attn_decode_tma_kernel and attn_decode_tma_fp8_kernel (csrc/kv_fp8.cuh).
+template <int REP>
+__device__ __forceinline__ void adt_merge(const AttnDecodeParams& p, const float (&sm_m)[ADT_CONSUMER_WARPS][REP],
+                                          const float (&sm_l)[ADT_CONSUMER_WARPS][REP], const float (&sm_acc)[ADT_CONSUMER_WARPS][REP][kHeadDim],
+                                          int& is_last, float* cm, float* cl, int s, int g, int b, int tid, int warp) {
+  constexpr float kMasked = -1.0e30f;
+  if (warp == ADT_CONSUMER_WARPS) {
+    if (p.S == 1) return;  // the producer warp takes no part in the merge
+  }
+
+  // ---- merge the warps: thread d (0..127) finishes dim d of every head of the group (log2 domain) ----
+  const int d = tid;
+  float fm[REP], fl[REP], fa[REP];
+  if (warp < ADT_CONSUMER_WARPS) {
+#pragma unroll
+    for (int r = 0; r < REP; ++r) {
+      float mn = kMasked;
+#pragma unroll
+      for (int w = 0; w < ADT_CONSUMER_WARPS; ++w) mn = fmaxf(mn, sm_m[w][r]);
+      float lt = 0.f, at = 0.f;
+#pragma unroll
+      for (int w = 0; w < ADT_CONSUMER_WARPS; ++w) {
+        const float c = exp2f(sm_m[w][r] - mn);  // empty warps: l = acc = 0
+        lt += sm_l[w][r] * c;
+        at += sm_acc[w][r][d] * c;
+      }
+      fm[r] = mn;
+      fl[r] = lt;
+      fa[r] = at;
+    }
+    if (p.S == 1) {
+#pragma unroll
+      for (int r = 0; r < REP; ++r) p.out[((int64_t)b * p.H + g * REP + r) * kHeadDim + d] = __float2bfloat16_rn(fa[r] / fl[r]);
+      return;
+    }
+    // ---- publish the partial; the last split of this (b, g) to arrive combines all of them ----
+    const int PSTRIDE = kHeadDim + 2;
+    float* mine = p.partial + ((((int64_t)b * p.KV + g) * p.S + s) * REP) * PSTRIDE;
+#pragma unroll
+    for (int r = 0; r < REP; ++r) {
+      mine[r * PSTRIDE + 2 + d] = fa[r];
+      if (d == 0) {
+        mine[r * PSTRIDE + 0] = fm[r];
+        mine[r * PSTRIDE + 1] = fl[r];
+      }
+    }
+    __threadfence();
+  }
+  __syncthreads();
+  if (tid == 0) {
+    const int prev = atomicAdd(&p.counters[b * p.KV + g], 1);
+    is_last = (prev == p.S - 1);
+    if (is_last) p.counters[b * p.KV + g] = 0;  // self-reset for the next launch (stream-ordered)
+  }
+  __syncthreads();
+  if (!is_last) return;
+  __threadfence();
+  const int PSTRIDE = kHeadDim + 2;
+  const float* all = p.partial + (((int64_t)b * p.KV + g) * p.S) * REP * PSTRIDE;
+  for (int i = tid; i < p.S * REP; i += ADT_THREADS) {
+    cm[i] = __ldcg(all + (int64_t)i * PSTRIDE);
+    cl[i] = __ldcg(all + (int64_t)i * PSTRIDE + 1);
+  }
+  __syncthreads();
+  if (warp >= ADT_CONSUMER_WARPS) return;
+#pragma unroll
+  for (int r = 0; r < REP; ++r) {
+    float mn = kMasked;
+    for (int t = 0; t < p.S; ++t) mn = fmaxf(mn, cm[t * REP + r]);
+    float lt = 0.f, at = 0.f;
+#pragma unroll 8
+    for (int t = 0; t < p.S; ++t) {
+      const float c = exp2f(cm[t * REP + r] - mn);
+      lt += cl[t * REP + r] * c;
+      at += __ldcg(all + ((int64_t)t * REP + r) * PSTRIDE + 2 + d) * c;
+    }
+    p.out[((int64_t)b * p.H + g * REP + r) * kHeadDim + d] = __float2bfloat16_rn(at / lt);
+  }
+}
+
 template <int REP>
 __global__ void __launch_bounds__(ADT_THREADS, 2)
     attn_decode_tma_kernel(const __grid_constant__ CUtensorMap map_k, const __grid_constant__ CUtensorMap map_v, const AttnDecodeParams p) {
@@ -196,78 +278,7 @@ __global__ void __launch_bounds__(ADT_THREADS, 2)
     }
   }
   __syncthreads();
-  if (warp == ADT_CONSUMER_WARPS) {
-    if (p.S == 1) return;  // the producer warp takes no part in the merge
-  }
-
-  // ---- merge the warps: thread d (0..127) finishes dim d of every head of the group (log2 domain) ----
-  const int d = tid;
-  float fm[REP], fl[REP], fa[REP];
-  if (warp < ADT_CONSUMER_WARPS) {
-#pragma unroll
-    for (int r = 0; r < REP; ++r) {
-      float mn = kMasked;
-#pragma unroll
-      for (int w = 0; w < ADT_CONSUMER_WARPS; ++w) mn = fmaxf(mn, sm_m[w][r]);
-      float lt = 0.f, at = 0.f;
-#pragma unroll
-      for (int w = 0; w < ADT_CONSUMER_WARPS; ++w) {
-        const float c = exp2f(sm_m[w][r] - mn);  // empty warps: l = acc = 0
-        lt += sm_l[w][r] * c;
-        at += sm_acc[w][r][d] * c;
-      }
-      fm[r] = mn;
-      fl[r] = lt;
-      fa[r] = at;
-    }
-    if (p.S == 1) {
-#pragma unroll
-      for (int r = 0; r < REP; ++r) p.out[((int64_t)b * p.H + g * REP + r) * kHeadDim + d] = __float2bfloat16_rn(fa[r] / fl[r]);
-      return;
-    }
-    // ---- publish the partial; the last split of this (b, g) to arrive combines all of them ----
-    const int PSTRIDE = kHeadDim + 2;
-    float* mine = p.partial + ((((int64_t)b * p.KV + g) * p.S + s) * REP) * PSTRIDE;
-#pragma unroll
-    for (int r = 0; r < REP; ++r) {
-      mine[r * PSTRIDE + 2 + d] = fa[r];
-      if (d == 0) {
-        mine[r * PSTRIDE + 0] = fm[r];
-        mine[r * PSTRIDE + 1] = fl[r];
-      }
-    }
-    __threadfence();
-  }
-  __syncthreads();
-  if (tid == 0) {
-    const int prev = atomicAdd(&p.counters[b * p.KV + g], 1);
-    is_last = (prev == p.S - 1);
-    if (is_last) p.counters[b * p.KV + g] = 0;  // self-reset for the next launch (stream-ordered)
-  }
-  __syncthreads();
-  if (!is_last) return;
-  __threadfence();
-  const int PSTRIDE = kHeadDim + 2;
-  const float* all = p.partial + (((int64_t)b * p.KV + g) * p.S) * REP * PSTRIDE;
-  for (int i = tid; i < p.S * REP; i += ADT_THREADS) {
-    cm[i] = __ldcg(all + (int64_t)i * PSTRIDE);
-    cl[i] = __ldcg(all + (int64_t)i * PSTRIDE + 1);
-  }
-  __syncthreads();
-  if (warp >= ADT_CONSUMER_WARPS) return;
-#pragma unroll
-  for (int r = 0; r < REP; ++r) {
-    float mn = kMasked;
-    for (int t = 0; t < p.S; ++t) mn = fmaxf(mn, cm[t * REP + r]);
-    float lt = 0.f, at = 0.f;
-#pragma unroll 8
-    for (int t = 0; t < p.S; ++t) {
-      const float c = exp2f(cm[t * REP + r] - mn);
-      lt += cl[t * REP + r] * c;
-      at += __ldcg(all + ((int64_t)t * REP + r) * PSTRIDE + 2 + d) * c;
-    }
-    p.out[((int64_t)b * p.H + g * REP + r) * kHeadDim + d] = __float2bfloat16_rn(at / lt);
-  }
+  adt_merge<REP>(p, sm_m, sm_l, sm_acc, is_last, cm, cl, s, g, b, tid, warp);
 }
 
 // [rows, cols] bf16 row-major cache seen as a 2-D tensor; box = [64 cols (128 B) x 64 rows], 128-byte swizzle, OOB rows read as zero

@@ -10,6 +10,7 @@
 // Mask (cache.py:240,243-248; SURVEY.md Appendix B): query at absolute position p sees keys in (p - W, p].
 #pragma once
 #include "gemm_mma.cuh"
+#include "kv_fp8.cuh"  // kv_dequant8
 
 namespace mb200 {
 
@@ -34,7 +35,16 @@ struct AttnPrefillParams {
 // byte offset of 16-byte chunk (0..15) of row (0..63) in a [64][128 bf16] tile; XOR swizzle on the low 3 chunk bits
 __device__ __forceinline__ uint32_t ap_swz(int row, int chunk) { return (uint32_t)(row * 256 + (((chunk & 8) | ((chunk ^ row) & 7)) << 4)); }
 
-__global__ void __launch_bounds__(AP_THREADS, 2) attn_prefill_kernel(const AttnPrefillParams p) {
+// Ring rows of an e4m3 cache (csrc/kv_fp8.cuh): cache_k / cache_v of AttnPrefillParams hold the codes, these the exponents.
+struct KvFp8Exps {
+  const int8_t* k;  // [max_batch * W, KV]
+  const int8_t* v;
+};
+
+// The kernel body.  FP8: the ring is e4m3, and its rows are rebuilt as bf16 x' with plain loads and shared-memory stores (cp.async
+// cannot convert); chunk rows are bf16 k' / v' and take cp.async as in the bf16 kernel, so the two kernels see the same tiles.
+template <bool FP8>
+__device__ __forceinline__ void attn_prefill_body(const AttnPrefillParams& p, const KvFp8Exps& ex) {
   extern __shared__ __align__(128) uint8_t smem[];
   const uint32_t sQ = (uint32_t)__cvta_generic_to_shared(smem);
   const uint32_t sKV = sQ + AP_TILE_BYTES;  // stage st: K at sKV + st*2*TILE, V right after
@@ -93,6 +103,18 @@ __global__ void __launch_bounds__(AP_THREADS, 2) attn_prefill_kernel(const AttnP
       const int row = idx >> 4, chunk = idx & 15;
       const int j = j0 + row;
       const bool ok = j <= key_hi;
+      if constexpr (FP8) {
+        if (ok && j < pos0) {
+          const int64_t ring_row = (int64_t)b * p.W + (j % p.W);
+          const int64_t off = ring_row * kv_ld + (int64_t)g * kHeadDim + chunk * 8;
+          const uint2 kq = *reinterpret_cast<const uint2*>(reinterpret_cast<const uint8_t*>(p.cache_k) + off);
+          const uint2 vq = *reinterpret_cast<const uint2*>(reinterpret_cast<const uint8_t*>(p.cache_v) + off);
+          const int ek = ex.k[ring_row * p.KV + g], ev = ex.v[ring_row * p.KV + g];
+          *reinterpret_cast<uint4*>(smem + (sK - sQ) + ap_swz(row, chunk)) = kv_dequant8(kq, ek);
+          *reinterpret_cast<uint4*>(smem + (sV - sQ) + ap_swz(row, chunk)) = kv_dequant8(vq, ev);
+          continue;
+        }
+      }
       const bf16 *ksrc, *vsrc;
       if (ok && j < pos0) {  // already cached: ring slot j % W of sequence b
         const int64_t off = ((int64_t)b * p.W + (j % p.W)) * kv_ld + (int64_t)g * kHeadDim + chunk * 8;
@@ -230,6 +252,13 @@ __global__ void __launch_bounds__(AP_THREADS, 2) attn_prefill_kernel(const AttnP
     for (int j = 0; j < 16; ++j)
       *reinterpret_cast<uint32_t*>(dst + j * 8) = pack_bf16x2(o[j][hh * 2] * inv, o[j][hh * 2 + 1] * inv);
   }
+}
+
+__global__ void __launch_bounds__(AP_THREADS, 2) attn_prefill_kernel(const AttnPrefillParams p) { attn_prefill_body<false>(p, KvFp8Exps{}); }
+
+// Chunked prefill over an e4m3 ring: bit-identical to attn_prefill_kernel on a bf16 ring that holds x'.
+__global__ void __launch_bounds__(AP_THREADS, 2) attn_prefill_fp8_kernel(const AttnPrefillParams p, const KvFp8Exps ex) {
+  attn_prefill_body<true>(p, ex);
 }
 
 }  // namespace mb200

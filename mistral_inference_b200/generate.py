@@ -70,7 +70,7 @@ def generate(encoded_prompts: List[List[int]], model: Transformer, images: List[
 
     # one ring per layer, sized like the reference's (generate.py:68-78)
     cache = BufferCache(model.n_local_layers, model.args.max_batch_size, max(plan.lens) + max_tokens, model.args.n_kv_heads,
-                        model.args.head_dim, model.args.sliding_window)
+                        model.args.head_dim, model.args.sliding_window, kv_cache=model.kv_cache)
     cache.to(device=dev, dtype=model.dtype)
     cache.reset()
 

@@ -16,7 +16,7 @@ from torch import nn
 
 from . import _abi
 from .args import PATCH_MERGE, TransformerArgs
-from .cache import BufferCache, CacheInputMetadata
+from .cache import KV_CACHE_FORMATS, BufferCache, CacheInputMetadata
 from .rope import precompute_freqs_cis
 from .moe import EXPERT_WEIGHTS, Fp8Expert
 from .transformer_layers import LoraAdapter, RMSNorm, TransformerBlock
@@ -59,13 +59,21 @@ class _OutputView:
 
 class Transformer(nn.Module):
     def __init__(self, args: TransformerArgs, pipeline_rank: int = 0, num_pipeline_ranks: int = 1, softmax_fp32: bool = True,
-                 expert_parallel: Optional[Tuple[int, int]] = None, expert_group: Any = None, expert_weights: str = "bf16"):
+                 expert_parallel: Optional[Tuple[int, int]] = None, expert_group: Any = None, expert_weights: str = "bf16", *,
+                 kv_cache: str = "bf16"):
         """Same signature as the reference (transformer.py:34-40) plus `expert_parallel = (rank, world)`: MoE experts sharded
         `e % world == rank` over the ranks of `expert_group` (default process group), everything else replicated, one
         all-reduce of [T, dim] per MoE layer (SURVEY.md 8e); and `expert_weights`: "bf16", or "fp8" to store every MoE expert
         matrix as e4m3 with one fp32 scale per row (moe.Fp8Expert; the model then computes exactly what the bf16 model computes
-        with the dequantised weights W', see include/mistral_b200.h)."""
+        with the dequantised weights W', see include/mistral_b200.h); and `kv_cache`: "bf16", or "fp8" to keep the KV cache as e4m3
+        with one power-of-two exponent per (slot, kv head) row (cache.BufferCache; the model is then the bf16 model with k, v
+        replaced by their dequantised k', v' right after RoPE in every forward that has a cache, see include/mistral_b200.h)."""
         super().__init__()
+        if kv_cache not in KV_CACHE_FORMATS:
+            raise ValueError(f"kv_cache={kv_cache!r}: expected one of {KV_CACHE_FORMATS}")
+        if kv_cache == "fp8" and args.head_dim != 128:
+            raise ValueError(f"kv_cache='fp8' needs head_dim 128: the FP8 attention kernels read 128-byte rows (got {args.head_dim})")
+        self.kv_cache = kv_cache
         if expert_weights not in EXPERT_WEIGHTS:
             raise ValueError(f"expert_weights={expert_weights!r}: expected one of {EXPERT_WEIGHTS}")
         if expert_weights == "fp8" and args.moe is None:
@@ -171,12 +179,17 @@ class Transformer(nn.Module):
         if self.device.type != "cuda" or self.dtype != torch.bfloat16:
             raise _abi.Mb200Error(f"the libmb200 hot path runs bf16 on CUDA only (got {self.dtype} on {self.device}); no fallback exists")
 
+    def _check_cache(self, cache: Optional[BufferCache]) -> None:
+        assert cache is None or cache.kv_cache == self.kv_cache, (
+            f"a {cache.kv_cache} KV cache passed to a model built with kv_cache={self.kv_cache!r}")
+
     @torch.inference_mode()
     def forward_partial(self, input_ids: torch.Tensor, seqlens: List[int], cache: Optional[BufferCache] = None,
                         images: Optional[List[torch.Tensor]] = None) -> torch.Tensor:
         """Local forward pass (transformer.py:163-219): hidden states of this stage; the last stage returns
         the normalised final embeddings."""
         self._check_runnable()
+        self._check_cache(cache)
         assert len(seqlens) <= self.args.max_batch_size, f"Max batch size is {self.args.max_batch_size}, got batch size of {len(seqlens)}"
         (num_toks,) = input_ids.shape
         assert sum(seqlens) == num_toks, (sum(seqlens), num_toks)
@@ -215,6 +228,7 @@ class Transformer(nn.Module):
                 images: Optional[List[torch.Tensor]] = None) -> torch.Tensor:
         """transformer.py:221-242.  [T, vocab] logits, fp32 when softmax_fp32."""
         self._check_runnable()
+        self._check_cache(cache)
         last = self.pipeline_rank == self.num_pipeline_ranks - 1
         if last and self.num_pipeline_ranks == 1:
             if not self._uses_images(images) and self._graph_decode_ok(seqlens, cache):
@@ -313,12 +327,12 @@ class Transformer(nn.Module):
                 and len(set(cache.cache_sizes)) <= 8)
 
     def _megakernel_ok(self, B: int) -> bool:
-        # the megakernel has no LoRA stage and reads bf16 experts only: with un-merged adapters or FP8 experts batch 1 takes the
-        # per-layer graph path
+        # the megakernel has no LoRA stage and reads bf16 experts and a bf16 KV cache only: with un-merged adapters, FP8 experts or
+        # an FP8 cache batch 1 takes the per-layer graph path
         # the shape limits (head ratio, K chunking, KV <= 8, MoE sizes, a shared-memory ring of >= 9 stages next to the
         # activations) are the library's, asked once per model: a model it refuses takes the per-layer path
         if not (B == 1 and self.num_pipeline_ranks == 1 and self.expert_parallel[1] == 1 and self.args.lora is None
-                and self.expert_weights == "bf16" and os.environ.get("MB200_MEGAKERNEL", "1") != "0"):
+                and self.expert_weights == "bf16" and self.kv_cache == "bf16" and os.environ.get("MB200_MEGAKERNEL", "1") != "0"):
             return False
         if self._megakernel_refused is None:
             a, moe = self.args, self.args.moe
@@ -402,6 +416,7 @@ class Transformer(nn.Module):
         round-1 design and a race).  Returns the STATIC fp32 logits buffer [B, V] (overwritten by the next step).  The first call
         per (cache, batch) runs eagerly (warm-up: loads modules, sets function attributes), the second captures."""
         B = tokens.shape[0]
+        self._check_cache(cache)
         if self._megakernel_ok(B):
             return self._decode_megakernel(tokens, cache)
         seqlens = [1] * B
@@ -473,6 +488,7 @@ class Transformer(nn.Module):
         per-token gathers (generate.py:97-118): the lm head runs over blocks of rows, each followed by the fused
         log-softmax + gather kernel, so the full [T, V] logits never exist."""
         self._last_static_logits = 0
+        self._check_cache(cache)
         T, V = input_ids.shape[0], self.vocab_size
         last_idx = torch.tensor(seqlens, device=input_ids.device).cumsum(0) - 1
         lp = torch.zeros(T, dtype=torch.float32, device=input_ids.device)
@@ -789,10 +805,11 @@ class Transformer(nn.Module):
     def from_folder(folder: Union[Path, str], max_batch_size: int = 1, num_pipeline_ranks: int = 1,
                     device: Union[torch.device, str] = "cuda", dtype: Optional[torch.dtype] = None,
                     softmax_fp32: bool = True, expert_parallel: Optional[Tuple[int, int]] = None, expert_group: Any = None,
-                    expert_weights: str = "bf16") -> "Transformer":
+                    expert_weights: str = "bf16", *, kv_cache: str = "bf16") -> "Transformer":
         """transformer.py:297-338.  Tensors stream from disk straight into the packed device buffers; with `expert_parallel`
         the experts of other ranks are skipped (never read into device memory).  With expert_weights="fp8" each bf16 expert
-        tensor is copied to the device and quantised into place: the peak is the FP8 model plus about one bf16 tensor."""
+        tensor is copied to the device and quantised into place: the peak is the FP8 model plus about one bf16 tensor.
+        `kv_cache` ("bf16" | "fp8") is the format of the KV cache that generate() builds (see Transformer)."""
         with open(Path(folder) / "params.json", "r") as f:
             model_args = TransformerArgs.from_dict(json.load(f))
         model_args.max_batch_size = max_batch_size
@@ -812,7 +829,7 @@ class Transformer(nn.Module):
             # on meta and assigns, transformer.py:321-331; a fp32 build followed by .to(bf16) would need 3x the model's bytes)
             return Transformer.empty(model_args, dev, dtype or ck_dtype, pipeline_rank=pipeline_rank, num_pipeline_ranks=num_pipeline_ranks,
                                      softmax_fp32=softmax_fp32, expert_parallel=expert_parallel, expert_group=expert_group,
-                                     expert_weights=expert_weights)
+                                     expert_weights=expert_weights, kv_cache=kv_cache)
 
         if pt_model_file.exists():
             loaded = torch.load(str(pt_model_file), mmap=True)

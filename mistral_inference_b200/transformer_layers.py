@@ -149,6 +149,8 @@ class Attention(nn.Module):
             _abi.attn_prefill(q, k, v, None, None, None, None, out, 1, T, 0, H, KV, hd, causal=False)
             return out
         md = cache.metadata
+        if cache.fp8:
+            return self._attend_fp8(x, norm_w, eps, rope, positions, cache, ws, q, k, v, out)
         if md.prefill:
             # read the old ring, THEN write (transformer_layers.py:75-76)
             self._qkv(x, norm_w, rope, positions, q, k, v, None, None, None, eps, ws)
@@ -160,6 +162,25 @@ class Attention(nn.Module):
             self._qkv(x, norm_w, rope, positions, q, k, v, cache.cache_k, cache.cache_v, md.cache_rows, eps, ws)
             B = len(md.seqlens)
             _abi.attn_decode(q, cache.cache_k, cache.cache_v, md.kv_len, out, H, KV, hd, decode_splits(B, KV, md.window), ws)
+        return out
+
+    def _attend_fp8(self, x, norm_w, eps, rope, positions, cache: CacheView, ws, q, k, v, out) -> torch.Tensor:
+        """The FP8-cache model: k, v become k', v' (include/mistral_b200.h) right after RoPE, and attention sees only those."""
+        H, KV, hd = self.n_heads, self.n_kv_heads, self.head_dim
+        md = cache.metadata
+        ring = (cache.cache_k, cache.cache_v, cache.cache_k_exp, cache.cache_v_exp)
+        self._qkv(x, norm_w, rope, positions, q, k, v, None, None, None, eps, ws)
+        if md.prefill:
+            # k', v' in place; read the old ring, THEN write it from k', v' (transformer_layers.py:75-76)
+            _abi.kv_quantize(k, v, True)
+            _abi.attn_prefill_fp8(q, k, v, *ring, md.q_start, md.seqpos, out, len(md.seqlens), md.max_seqlen, md.window, H, KV, hd,
+                                  first_prefill=md.first_prefill)
+            _abi.kv_quantize(k, v, False, *ring, md.cache_rows)
+        else:
+            # write, THEN read the ring (transformer_layers.py:78-81)
+            _abi.kv_quantize(k, v, False, *ring, md.cache_rows)
+            B = len(md.seqlens)
+            _abi.attn_decode_fp8(q, *ring, md.kv_len, out, H, KV, hd, decode_splits(B, KV, md.window), ws)
         return out
 
     def _qkv(self, x, norm_w, rope, positions, q, k, v, cache_k, cache_v, cache_rows, eps, ws) -> None:
