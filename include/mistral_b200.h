@@ -425,6 +425,49 @@ int mb200_debug_decode_buffers(int64_t dim, int64_t hidden, int64_t n_heads, int
 int mb200_decode_step_supported(int64_t dim, int64_t hidden, int64_t n_heads, int64_t n_kv_heads, int64_t head_dim, int64_t vocab,
                                 int64_t n_experts, int64_t top_k, int64_t smem_optin);
 
+/* ---------------------------------------------------------------------------------------------
+ * FP8 (e4m3) dense weights (Python: Transformer(..., dense_weights="fp8")).  The storage format is that of the FP8 experts: per row
+ * n of a Linear's weight W [N, K], s[n] = fp32(amax_k |W[n, k]| / 448) (1 for an all-zero row) and
+ * q[n, k] = e4m3fn_rn(clamp(fp32(W[n, k] / s[n]), -448, 448)), written by mb200_quantize_e4m3_rows.  The compute is different
+ * from the experts' W' contract: the scale leaves the dot product,
+ *     acc[t, n] = fp32 sum over k of x[t, k] * float(q[n, k])      (any order: the operand is q itself, converted exactly)
+ *     y[t, n]   = bf16(fp32(s[n] * acc[t, n]))                      (one fp32 product, then the Linear's bf16 rounding)
+ * followed by the mode's own epilogue on y exactly as in the bf16 entry points (residual add, SiLU * mul, RoPE + ring scatter).
+ * Every e4m3 value is a bf16 value, so the tensor-core kernels feed q to the same bf16 MMAs.  The FP8 dense model is not bit-identical
+ * to any bf16 model.
+ *
+ * mb200_attn_qkv_fp8, mb200_ffn_gateup_fp8, mb200_linear_residual_fp8: the counterpart's arguments with the weight replaced by
+ *     w_q (e4m3 [N, K], one byte per element; wqkv rows cat(q, k, v), w13 rows interleaved w1 / w3) and w_scale (fp32 [N]).
+ *     Kernel choice is mb200_linear's (T <= 4: weight-streaming GEMV; 5..128 tokens with N % 128 == 0: stream-K; else wgmma, single
+ *     CTA at the bf16 tile width); a shape the bf16 path would run on mma.sync (K % 64 != 0, or N not a multiple of 32 below 128
+ *     tokens, of 128 or 192 from 128 tokens on) returns MB200_E_INVALID.
+ * mb200_decode_step_fp8: mb200_decode_step for a dense model whose layer matrices are e4m3: layers_dev is a DEVICE array of
+ *     mb200_layer_desc_fp8.  The norms, the K/V ring, the embedding and the lm head stay bf16.  mb200_decode_step_fp8_supported is
+ *     its mb200_decode_step_supported (dense shapes only).
+ */
+int mb200_attn_qkv_fp8(const void* x, const void* norm_w, const void* w_q, const float* w_scale, const float* rope, const int32_t* positions,
+                       void* q_out, void* k_out, void* v_out, void* cache_k, void* cache_v, const int32_t* cache_rows, int64_t T, int64_t dim,
+                       int64_t n_heads, int64_t n_kv_heads, int64_t head_dim, float eps, void* workspace, size_t workspace_bytes, void* stream);
+int mb200_ffn_gateup_fp8(const void* x, const void* norm_w, const void* w_q, const float* w_scale, void* g_out, int64_t T, int64_t dim,
+                         int64_t hidden, float eps, void* workspace, size_t workspace_bytes, void* stream);
+int mb200_linear_residual_fp8(const void* x, const void* w_q, const float* w_scale, const void* residual, void* out, int64_t T, int64_t N,
+                              int64_t K, void* workspace, size_t workspace_bytes, void* stream);
+
+typedef struct mb200_layer_desc_fp8 {
+  mb200_layer_desc layer;  /* wqkv / wo / w13 / w2 point to e4m3 matrices of the shapes above */
+  const float* wqkv_scale; /* [(H+2KV)*hd] */
+  const float* wo_scale;   /* [dim] */
+  const float* w13_scale;  /* [2*hidden] */
+  const float* w2_scale;   /* [dim] */
+} mb200_layer_desc_fp8;
+
+int mb200_decode_step_fp8(const mb200_layer_desc_fp8* layers_dev, const int32_t* windows_dev, int64_t n_layers, const void* emb,
+                          const void* final_norm, const void* w_out, const float* rope, const int64_t* token_dev, int64_t pos,
+                          int64_t batch_row, float* logits, int64_t* next_token_dev, int64_t dim, int64_t hidden, int64_t n_heads,
+                          int64_t n_kv_heads, int64_t head_dim, int64_t vocab, float eps, void* workspace, size_t workspace_bytes, void* stream);
+int mb200_decode_step_fp8_supported(int64_t dim, int64_t hidden, int64_t n_heads, int64_t n_kv_heads, int64_t head_dim, int64_t vocab,
+                                    int64_t smem_optin);
+
 /* Test-only: CUDA-core fp32 GEMM c[T, N] = a[T, K] w[N, K]^T used to cross-check the tensor-core kernels. */
 int mb200_test_gemm_naive(const void* a, const void* w, float* c, int64_t T, int64_t N, int64_t K, void* stream);
 

@@ -79,6 +79,16 @@ _SIGNATURES = {
     "mb200_debug_decode_scratch": (c_int, [c_int64] * 7 + [ctypes.POINTER(c_size_t), ctypes.POINTER(c_size_t)]),
     "mb200_debug_decode_buffers": (c_int, [c_int64] * 7 + [ctypes.POINTER(c_size_t)]),
     "mb200_decode_step_supported": (c_int, [c_int64] * 9),
+    "mb200_attn_qkv_fp8": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                   c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int64, c_int64, c_float, c_void_p, c_size_t, c_void_p]),
+    "mb200_ffn_gateup_fp8": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_float, c_void_p,
+                                     c_size_t, c_void_p]),
+    "mb200_linear_residual_fp8": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_void_p,
+                                          c_size_t, c_void_p]),
+    "mb200_decode_step_fp8": (c_int, [c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64,
+                                      c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int64, c_int64, c_int64, c_float, c_void_p, c_size_t,
+                                      c_void_p]),
+    "mb200_decode_step_fp8_supported": (c_int, [c_int64] * 7),
     "mb200_test_gemm_naive": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_void_p]),
 }
 
@@ -283,6 +293,36 @@ def ffn_gateup(x, norm_w, w13, g_out, eps, ws: Workspace) -> None:
            "mb200_ffn_gateup")
 
 
+# ---- FP8 dense weights (include/mistral_b200.h): w_q is the e4m3 matrix as uint8 [N, K], w_scale its fp32 row scales [N] ----
+def _check_fp8(w_q: torch.Tensor, w_scale: torch.Tensor) -> None:
+    assert w_q.dtype == torch.uint8 and w_scale.dtype == torch.float32 and w_scale.shape == (w_q.shape[0],), (w_q.dtype, w_scale.dtype)
+
+
+def attn_qkv_fp8(x, norm_w, w_q, w_scale, rope, positions, q_out, k_out, v_out, cache_k, cache_v, cache_rows, n_heads, n_kv_heads, head_dim,
+                 eps, ws: Workspace) -> None:
+    _check_fp8(w_q, w_scale)
+    T, dim = x.shape
+    _check(lib().mb200_attn_qkv_fp8(_ptr(x), _ptr(norm_w), _ptr(w_q), _ptr(w_scale), _ptr(rope), _ptr(positions), _ptr(q_out), _ptr(k_out),
+                                    _ptr(v_out), _ptr(cache_k), _ptr(cache_v), _ptr(cache_rows), T, dim, n_heads, n_kv_heads, head_dim, eps,
+                                    ws.ptr, ws.nbytes, _stream()), "mb200_attn_qkv_fp8")
+
+
+def ffn_gateup_fp8(x, norm_w, w_q, w_scale, g_out, eps, ws: Workspace) -> None:
+    _check_fp8(w_q, w_scale)
+    T, dim = x.shape
+    hidden = w_q.shape[0] // 2
+    _check(lib().mb200_ffn_gateup_fp8(_ptr(x), _ptr(norm_w), _ptr(w_q), _ptr(w_scale), _ptr(g_out), T, dim, hidden, eps, ws.ptr, ws.nbytes,
+                                      _stream()), "mb200_ffn_gateup_fp8")
+
+
+def linear_residual_fp8(x, w_q, w_scale, residual, out, ws: Workspace) -> None:
+    _check_fp8(w_q, w_scale)
+    T, K = x.shape
+    N = w_q.shape[0]
+    _check(lib().mb200_linear_residual_fp8(_ptr(x), _ptr(w_q), _ptr(w_scale), _ptr(residual), _ptr(out), T, N, K, ws.ptr, ws.nbytes,
+                                           _stream()), "mb200_linear_residual_fp8")
+
+
 class LoraStruct(ctypes.Structure):
     """mb200_lora (include/mistral_b200.h)."""
     _fields_ = [("a_w", c_void_p), ("b_w", c_void_p), ("rank_cols", c_int64), ("scaling", c_float), ("a_buf", c_void_p), ("l_buf", c_void_p)]
@@ -441,6 +481,22 @@ def decode_step(layers_dev, windows_dev, n_layers, emb, final_norm, w_out, rope,
                                    _ptr(token_dev), pos, batch_row, _ptr(logits), _ptr(next_token), dim, hidden, n_heads, n_kv_heads, head_dim,
                                    vocab, eps, n_experts, top_k, _ptr(moe_gate), _ptr(moe_w13), _ptr(moe_w2), ws.ptr, ws.nbytes, _stream()),
            "mb200_decode_step")
+
+
+def decode_step_fp8(layers_dev, windows_dev, n_layers, emb, final_norm, w_out, rope, token_dev, pos, batch_row, logits, next_token, dim,
+                    hidden, n_heads, n_kv_heads, head_dim, vocab, eps, ws: Workspace) -> None:
+    """decode_step for a dense FP8 model: layers_dev holds one mb200_layer_desc_fp8 (12 pointers) per layer."""
+    _check(lib().mb200_decode_step_fp8(_ptr(layers_dev), _ptr(windows_dev), n_layers, _ptr(emb), _ptr(final_norm), _ptr(w_out), _ptr(rope),
+                                       _ptr(token_dev), pos, batch_row, _ptr(logits), _ptr(next_token), dim, hidden, n_heads, n_kv_heads,
+                                       head_dim, vocab, eps, ws.ptr, ws.nbytes, _stream()), "mb200_decode_step_fp8")
+
+
+def decode_step_fp8_unsupported(dim, hidden, n_heads, n_kv_heads, head_dim, vocab, smem_optin: int = 0) -> Optional[str]:
+    """decode_step_unsupported for decode_step_fp8 (dense shapes)."""
+    if lib().mb200_decode_step_fp8_supported(dim, hidden, n_heads, n_kv_heads, head_dim, vocab, smem_optin) == 0:
+        return None
+    msg = lib().mb200_last_error()
+    return msg.decode() if msg else "?"
 
 
 def set_decode_timeline(buf: Optional[torch.Tensor]) -> None:

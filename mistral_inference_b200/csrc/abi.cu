@@ -38,7 +38,7 @@ struct DecodePlan {
   size_t xs_bytes, smem;
 };
 static int decode_plan(int64_t dim, int64_t hidden, int64_t n_heads, int64_t n_kv_heads, int64_t head_dim, int64_t vocab, int64_t n_experts,
-                       int64_t top_k, int64_t smem_max, DecodePlan* out) {
+                       int64_t top_k, int64_t smem_max, DecodePlan* out, bool w8 = false) {
   MB_CHECK_ARG(head_dim == kHeadDim, "decode_step: head_dim=%lld unsupported (128 only)", (long long)head_dim);
   MB_CHECK_ARG(dim > 0 && hidden > 0 && n_kv_heads >= 1 && n_heads % n_kv_heads == 0, "decode_step: H %% KV != 0");
   const int64_t rep = n_heads / n_kv_heads;
@@ -49,6 +49,10 @@ static int decode_plan(int64_t dim, int64_t hidden, int64_t n_heads, int64_t n_k
   const int64_t q_dim = n_heads * head_dim;
   auto cut_ok = [](int64_t K) { const int64_t nch = (K + MK_MAX_KC - 1) / MK_MAX_KC; return K % (nch * 8) == 0; };
   MB_CHECK_ARG(cut_ok(dim) && cut_ok(hidden) && cut_ok(q_dim), "decode_step: dim/hidden/q_dim must split into 16-byte-aligned row chunks");
+  // e4m3 layer matrices (cut_matrix with w8): chunks of up to MK_MAX_KC8 bytes, 16-byte aligned
+  auto cut8_ok = [](int64_t K) { const int64_t nch = (K + MK_MAX_KC8 - 1) / MK_MAX_KC8; return K % (nch * 16) == 0; };
+  MB_CHECK_ARG(!w8 || (cut8_ok(dim) && cut8_ok(hidden) && cut8_ok(q_dim)), "decode_step (fp8): dim/hidden/q_dim must split into 16-byte row chunks");
+  MB_CHECK_ARG(!w8 || n_experts == 0, "decode_step (fp8): dense models only");
   MB_CHECK_ARG(vocab > 0 && vocab % 2 == 0, "decode_step: vocab must be even");
   MB_CHECK_ARG(n_experts == 0 || (top_k >= 1 && top_k <= MK_MAX_TOPK && top_k <= n_experts && n_experts <= 32),
                "decode_step: bad MoE arguments (E=%lld, k=%lld)", (long long)n_experts, (long long)top_k);
@@ -113,6 +117,47 @@ static int run_linear(const void* x, const void* norm_w, const void* w, const Ep
   if (streamk_eligible(T, N, K)) return launch_streamk<MODE>(g, workspace, workspace_bytes, st);  // decode-sized batches: HBM-bound
   if (wgmma_gemm_eligible(T, N, K)) return launch_gemm_wgmma<MODE>(g, st);
   return launch_gemm_mma<MODE>(g, st);
+}
+
+// FP8 dense weights (include/mistral_b200.h): w is e4m3 [N, K], epi.w_scale its fp32 row scales.  The bf16 dispatch, except that
+// a shape run_linear would give to gemm_mma_kernel is refused: that kernel has no e4m3 variant.
+template <int MODE>
+static int run_linear_fp8(const void* x, const void* norm_w, const void* w, const EpiParams& epi, int64_t T, int64_t N, int64_t K, float eps,
+                          void* workspace, size_t workspace_bytes, cudaStream_t st) {
+  MB_CHECK_ARG(T >= 1, "linear (fp8): T=%lld", (long long)T);
+  MB_CHECK_ARG(epi.w_scale != nullptr && ((uintptr_t)epi.w_scale & 7) == 0, "linear (fp8): w_scale must be an 8-byte aligned fp32 array");
+  if (T <= MB200_SKINNY_MAX_T) {
+    SkinnyParams p;
+    p.x = x;
+    p.norm_w = norm_w;
+    p.w = w;
+    p.N = (int)N;
+    p.K = (int)K;
+    p.eps = eps;
+    p.epi = epi;
+    return norm_w ? launch_skinny_fp8<MODE | EPI_WSCALE, true>(p, (int)T, st) : launch_skinny_fp8<MODE | EPI_WSCALE, false>(p, (int)T, st);
+  }
+  const bool sk = streamk_eligible(T, N, K);
+  MB_CHECK_ARG(sk || wgmma_gemm_eligible(T, N, K), "linear (fp8): T=%lld N=%lld K=%lld needs the mma.sync GEMM, which has no e4m3 variant",
+               (long long)T, (long long)N, (long long)K);
+  const void* a = x;
+  if (norm_w) {
+    const WsRegion nr = ws_normed(T, K);
+    if (workspace == nullptr || workspace_bytes < nr.end()) return fail(MB200_E_WORKSPACE, "linear: workspace %zu < %zu", workspace_bytes, nr.end());
+    void* normed = (uint8_t*)workspace + nr.offset;
+    int rc = run_rmsnorm(x, norm_w, normed, T, K, eps, st);
+    if (rc) return rc;
+    a = normed;
+  }
+  GemmParams g;
+  g.a = a;
+  g.w = w;
+  g.T = (int)T;
+  g.N = (int)N;
+  g.K = (int)K;
+  g.epi = epi;
+  if (sk) return launch_streamk_fp8<MODE | EPI_WSCALE>(g, workspace, workspace_bytes, st);
+  return launch_gemm_wgmma_fp8<MODE | EPI_WSCALE>(g, st);
 }
 
 // Un-merged LoRA around one fused Linear (include/mistral_b200.h): down projection -> up projection -> base GEMM whose epilogue
@@ -201,7 +246,7 @@ int mb200_rmsnorm(const void* x, const void* w, void* out, int64_t T, int64_t di
 static int attn_qkv_impl(const void* x, const void* norm_w, const void* wqkv, const float* rope, const int32_t* positions, void* q_out,
                          void* k_out, void* v_out, void* cache_k, void* cache_v, const int32_t* cache_rows, int64_t T, int64_t dim,
                          int64_t n_heads, int64_t n_kv_heads, int64_t head_dim, float eps, void* workspace, size_t workspace_bytes,
-                         void* stream, const mb200_lora* lora) {
+                         void* stream, const mb200_lora* lora, const float* w_scale = nullptr) {
   MB_CHECK_ARG(x && norm_w && wqkv && rope && positions && q_out && k_out && v_out, "attn_qkv: null pointer");
   MB_CHECK_ARG(head_dim == kHeadDim || head_dim == 64, "attn_qkv: head_dim=%lld unsupported (64 or 128)", (long long)head_dim);
   MB_CHECK_ARG(cache_rows == nullptr || (cache_k && cache_v), "attn_qkv: cache_rows without cache pointers");
@@ -218,6 +263,10 @@ static int attn_qkv_impl(const void* x, const void* norm_w, const void* wqkv, co
   e.kv_dim = (int)(n_kv_heads * head_dim);
   e.head_dim = (int)head_dim;
   const int64_t N = (n_heads + 2 * n_kv_heads) * head_dim;
+  if (w_scale) {
+    e.w_scale = w_scale;
+    return run_linear_fp8<EPI_QKV_ROPE>(x, norm_w, wqkv, e, T, N, dim, eps, workspace, workspace_bytes, (cudaStream_t)stream);
+  }
   if (lora) return run_linear_lora<EPI_QKV_ROPE>(x, norm_w, wqkv, e, lora, T, N, dim, eps, workspace, workspace_bytes, (cudaStream_t)stream);
   return run_linear<EPI_QKV_ROPE>(x, norm_w, wqkv, e, T, N, dim, eps, workspace, workspace_bytes, (cudaStream_t)stream);
 }
@@ -461,6 +510,36 @@ int mb200_linear_residual(const void* x, const void* w, const void* residual, vo
   e.ld_out = N;
   if (residual) return run_linear<EPI_RESIDUAL>(x, nullptr, w, e, T, N, K, 0.f, workspace, workspace_bytes, (cudaStream_t)stream);
   return run_linear<EPI_STORE>(x, nullptr, w, e, T, N, K, 0.f, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+int mb200_attn_qkv_fp8(const void* x, const void* norm_w, const void* w_q, const float* w_scale, const float* rope, const int32_t* positions,
+                       void* q_out, void* k_out, void* v_out, void* cache_k, void* cache_v, const int32_t* cache_rows, int64_t T, int64_t dim,
+                       int64_t n_heads, int64_t n_kv_heads, int64_t head_dim, float eps, void* workspace, size_t workspace_bytes, void* stream) {
+  MB_CHECK_ARG(w_scale, "attn_qkv_fp8: null scale");
+  return attn_qkv_impl(x, norm_w, w_q, rope, positions, q_out, k_out, v_out, cache_k, cache_v, cache_rows, T, dim, n_heads, n_kv_heads,
+                       head_dim, eps, workspace, workspace_bytes, stream, nullptr, w_scale);
+}
+
+int mb200_linear_residual_fp8(const void* x, const void* w_q, const float* w_scale, const void* residual, void* out, int64_t T, int64_t N,
+                              int64_t K, void* workspace, size_t workspace_bytes, void* stream) {
+  MB_CHECK_ARG(x && w_q && w_scale && out, "linear_residual_fp8: null pointer");
+  EpiParams e;
+  e.out = out;
+  e.residual = residual;
+  e.ld_out = N;
+  e.w_scale = w_scale;
+  if (residual) return run_linear_fp8<EPI_RESIDUAL>(x, nullptr, w_q, e, T, N, K, 0.f, workspace, workspace_bytes, (cudaStream_t)stream);
+  return run_linear_fp8<EPI_STORE>(x, nullptr, w_q, e, T, N, K, 0.f, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+int mb200_ffn_gateup_fp8(const void* x, const void* norm_w, const void* w_q, const float* w_scale, void* g_out, int64_t T, int64_t dim,
+                         int64_t hidden, float eps, void* workspace, size_t workspace_bytes, void* stream) {
+  MB_CHECK_ARG(x && w_q && w_scale && g_out, "ffn_gateup_fp8: null pointer");
+  EpiParams e;
+  e.out = g_out;
+  e.ld_out = hidden;
+  e.w_scale = w_scale;
+  return run_linear_fp8<EPI_SWIGLU>(x, norm_w, w_q, e, T, 2 * hidden, dim, eps, workspace, workspace_bytes, (cudaStream_t)stream);
 }
 
 int mb200_linear_residual_lora(const void* x, const void* w, const void* residual, void* out, int64_t T, int64_t N, int64_t K,
@@ -765,13 +844,17 @@ int mb200_comm_close(void* ptr) {
   return MB200_OK;
 }
 
-int mb200_decode_step(const mb200_layer_desc* layers_dev, const int32_t* windows_dev, int64_t n_layers, const void* emb, const void* final_norm,
-                      const void* w_out, const float* rope, const int64_t* token_dev, int64_t pos, int64_t batch_row, float* logits,
-                      int64_t* next_token_dev, int64_t dim,
-                      int64_t hidden, int64_t n_heads, int64_t n_kv_heads, int64_t head_dim, int64_t vocab, float eps, int64_t n_experts,
-                      int64_t top_k, const void* const* moe_gate_dev, const void* const* moe_w13_dev, const void* const* moe_w2_dev,
-                      void* workspace, size_t workspace_bytes, void* stream) {
+}  // extern "C"
+
+// mb200_decode_step and mb200_decode_step_fp8 (w8: layers_dev is an mb200_layer_desc_fp8 array, dense only)
+static int decode_step_impl(const void* layers_dev, const int32_t* windows_dev, int64_t n_layers, const void* emb, const void* final_norm,
+                            const void* w_out, const float* rope, const int64_t* token_dev, int64_t pos, int64_t batch_row, float* logits,
+                            int64_t* next_token_dev, int64_t dim, int64_t hidden, int64_t n_heads, int64_t n_kv_heads, int64_t head_dim,
+                            int64_t vocab, float eps, int64_t n_experts, int64_t top_k, const void* const* moe_gate_dev,
+                            const void* const* moe_w13_dev, const void* const* moe_w2_dev, void* workspace, size_t workspace_bytes, void* stream,
+                            bool w8) {
   static_assert(sizeof(mb200_layer_desc) == sizeof(MkLayer), "layer descriptor layout");
+  static_assert(sizeof(mb200_layer_desc_fp8) == sizeof(MkLayerFp8), "FP8 layer descriptor layout");
   MB_CHECK_ARG(layers_dev && windows_dev && emb && final_norm && w_out && rope && token_dev && logits && workspace, "decode_step: null pointer");
   MB_CHECK_ARG(n_experts == 0 || (moe_gate_dev && moe_w13_dev && moe_w2_dev), "decode_step: MoE weight tables missing");
   int dev = 0, sms = 0, smem_max = 0, coop = 0;
@@ -781,7 +864,7 @@ int mb200_decode_step(const mb200_layer_desc* layers_dev, const int32_t* windows
   MB_CHECK_CUDA(cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev));
   MB_CHECK_ARG(coop, "decode_step: device does not support cooperative launch");
   DecodePlan plan;
-  const int rc = decode_plan(dim, hidden, n_heads, n_kv_heads, head_dim, vocab, n_experts, top_k, smem_max, &plan);
+  const int rc = decode_plan(dim, hidden, n_heads, n_kv_heads, head_dim, vocab, n_experts, top_k, smem_max, &plan, w8);
   if (rc) return rc;
   const int rep = plan.rep;
 
@@ -834,17 +917,54 @@ int mb200_decode_step(const mb200_layer_desc* layers_dev, const int32_t* windows
   void* args[] = {(void*)&p};
   const void* fn = nullptr;
   switch (rep) {
-    case 1: fn = (const void*)decode_megakernel<1>; break;
-    case 2: fn = (const void*)decode_megakernel<2>; break;
-    case 4: fn = (const void*)decode_megakernel<4>; break;
-    case 6: fn = (const void*)decode_megakernel<6>; break;
-    case 8: fn = (const void*)decode_megakernel<8>; break;
+    case 1: fn = w8 ? (const void*)decode_megakernel<1, true> : (const void*)decode_megakernel<1>; break;
+    case 2: fn = w8 ? (const void*)decode_megakernel<2, true> : (const void*)decode_megakernel<2>; break;
+    case 4: fn = w8 ? (const void*)decode_megakernel<4, true> : (const void*)decode_megakernel<4>; break;
+    case 6: fn = w8 ? (const void*)decode_megakernel<6, true> : (const void*)decode_megakernel<6>; break;
+    case 8: fn = w8 ? (const void*)decode_megakernel<8, true> : (const void*)decode_megakernel<8>; break;
     default: return fail(MB200_E_INVALID, "decode_step: H/KV=%d unsupported (1,2,4,6,8)", rep);
   }
-  note_launch("decode_megakernel<%d>", rep);
+  if (w8)
+    note_launch("decode_megakernel<%d, true>", rep);
+  else
+    note_launch("decode_megakernel<%d>", rep);
   MB_CHECK_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   MB_CHECK_CUDA(cudaLaunchCooperativeKernel(fn, dim3((unsigned)sms), dim3(MK_THREADS), args, smem, (cudaStream_t)stream));
   return MB200_OK;
+}
+
+extern "C" {
+
+int mb200_decode_step(const mb200_layer_desc* layers_dev, const int32_t* windows_dev, int64_t n_layers, const void* emb, const void* final_norm,
+                      const void* w_out, const float* rope, const int64_t* token_dev, int64_t pos, int64_t batch_row, float* logits,
+                      int64_t* next_token_dev, int64_t dim,
+                      int64_t hidden, int64_t n_heads, int64_t n_kv_heads, int64_t head_dim, int64_t vocab, float eps, int64_t n_experts,
+                      int64_t top_k, const void* const* moe_gate_dev, const void* const* moe_w13_dev, const void* const* moe_w2_dev,
+                      void* workspace, size_t workspace_bytes, void* stream) {
+  return decode_step_impl(layers_dev, windows_dev, n_layers, emb, final_norm, w_out, rope, token_dev, pos, batch_row, logits, next_token_dev, dim,
+                          hidden, n_heads, n_kv_heads, head_dim, vocab, eps, n_experts, top_k, moe_gate_dev, moe_w13_dev, moe_w2_dev, workspace,
+                          workspace_bytes, stream, false);
+}
+
+int mb200_decode_step_fp8(const mb200_layer_desc_fp8* layers_dev, const int32_t* windows_dev, int64_t n_layers, const void* emb,
+                          const void* final_norm, const void* w_out, const float* rope, const int64_t* token_dev, int64_t pos,
+                          int64_t batch_row, float* logits, int64_t* next_token_dev, int64_t dim, int64_t hidden, int64_t n_heads,
+                          int64_t n_kv_heads, int64_t head_dim, int64_t vocab, float eps, void* workspace, size_t workspace_bytes, void* stream) {
+  return decode_step_impl(layers_dev, windows_dev, n_layers, emb, final_norm, w_out, rope, token_dev, pos, batch_row, logits, next_token_dev, dim,
+                          hidden, n_heads, n_kv_heads, head_dim, vocab, eps, 0, 0, nullptr, nullptr, nullptr, workspace, workspace_bytes, stream,
+                          true);
+}
+
+int mb200_decode_step_fp8_supported(int64_t dim, int64_t hidden, int64_t n_heads, int64_t n_kv_heads, int64_t head_dim, int64_t vocab,
+                                    int64_t smem_optin) {
+  if (smem_optin <= 0) {
+    int dev = 0, smem_max = 0;
+    MB_CHECK_CUDA(cudaGetDevice(&dev));
+    MB_CHECK_CUDA(cudaDeviceGetAttribute(&smem_max, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
+    smem_optin = smem_max;
+  }
+  DecodePlan plan;
+  return decode_plan(dim, hidden, n_heads, n_kv_heads, head_dim, vocab, 0, 0, smem_optin, &plan, true);
 }
 
 int mb200_debug_decode_scratch(int64_t dim, int64_t hidden, int64_t n_heads, int64_t n_kv_heads, int64_t head_dim, int64_t n_experts,

@@ -1,6 +1,8 @@
 // Shared device/host helpers for libmb200 (sm_90a only).
 #pragma once
 #include <cuda_bf16.h>
+#include <cuda_fp16.h>
+#include <cuda_fp8.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -75,6 +77,14 @@ __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
   return (uint32_t)bf16_bits(lo) | ((uint32_t)bf16_bits(hi) << 16);
 }
 __device__ __forceinline__ float bf16_to_float(uint16_t b) { return __uint_as_float(((uint32_t)b) << 16); }
+
+// ---- e4m3 -> fp32, exactly ----------------------------------------------------------------------
+// Two e4m3 bytes (low byte first) -> their values: cvt.rn.f16x2.e4m3x2 is exact (every e4m3 value is an f16 value) and so is f16 ->
+// f32 -- three instructions per pair, no rounding.  Every e4m3 value is also a bf16 value, so a bf16 pack of the result is exact too.
+__device__ __forceinline__ float2 e4m3x2_to_float2(uint32_t two) {
+  const __half2_raw h = __nv_cvt_fp8x2_to_halfraw2((__nv_fp8x2_storage_t)(two & 0xffffu), __NV_E4M3);
+  return __half22float2(*reinterpret_cast<const __half2*>(&h));
+}
 
 // ---- memory ----------------------------------------------------------------------------------
 // streaming 16-byte load that does not pollute L1 (weights / KV rows are read exactly once per step)

@@ -35,6 +35,7 @@ constexpr int MK_PRODUCER_WARPS = 2;  // one issuing thread each, stages dealt r
 constexpr int MK_THREADS = MK_CONSUMERS + 32 * MK_PRODUCER_WARPS;
 constexpr int MK_WEIGHT_STAGE_BYTES = 16 * 1024;   // a weight stage: 2 rows x KC elements x 2 B
 constexpr int MK_MAX_KC = MK_WEIGHT_STAGE_BYTES / 4;  // elements per row chunk
+constexpr int MK_MAX_KC8 = MK_WEIGHT_STAGE_BYTES / 2;  // elements per row chunk of an e4m3 matrix (FP8 dense weights)
 constexpr int MK_KV_PAD = 16;                      // K/V position rows are laid out with a 16-byte pad (ldmatrix bank spread)
 constexpr int MK_STAGE_BYTES = 16 * 1024 + 16 * MK_KV_PAD;  // ring slot stride: also fits 8 padded 2 KB K/V position rows
 constexpr int MK_MAX_STAGES = 12;
@@ -51,8 +52,18 @@ struct MkLayer {  // 64 bytes, device array prepared by the caller (include/mist
   bf16* cache_v;
 };
 
+// FP8 dense weights (include/mistral_b200.h: mb200_layer_desc_fp8): wqkv / wo / w13 / w2 of `w` point to e4m3 [N, K] matrices,
+// s_* to their fp32 row scales.  The norms, the K/V ring and the lm head stay bf16.
+struct MkLayerFp8 {
+  MkLayer w;
+  const float* s_qkv;
+  const float* s_o;
+  const float* s_13;
+  const float* s_2;
+};
+
 struct MkParams {
-  const MkLayer* layers;
+  const MkLayer* layers;  // W8: an MkLayerFp8 array
   const int32_t* windows;  // [n_layers] ring size per layer
   // Mixture of experts (moe.py:16-32): n_experts == 0 -> dense FeedForward (layers[l].w13 / w2)
   int n_experts, top_k;
@@ -223,17 +234,30 @@ __device__ __forceinline__ void grid_barrier(const MkParams& p, int tid, unsigne
 }
 
 // How a [N, K] matrix is cut for the ring: pairs of rows, K in `nch` chunks of `kc` elements.
+// An e4m3 matrix (w8) is cut with twice the elements per chunk: a stage carries at most the same 16 KB (7B's dim-4096 rows: 8 KB).
 struct MatCut {
   int pairs, nch, kc, p0, p1;
 };
-__device__ __forceinline__ MatCut cut_matrix(int N, int K) {
+__device__ __forceinline__ MatCut cut_matrix(int N, int K, bool w8 = false) {
   MatCut c;
   c.pairs = N >> 1;
-  c.nch = (K + MK_MAX_KC - 1) / MK_MAX_KC;
+  const int max_kc = w8 ? MK_MAX_KC8 : MK_MAX_KC;
+  c.nch = (K + max_kc - 1) / max_kc;
   c.kc = K / c.nch;
   c.p0 = (int)(((long long)blockIdx.x * c.pairs) / gridDim.x);
   c.p1 = (int)(((long long)(blockIdx.x + 1) * c.pairs) / gridDim.x);
   return c;
+}
+
+// FP8 dense weights: an e4m3 matrix whose rows are at most 4 KB (7B's dim-4096 rows) carries TWO pairs per stage, so that a stage
+// stays at 16 KB (the bytes in flight of the bf16 ring, the same per-stage cost for the producers).  Warps 2i and 2i + 1 of a group
+// read stage i (the two pairs are four contiguous rows); each arrives MK_CONSUMER_WARPS / 2 times on its empty barrier, or
+// MK_CONSUMER_WARPS when its pair is alone in the stage (the last pair of an odd group).  A group of g pairs has (g + 1) / 2 stages,
+// so a warp's stages stay within one lap of the ring (tests/test_fp8_dense_cpu.py model-checks the order).
+__device__ __forceinline__ bool two_pairs_per_stage(const MatCut& c, bool w8) { return w8 && c.nch == 1 && 4 * c.kc <= MK_WEIGHT_STAGE_BYTES; }
+__device__ __forceinline__ int matrix_stages(const MatCut& c, bool w8) {
+  const int P = c.p1 - c.p0;
+  return two_pairs_per_stage(c, w8) ? (P / MK_CONSUMER_WARPS) * (MK_CONSUMER_WARPS / 2) + ((P % MK_CONSUMER_WARPS) + 1) / 2 : P * c.nch;
 }
 
 // routing decision of one MoE layer (moe.py:24-32), produced on every CTA by moe_route
@@ -295,10 +319,12 @@ struct StageCopy {
 
 enum : int { SEG_QKV, SEG_KV, SEG_WO, SEG_UP, SEG_DOWN };  // segments of a layer, in stream order (SEG_UP once per expert)
 
+template <bool W8 = false>
 struct Walk {
   uint32_t it;              // running stage number (the consumers' RingState::it of the same stage)
   int layer, seg, e, s, n;  // layer (n_layers: the lm head), segment, gate/up expert of a MoE layer, stage s of the segment's n
   MatCut c;                 // matrix: its cut (row length c.kc * c.nch)
+  bool w8;                  // W8: the matrix is e4m3 (every layer matrix; not the lm head)
   int k_begin, k_end, pps;  // K/V slice: positions and positions per stage (attn_slice)
   const bf16* W;            // matrix (unused in a MoE down segment: one per routed expert), or the K rows of the K/V slice
   const bf16* V;            // V rows of the K/V slice
@@ -308,10 +334,11 @@ struct Walk {
   __device__ __forceinline__ bool gated(const MkParams& p, int routed) const {
     return p.n_experts != 0 && layer < p.n_layers && seg == SEG_UP && e == 0 && routed != layer;
   }
-  __device__ __forceinline__ void matrix(const bf16* w, int N, int K) {
+  __device__ __forceinline__ void matrix(const bf16* w, int N, int K, bool e4m3 = false) {
     W = w;
-    c = cut_matrix(N, K);
-    n = (c.p1 - c.p0) * c.nch;
+    w8 = e4m3;
+    c = cut_matrix(N, K, e4m3);
+    n = matrix_stages(c, e4m3);
   }
   // experts interleaved per group of pairs: the routed ones in the down segment of a MoE layer, else 1
   __device__ __forceinline__ int experts(const MkParams& p) const { return (seg == SEG_DOWN && p.n_experts) ? p.top_k : 1; }
@@ -323,9 +350,9 @@ struct Walk {
       matrix(p.w_out, p.vocab, p.dim);
       return;
     }
-    const MkLayer& L = p.layers[layer];
+    const MkLayer& L = W8 ? reinterpret_cast<const MkLayerFp8*>(p.layers)[layer].w : p.layers[layer];
     if (seg == SEG_QKV) {
-      matrix(L.wqkv, q_dim + 2 * kv_dim, p.dim);
+      matrix(L.wqkv, q_dim + 2 * kv_dim, p.dim, W8);
     } else if (seg == SEG_KV) {
       const int win = p.windows[layer];
       const AttnSlice a = attn_slice(p, win);
@@ -336,11 +363,11 @@ struct Walk {
       W = L.cache_k + ((int64_t)p.batch_row * win) * kv_dim;
       V = L.cache_v + ((int64_t)p.batch_row * win) * kv_dim;
     } else if (seg == SEG_WO) {
-      matrix(L.wo, p.dim, q_dim);
+      matrix(L.wo, p.dim, q_dim, W8);
     } else if (seg == SEG_UP) {
-      matrix(p.n_experts ? p.moe_w13[layer * p.n_experts + ((sel >> (8 * e)) & 0xff)] : L.w13, 2 * p.hidden, p.dim);
+      matrix(p.n_experts ? p.moe_w13[layer * p.n_experts + ((sel >> (8 * e)) & 0xff)] : L.w13, 2 * p.hidden, p.dim, W8);
     } else {
-      matrix(L.w2, p.dim, p.hidden);
+      matrix(L.w2, p.dim, p.hidden, W8);
       n *= experts(p);
     }
   }
@@ -397,6 +424,29 @@ struct Walk {
     const int j = r / (c.nch * g), r2 = r - j * (c.nch * g);
     const int ch = r2 / g, w = r2 - ch * g;
     const bf16* m = (seg == SEG_DOWN && p.n_experts) ? p.moe_w2[layer * p.n_experts + ((sel >> (8 * j)) & 0xff)] : W;
+    if (W8 && w8 && two_pairs_per_stage(c, true)) {  // e4m3, two pairs (four contiguous rows) per stage
+      constexpr int kStagesPerGroup = MK_CONSUMER_WARPS / 2;
+      const int g0 = c.p0 + (s / kStagesPerGroup) * MK_CONSUMER_WARPS, first = g0 + 2 * (s % kStagesPerGroup);
+      sc.src = m + (int64_t)first * K;  // K bytes per row, in bf16 units: pair p starts at row 2p
+      sc.src_step = 0;
+      sc.bytes = (uint32_t)(min(2, c.p1 - first) * 2 * c.kc);
+      sc.dst_step = 0;
+      sc.count = 1;
+      return sc;
+    }
+    if (W8 && w8) {  // e4m3: K bytes per row, in bf16 units (K and kc are multiples of 16)
+      const bf16* r8 = m + (int64_t)(g0 + w) * K;
+      sc.bytes = (uint32_t)c.kc;
+      sc.src = r8 + ((c.nch == 1) ? 0 : ch * (c.kc >> 1));
+      sc.src_step = K >> 1;
+      sc.dst_step = sc.bytes;
+      sc.count = 2;
+      if (c.nch == 1) {  // the two rows are contiguous
+        sc.bytes *= 2;
+        sc.count = 1;
+      }
+      return sc;
+    }
     const bf16* r0 = m + (int64_t)(2 * (g0 + w)) * K;
     sc.bytes = (uint32_t)c.kc * 2;
     if (c.nch == 1) {  // the two rows are contiguous
@@ -435,7 +485,7 @@ __device__ __forceinline__ unsigned long long globaltimer() {
 // every stage, K/V slice stages included.
 constexpr int MK_INFLIGHT_CAP = 5;
 static_assert(MK_INFLIGHT_CAP <= MK_CONSUMER_WARPS, "below the smallest ring decode_plan accepts (n_stages > MK_CONSUMER_WARPS)");
-
+template <bool W8 = false>
 struct Producer {
   uint8_t* ring;
   uint64_t* full;
@@ -464,7 +514,7 @@ struct Producer {
   // fills the ring slot of the copy cursor's stage once stage it - cap has landed (its slot cannot have been refilled yet) and
   // the slot is free.  With the timeline on, the time blocked on either condition is added to the producer's words of the
   // copy cursor's layer.
-  __device__ __forceinline__ void copy(const MkParams& p, const Walk& cp) {
+  __device__ __forceinline__ void copy(const MkParams& p, const Walk<W8>& cp) {
     bool landed = cp.it < (uint32_t)MK_INFLIGHT_CAP || mbar_try_wait(&full[cslot], cpar);
     if (!landed || !mbar_try_wait(&empty[slot], par ^ 1)) {
       const unsigned long long t0 = prof != nullptr ? globaltimer() : 0ull;
@@ -495,9 +545,10 @@ struct Producer {
   }
 };
 
+template <bool W8 = false>
 __device__ __forceinline__ void producer_main(const MkParams& p, uint8_t* ring, uint64_t* full, uint64_t* empty, int me, const MoeRoute* route,
                                               uint64_t* route_bar) {
-  Producer pr;
+  Producer<W8> pr;
   pr.ring = ring;
   pr.full = full;
   pr.empty = empty;
@@ -508,7 +559,7 @@ __device__ __forceinline__ void producer_main(const MkParams& p, uint8_t* ring, 
   pr.routed = -1;
   pr.prof = (p.prof != nullptr && blockIdx.x % 21 == 0) ? p.prof + (int64_t)(blockIdx.x / 21) * p.n_layers * MK_PROF_WORDS : nullptr;
   asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pr.policy));
-  Walk cp;
+  Walk<W8> cp;
   cp.it = 0;
   cp.layer = cp.seg = cp.e = 0;
   cp.settle(p, pr.sel, pr.routed);
@@ -562,31 +613,86 @@ __device__ __forceinline__ void consume_pair_stage(const uint8_t* ring, uint64_t
   if (lane == 0) mbar_arrive_n(&empty[slot], MK_CONSUMER_WARPS);
 }
 
+// The same for a stage of an e4m3 pair (FP8 dense weights): kq 16-byte chunks per row, each 16 weights converted exactly
+// (e4m3x2_to_float2) and FMA'd against x chunks 2i, 2i + 1 in the bf16 path's element order.
+// The pair's rows start `row0` 16-byte chunks into the stage; the warp arrives `arrivals` times on the empty barrier.
+__device__ __forceinline__ void consume_pair_stage_w8(const uint8_t* ring, uint64_t* full, uint64_t* empty, int n_stages, uint32_t it,
+                                                      const uint4* xc, int kq, int row0, uint32_t arrivals, int lane, float& a0, float& a1) {
+  const uint32_t slot = it % n_stages, par = (it / n_stages) & 1;
+  mbar_wait(&empty[slot], par ^ 1, 2, it);  // see consume_pair_stage
+  mbar_wait(&full[slot], par, 3, it);
+  const uint4* w0 = reinterpret_cast<const uint4*>(ring + (size_t)slot * MK_STAGE_BYTES) + row0;
+  const uint4* w1 = w0 + kq;
+#pragma unroll 2
+  for (int i = lane; i < kq; i += 32) {
+    const uint4 a = w0[i], b = w1[i];
+    const uint32_t aq[4] = {a.x, a.y, a.z, a.w}, bq[4] = {b.x, b.y, b.z, b.w};
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const uint4 x = xc[2 * i + h];
+      const uint32_t xw[4] = {x.x, x.y, x.z, x.w};
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const float2 af = e4m3x2_to_float2(aq[2 * h + (j >> 1)] >> (16 * (j & 1)));
+        const float2 bf = e4m3x2_to_float2(bq[2 * h + (j >> 1)] >> (16 * (j & 1)));
+        const float xl = bf16lo(xw[j]), xh = bf16hi(xw[j]);
+        a0 = fmaf(af.x, xl, a0);
+        a0 = fmaf(af.y, xh, a0);
+        a1 = fmaf(bf.x, xl, a1);
+        a1 = fmaf(bf.y, xh, a1);
+      }
+    }
+  }
+  __syncwarp();
+  if (lane == 0) mbar_arrive_n(&empty[slot], arrivals);
+}
+
 // ---- consumers: y[pair] = W[pair rows] . xs, epilogue(pair, acc0, acc1) on one lane ----------------
 // Warp-per-pair inside a group: warp w owns pair g0+w and consumes its `nch` stages by itself.  One block barrier per GROUP
 // keeps all warps within a group of each other (see the stage-order note above).
 // `pre(n)` runs on the finishing lane BEFORE the pair's stages are consumed and its result is handed to `epi`: loads the
 // epilogue needs (the residual) are then off the critical path of the phase's last pair (an L2 round trip right before the
 // barrier's release store: measured 3.2-4.2 us barrier latency after wo / down vs 1.75 us after gate/up, which loads nothing).
-template <class Pre, class Epi>
+// W8: an e4m3 matrix with fp32 row scales `wscale`; the finishing lane loads the pair's scales with `pre` and hands
+// epi fp32(s * acc), the one product of the FP8 definition, in place of acc.
+template <bool W8 = false, class Pre, class Epi>
 __device__ __forceinline__ void consume_matrix(int N, int K, const uint8_t* ring, uint64_t* full, uint64_t* empty, int n_stages, RingState& rs,
-                                               const uint4* xs, int tid, Pre pre, Epi epi) {
-  const MatCut c = cut_matrix(N, K);
+                                               const uint4* xs, int tid, Pre pre, Epi epi, const float* wscale = nullptr) {
+  const MatCut c = cut_matrix(N, K, W8);
+  const bool two = two_pairs_per_stage(c, W8);
   const int lane = tid & 31, warp = tid >> 5;
   const int kc8 = c.kc >> 3;  // 16-byte chunks per row chunk
   for (int g0 = c.p0; g0 < c.p1; g0 += MK_CONSUMER_WARPS) {
     const int g = min(MK_CONSUMER_WARPS, c.p1 - g0);
+    const int g_stages = two ? (g + 1) >> 1 : g * c.nch;
     if (warp < g) {
       uint2 prefetched = make_uint2(0u, 0u);
-      if (lane == 0) prefetched = pre(2 * (g0 + warp));
+      float2 ws = make_float2(1.f, 1.f);
+      if (lane == 0) {
+        prefetched = pre(2 * (g0 + warp));
+        if constexpr (W8) ws = __ldg(reinterpret_cast<const float2*>(wscale + 2 * (g0 + warp)));
+      }
       float a0 = 0.f, a1 = 0.f;
-      for (int ch = 0; ch < c.nch; ++ch)
-        consume_pair_stage(ring, full, empty, n_stages, rs.it + (uint32_t)(ch * g + warp), xs + ch * kc8, kc8, lane, a0, a1);
+      for (int ch = 0; ch < c.nch; ++ch) {
+        if constexpr (W8) {
+          if (two)
+            consume_pair_stage_w8(ring, full, empty, n_stages, rs.it + (uint32_t)(warp >> 1), xs, c.kc >> 4, (warp & 1) * (c.kc >> 3),
+                                  (warp == g - 1 && (g & 1)) ? MK_CONSUMER_WARPS : MK_CONSUMER_WARPS / 2, lane, a0, a1);
+          else
+            consume_pair_stage_w8(ring, full, empty, n_stages, rs.it + (uint32_t)(ch * g + warp), xs + ch * kc8, c.kc >> 4, 0, MK_CONSUMER_WARPS,
+                                  lane, a0, a1);
+        } else
+          consume_pair_stage(ring, full, empty, n_stages, rs.it + (uint32_t)(ch * g + warp), xs + ch * kc8, kc8, lane, a0, a1);
+      }
       a0 = warp_sum(a0);
       a1 = warp_sum(a1);
+      if constexpr (W8) {
+        a0 = __fmul_rn(ws.x, a0);
+        a1 = __fmul_rn(ws.y, a1);
+      }
       if (lane == 0) epi(2 * (g0 + warp), a0, a1, prefetched);
     }
-    rs.it += (uint32_t)(g * c.nch);
+    rs.it += (uint32_t)g_stages;
     consumer_sync();
   }
 }
@@ -944,7 +1050,8 @@ __device__ __forceinline__ void consume_moe_down(const MkParams& p, const MoeRou
   }
 }
 
-template <int REP>
+// W8: FP8 dense weights (p.layers is an MkLayerFp8 array, no MoE): every layer matrix streams as e4m3, the lm head as bf16.
+template <int REP, bool W8 = false>
 __global__ void __launch_bounds__(MK_THREADS, 1) decode_megakernel(const MkParams p) {
   extern __shared__ __align__(128) uint8_t smem[];
   // layout: [ring: n_stages x 16 KB][xs: xs_bytes][barriers][reduction scratch]
@@ -973,7 +1080,7 @@ __global__ void __launch_bounds__(MK_THREADS, 1) decode_megakernel(const MkParam
 
   if (tid >= MK_CONSUMERS) {
     // ================= producers (one thread per producer warp; weights and old K/V rows never wait for activations) =================
-    if ((tid & 31) == 0) producer_main(p, ring, full, empty, (tid - MK_CONSUMERS) >> 5, route, route_bar);
+    if ((tid & 31) == 0) producer_main<W8>(p, ring, full, empty, (tid - MK_CONSUMERS) >> 5, route, route_bar);
     return;
   }
 
@@ -983,7 +1090,8 @@ __global__ void __launch_bounds__(MK_THREADS, 1) decode_megakernel(const MkParam
   unsigned epoch = ld_acquire_u32(p.bar_epoch);
   const int64_t token = *p.token;
   for (int l = 0; l < p.n_layers; ++l) {
-    const MkLayer L = p.layers[l];
+    const MkLayer L = W8 ? reinterpret_cast<const MkLayerFp8*>(p.layers)[l].w : p.layers[l];
+    const MkLayerFp8* L8 = W8 ? reinterpret_cast<const MkLayerFp8*>(p.layers) + l : nullptr;
     const int W = p.windows[l];
     const bf16* x_in = (l == 0) ? p.emb + token * p.dim : p.xbuf + (size_t)(l & 1) * p.dim;
     bf16* x_out = p.xbuf + (size_t)((l + 1) & 1) * p.dim;
@@ -997,7 +1105,7 @@ __global__ void __launch_bounds__(MK_THREADS, 1) decode_megakernel(const MkParam
       const float* rope_row = p.rope + (int64_t)p.pos * (kHeadDim / 2) * 2;
       bf16* ck = L.cache_k + (int64_t)slot_row * kv_dim;
       bf16* cv = L.cache_v + (int64_t)slot_row * kv_dim;
-      consume_matrix(q_dim + 2 * kv_dim, p.dim, ring, full, empty, p.n_stages, rs, xs, tid,
+      consume_matrix<W8>(q_dim + 2 * kv_dim, p.dim, ring, full, empty, p.n_stages, rs, xs, tid,
                      [&](int n) { return *reinterpret_cast<const uint2*>(rope_row + ((n & (kHeadDim - 1)) >> 1) * 2); },
                      [&](int n, float a0, float a1, uint2 pf) {
         const float y0 = round_bf16(a0), y1 = round_bf16(a1);
@@ -1013,7 +1121,7 @@ __global__ void __launch_bounds__(MK_THREADS, 1) decode_megakernel(const MkParam
         } else {
           *reinterpret_cast<uint32_t*>(cv + (n - q_dim - kv_dim)) = pack_bf16x2(y0, y1);
         }
-      });
+      }, W8 ? L8->s_qkv : nullptr);
     }
     mk_stamp(p, tid, l, 2);
     grid_barrier(p, tid, epoch, l, 0);
@@ -1034,10 +1142,10 @@ __global__ void __launch_bounds__(MK_THREADS, 1) decode_megakernel(const MkParam
 
     // ---- phase 3: wo + residual ----
     stage_x(xs, p.abuf, nullptr, q_dim, 0.f, red, tid);
-    consume_matrix(p.dim, q_dim, ring, full, empty, p.n_stages, rs, xs, tid, [&](int n) { return make_uint2(ldcg_u32(x_in + n), 0u); }, [&](int n, float a0, float a1, uint2 pf) {
+    consume_matrix<W8>(p.dim, q_dim, ring, full, empty, p.n_stages, rs, xs, tid, [&](int n) { return make_uint2(ldcg_u32(x_in + n), 0u); }, [&](int n, float a0, float a1, uint2 pf) {
       const uint32_t r = pf.x;
       *reinterpret_cast<uint32_t*>(p.hbuf + n) = pack_bf16x2(round_bf16(a0) + bf16lo(r), round_bf16(a1) + bf16hi(r));
-    });
+    }, W8 ? L8->s_o : nullptr);
     mk_stamp(p, tid, l, 6);
     grid_barrier(p, tid, epoch, l, 3);
     mk_stamp(p, tid, l, 7);
@@ -1045,10 +1153,10 @@ __global__ void __launch_bounds__(MK_THREADS, 1) decode_megakernel(const MkParam
     if (p.n_experts == 0) {
     // ---- phase 4: RMSNorm + gate/up + SiLU*mul ----
       stage_x(xs, p.hbuf, L.ffn_norm, p.dim, p.eps, red, tid);
-      consume_matrix(2 * p.hidden, p.dim, ring, full, empty, p.n_stages, rs, xs, tid, [&](int) { return make_uint2(0u, 0u); }, [&](int n, float a0, float a1, uint2) {
+      consume_matrix<W8>(2 * p.hidden, p.dim, ring, full, empty, p.n_stages, rs, xs, tid, [&](int) { return make_uint2(0u, 0u); }, [&](int n, float a0, float a1, uint2) {
         const float s = round_bf16(ref_silu(round_bf16(a0)));
         p.gbuf[n >> 1] = __float2bfloat16_rn(s * round_bf16(a1));
-      });
+      }, W8 ? L8->s_13 : nullptr);
       mk_stamp(p, tid, l, 8);
       grid_barrier(p, tid, epoch, l, 4);
       mk_stamp(p, tid, l, 9);
@@ -1058,12 +1166,12 @@ __global__ void __launch_bounds__(MK_THREADS, 1) decode_megakernel(const MkParam
       //  complete, waiting on those words only.  Correct, but 4 polling rounds + 4 block syncs cost more than the ~5 us gate/up
       //  arrival skew they hide: 345 vs 351 tok/s.)
       stage_x(xs, p.gbuf, nullptr, p.hidden, 0.f, red, tid);
-      consume_matrix(p.dim, p.hidden, ring, full, empty, p.n_stages, rs, xs, tid, [&](int n) { return make_uint2(ldcg_u32(p.hbuf + n), 0u); },
+      consume_matrix<W8>(p.dim, p.hidden, ring, full, empty, p.n_stages, rs, xs, tid, [&](int n) { return make_uint2(ldcg_u32(p.hbuf + n), 0u); },
                      [&](int n, float a0, float a1, uint2 pf) {
                        const uint32_t r = pf.x;
                        *reinterpret_cast<uint32_t*>(x_out + n) = pack_bf16x2(round_bf16(a0) + bf16lo(r), round_bf16(a1) + bf16hi(r));
-                     });
-    } else {
+                     }, W8 ? L8->s_2 : nullptr);
+    } else if constexpr (!W8) {
       // ---- phase 4 (MoE): RMSNorm + router; gate/up + SiLU*mul of the selected experts (ascending expert index) ----
       stage_x(xs, p.hbuf, L.ffn_norm, p.dim, p.eps, red, tid);
       moe_route(p, l, xs, red, route, route_bar, tid);

@@ -23,6 +23,11 @@ enum EpiMode : int {
 //   y = bf16(y + bf16(L[t, n] * scaling))     L = the adapter's up-projection output, bf16 [T, ld_lora]
 // Instantiations without the flag compile to the same code as before.
 constexpr int EPI_LORA = 16;
+// Flag OR-ed into EPI_STORE / EPI_RESIDUAL / EPI_SWIGLU / EPI_QKV_ROPE: FP8 dense weights (include/mistral_b200.h).  The
+// accumulator is sum_k x[t, k] * float(q[n, k]); the row scale is applied once, as one fp32 product, before the Linear's rounding:
+//   y = bf16(fp32(w_scale[n] * acc))
+// Instantiations without the flag compile to the same code as before.
+constexpr int EPI_WSCALE = 32;
 
 constexpr int kMaxPeers = 8;
 
@@ -53,11 +58,19 @@ struct EpiParams {
   const void* lora_l = nullptr;  // bf16 [T, ld_lora], columns in the weight's row order
   int64_t ld_lora = 0;
   float lora_scaling = 0.f;
+  // EPI_WSCALE
+  const float* w_scale = nullptr;  // fp32 [N]
 };
 
 template <int FLAGS>
 __device__ __forceinline__ void epi_pair(const EpiParams& p, int t, int n, float acc0, float acc1) {
-  constexpr int MODE = FLAGS & ~EPI_LORA;
+  constexpr int MODE = FLAGS & ~(EPI_LORA | EPI_WSCALE);
+  if constexpr ((FLAGS & EPI_WSCALE) != 0) {
+    static_assert(MODE == EPI_STORE || MODE == EPI_RESIDUAL || MODE == EPI_SWIGLU || MODE == EPI_QKV_ROPE, "FP8 row scale: unsupported mode");
+    const float2 s = *reinterpret_cast<const float2*>(p.w_scale + n);
+    acc0 = __fmul_rn(s.x, acc0);
+    acc1 = __fmul_rn(s.y, acc1);
+  }
   // the Linear's own output rounding (bf16 result of nn.Linear)
   float y0 = round_bf16(acc0), y1 = round_bf16(acc1);
   if constexpr ((FLAGS & EPI_LORA) != 0) {

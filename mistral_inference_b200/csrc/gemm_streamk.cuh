@@ -55,12 +55,13 @@ struct SkParams {
   unsigned* flags;  // [gridDim], zero between launches
 };
 
-// W8 (grouped only): FP8 expert weights, converted per stage by warps 1-3 exactly as in tc_gemm_body (gemm_wgmma.cuh).  The
-// partition into (tile, k-block) units is the bf16 kernel's, so an FP8 call splits and sums every tile the same way.
+// W8: FP8 weights, converted per stage by warps 1-3 exactly as in tc_gemm_body (gemm_wgmma.cuh): the experts' W' tiles (grouped)
+// or the exact q tiles of a dense Linear, whose row scales the epilogue applies (MODE carries EPI_WSCALE).  The partition into
+// (tile, k-block) units is the bf16 kernel's, so an FP8 call splits and sums every tile the same way.
 template <int MODE, int TA, bool GROUPED, bool W8 = false>
 __device__ __forceinline__ void sk_gemm_body(const CUtensorMap& map_a, const CUtensorMap* map_w_base, const SkParams& p, const int32_t* plan,
                                              const MoeWeightScales* scales = nullptr) {
-  static_assert(!W8 || GROUPED, "FP8 weights: grouped variant only");
+  static_assert(!W8 || GROUPED || (MODE & EPI_WSCALE) != 0, "FP8 dense weights: the epilogue applies the row scales");
   using Cfg = TgCfg<SK_BN, TA, W8>;
   constexpr int STAGES = Cfg::kStages, STAGE_BYTES = Cfg::kStageBytes, A_BYTES = Cfg::kABytes, NCONS = 128 * Cfg::kWG;
   extern __shared__ uint8_t smem_raw[];
@@ -127,7 +128,7 @@ __device__ __forceinline__ void sk_gemm_body(const CUtensorMap& map_a, const CUt
       };
       const uint32_t head = GROUPED ? 0u : (n_it < (uint32_t)STAGES ? n_it : (uint32_t)STAGES);  // (grouped: the tile list itself is the previous kernel's output)
       for (uint32_t it = 0; it < head; ++it) {
-        mbar_arrive_expect_tx(&full[it % STAGES], STAGE_BYTES);  // first lap: every slot is free
+        mbar_arrive_expect_tx(&full[it % STAGES], W8 ? A_BYTES : STAGE_BYTES);  // first lap: every slot is free
         issue(it, false, true);
       }
       pdl_wait();
@@ -150,7 +151,10 @@ __device__ __forceinline__ void sk_gemm_body(const CUtensorMap& map_a, const CUt
       const uint32_t s = it % STAGES, par = (it / STAGES) & 1;
       mbar_wait_quiet(&raw[s], par);
       uint8_t* sa = smem + s * STAGE_BYTES;
-      convert_w8_tile<SK_BN>(sa + A_BYTES + Cfg::kBBytes, sa + A_BYTES, scales->s[tile_expert[tile % num_m]] + (tile / num_m) * SK_BN, ct);
+      if constexpr (GROUPED)
+        convert_w8_tile<SK_BN>(sa + A_BYTES + Cfg::kBBytes, sa + A_BYTES, scales->s[tile_expert[tile % num_m]] + (tile / num_m) * SK_BN, ct);
+      else
+        convert_w8_tile<SK_BN, true>(sa + A_BYTES + Cfg::kBBytes, sa + A_BYTES, nullptr, ct);
       mbar_arrive(&full[s]);
     }
   } else if (warp >= 4) {
@@ -262,6 +266,12 @@ __global__ void __launch_bounds__(TgCfg<SK_BN, TA>::kThreads, 1)
 
 template <int MODE, int TA>
 __global__ void __launch_bounds__(TgCfg<SK_BN, TA, true>::kThreads, 1)
+    gemm_streamk_fp8_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_w, const SkParams p) {
+  sk_gemm_body<MODE, TA, false, true>(map_a, &map_w, p, nullptr);
+}
+
+template <int MODE, int TA>
+__global__ void __launch_bounds__(TgCfg<SK_BN, TA, true>::kThreads, 1)
     gemm_streamk_grouped_fp8_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ MoeWeightMaps maps_w,
                                     const __grid_constant__ MoeWeightScales scales, const SkParams p, const int32_t* __restrict__ plan) {
   sk_gemm_body<MODE, TA, true, true>(map_a, maps_w.m, p, plan, &scales);
@@ -307,6 +317,42 @@ int launch_streamk(const GemmParams& g, void* workspace, size_t workspace_bytes,
   if (g.T <= 32) return launch_streamk_ta<MODE, 32>(g, workspace, workspace_bytes, stream);
   if (g.T <= 64) return launch_streamk_ta<MODE, 64>(g, workspace, workspace_bytes, stream);
   return launch_streamk_ta<MODE, 128>(g, workspace, workspace_bytes, stream);
+}
+
+// FP8 dense weights (MODE carries EPI_WSCALE): the bf16 launcher's partition and workspace, an e4m3 weight map
+template <int MODE, int TA>
+int launch_streamk_fp8_ta(const GemmParams& g, void* workspace, size_t workspace_bytes, cudaStream_t stream) {
+  using Cfg = TgCfg<SK_BN, TA, true>;
+  int dev = 0, sms = 0;
+  MB_CHECK_CUDA(cudaGetDevice(&dev));
+  MB_CHECK_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  if (sms > SK_MAX_CTAS) sms = SK_MAX_CTAS;
+  if (workspace == nullptr || workspace_bytes < kWsSkPartials.end()) return fail(MB200_E_WORKSPACE, "stream-K gemm (fp8): workspace %zu < %zu", workspace_bytes, kWsSkPartials.end());
+  CUtensorMap map_a, map_w;
+  int rc = make_tensor_map_2d(&map_a, g.a, g.T, g.K, TA);
+  if (rc) return rc;
+  rc = make_tensor_map_e4m3(&map_w, g.w, g.N, g.K, SK_BN);
+  if (rc) return rc;
+  SkParams p;
+  p.T = g.T;
+  p.N = g.N;
+  p.K = g.K;
+  p.epi = g.epi;
+  p.partials = reinterpret_cast<float*>((uint8_t*)workspace + kWsSkPartials.offset);
+  p.flags = reinterpret_cast<unsigned*>((uint8_t*)workspace + kWsSkFlags.offset);
+  const long long units = (long long)(g.N / SK_BN) * (g.K / TG_BK);
+  const int grid = (int)(units < sms ? units : sms);
+  MB_CHECK_CUDA(cudaFuncSetAttribute(gemm_streamk_fp8_kernel<MODE, TA>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmem));
+  MB_CHECK_CUDA(launch_pdl(gemm_streamk_fp8_kernel<MODE, TA>, dim3((unsigned)grid), dim3(Cfg::kThreads), (size_t)Cfg::kSmem, stream, map_a, map_w, p));
+  note_launch("gemm_streamk_fp8_kernel<%d, %d>", MODE, TA);
+  return MB200_OK;
+}
+
+template <int MODE>
+int launch_streamk_fp8(const GemmParams& g, void* workspace, size_t workspace_bytes, cudaStream_t stream) {
+  if (g.T <= 32) return launch_streamk_fp8_ta<MODE, 32>(g, workspace, workspace_bytes, stream);
+  if (g.T <= 64) return launch_streamk_fp8_ta<MODE, 64>(g, workspace, workspace_bytes, stream);
+  return launch_streamk_fp8_ta<MODE, 128>(g, workspace, workspace_bytes, stream);
 }
 
 }  // namespace mb200

@@ -99,22 +99,32 @@ __device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta)
 // layout TMA gives the bf16 kernels (16-byte chunk c of row r at chunk c ^ (r & 7)), so the wgmma descriptors are unchanged.
 // Thread ct of W8_CONVERTERS takes 16-byte e4m3 chunks ct, ct + W8_CONVERTERS, ...: consecutive threads read consecutive 16 bytes,
 // and each quarter warp's 16-byte stores hit 8 distinct chunk columns of two rows (no bank conflicts).
+// DENSE (FP8 dense weights, include/mistral_b200.h): the tile is q itself, converted exactly (e4m3x2_to_float2, then a bf16 pack
+// that cannot round: no multiply); the row scale is applied to the accumulator in the epilogue (EPI_WSCALE) and scale_rows is unused.
 constexpr int W8_CONVERTERS = 96;  // warps 1-3 of the producer warpgroup
-template <int BN>
+template <int BN, bool DENSE = false>
 __device__ __forceinline__ void convert_w8_tile(const uint8_t* raw, uint8_t* wtile, const float* __restrict__ scale_rows, int ct) {
 #pragma unroll 2
   for (int q = ct; q < BN * (TG_BK / 16); q += W8_CONVERTERS) {
     const int row = q >> 2, c = q & 3;
     const uint4 v = *reinterpret_cast<const uint4*>(raw + row * TG_BK + c * 16);
-    const float s = __ldg(scale_rows + row);
     const uint32_t in[4] = {v.x, v.y, v.z, v.w};
     uint32_t o[8];
+    if constexpr (DENSE) {
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const float2 f = e4m3x2_to_float2(in[j >> 1] >> (16 * (j & 1)));
+        o[j] = pack2_rn(f.x, f.y);
+      }
+    } else {
+    const float s = __ldg(scale_rows + row);
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
       const __half2_raw hr = __nv_cvt_fp8x2_to_halfraw2((__nv_fp8x2_storage_t)(in[j >> 1] >> (16 * (j & 1))), __NV_E4M3);
       const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&hr));
       const __nv_bfloat162 b = __floats2bfloat162_rn(__fmul_rn(f.x, s), __fmul_rn(f.y, s));
       o[j] = *reinterpret_cast<const uint32_t*>(&b);
+    }
     }
     uint8_t* dst = wtile + row * (TG_BK * 2);
     *reinterpret_cast<uint4*>(dst + (((2 * c) ^ (row & 7)) << 4)) = make_uint4(o[0], o[1], o[2], o[3]);
@@ -165,13 +175,15 @@ struct MoeWeightScales {  // W8: per-row fp32 scales of each expert's matrix (nu
   const float* s[MOE_MAX_EXPERTS];
 };
 
-// W8 (grouped, single CTA only): the producer thread loads the e4m3 W tile into the stage's raw area on raw[s]; warps 1-3 wait on
-// raw[s], write the bf16 tile and arrive on full[s] (W8_CONVERTERS arrivals next to the producer's expect_tx for the A tile).
+// W8 (single CTA only): the producer thread loads the e4m3 W tile into the stage's raw area on raw[s]; warps 1-3 wait on raw[s],
+// write the bf16 tile and arrive on full[s] (W8_CONVERTERS arrivals next to the producer's expect_tx for the A tile).  Grouped:
+// the experts' W' tiles (§3.9); dense: the exact q tiles, the row scales applied by the epilogue (MODE carries EPI_WSCALE).
 template <int MODE, int CL, int BN, int TA, bool GROUPED, bool W8 = false>
 __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& map_a, const CUtensorMap* map_w_base, const TcGemmParams& p, const int32_t* plan,
                                              const MoeWeightScales* scales = nullptr) {
   static_assert(TA == 128 || CL == 1, "small-batch variant is single-CTA");
-  static_assert(!W8 || (GROUPED && CL == 1), "FP8 weights: grouped single-CTA variant only");
+  static_assert(!W8 || CL == 1, "FP8 weights: single-CTA variant only");
+  static_assert(!W8 || GROUPED || (MODE & EPI_WSCALE) != 0, "FP8 dense weights: the epilogue applies the row scales");
   using Cfg = TgCfg<BN, TA, W8>;
   constexpr int STAGES = Cfg::kStages, B_BYTES = Cfg::kBBytes, STAGE_BYTES = Cfg::kStageBytes, A_BYTES = Cfg::kABytes;
   extern __shared__ uint8_t smem_raw[];
@@ -292,12 +304,12 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& map_a, const CUt
     for (int tile = cta; tile < num_tiles; tile += n_cta) {
       int mu, nt;
       tile_mn(tile, mu, nt);
-      const float* srows = scales->s[tile_expert[mu]] + nt * BN;
+      const float* srows = GROUPED ? scales->s[tile_expert[mu]] + nt * BN : nullptr;
       for (int kb = 0; kb < num_k; ++kb, ++it) {
         const uint32_t s = it % STAGES, par = (it / STAGES) & 1;
         mbar_wait_quiet(&raw[s], par);
         uint8_t* sa = smem + s * STAGE_BYTES;
-        convert_w8_tile<BN>(sa + A_BYTES + B_BYTES, sa + A_BYTES, srows, ct);
+        convert_w8_tile<BN, !GROUPED>(sa + A_BYTES + B_BYTES, sa + A_BYTES, srows, ct);
         mbar_arrive(&full[s]);
       }
     }
@@ -353,6 +365,13 @@ __global__ void __launch_bounds__(TgCfg<BN, TA>::kThreads, 1)
     gemm_wgmma_grouped_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ MoeWeightMaps maps_w, const TcGemmParams p,
                               const int32_t* __restrict__ plan) {
   tc_gemm_body<MODE, CL, BN, TA, true>(map_a, maps_w.m, p, plan);
+}
+
+// FP8 dense weights: map_w is an e4m3 [N, K] map (box [BN x 64] bytes, no swizzle); MODE carries EPI_WSCALE.
+template <int MODE, int BN, int TA>
+__global__ void __launch_bounds__(TgCfg<BN, TA, true>::kThreads, 1)
+    gemm_wgmma_fp8_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_w, const TcGemmParams p) {
+  tc_gemm_body<MODE, 1, BN, TA, false, true>(map_a, &map_w, p, nullptr);
 }
 
 // FP8 expert weights: maps_w are e4m3 [N, K] maps (box [BN x 64] bytes, no swizzle), scales the per-row fp32 scales.
@@ -540,6 +559,62 @@ int launch_gemm_wgmma(const GemmParams& g, cudaStream_t stream) {
   if (bn == 192) return launch_gemm_wgmma_bn<MODE, 192>(g, pair, sms, stream);
   const bool narrow = bn == 128;
   return narrow ? launch_gemm_wgmma_bn<MODE, 128>(g, pair, sms, stream) : launch_gemm_wgmma_bn<MODE, 256>(g, pair, sms, stream);
+}
+
+// ---- FP8 dense weights: the same tile choices as launch_gemm_wgmma, single CTA only ------------------------------------------
+// A shape that the bf16 launcher runs as 2-CTA clusters (T >= 512) runs as single CTAs at the same BN: the W8 stage holds the
+// e4m3 tile next to the bf16 tile its converter warps write, and the multicast halves of the cluster variant have no such pair.
+template <int MODE, int BN, int TA>
+int launch_gemm_wgmma_fp8_bn(const GemmParams& g, int sms, cudaStream_t stream) {
+  using Cfg = TgCfg<BN, TA, true>;
+  CUtensorMap map_a, map_w;
+  int rc = make_tensor_map_2d(&map_a, g.a, g.T, g.K, TA);
+  if (rc) return rc;
+  rc = make_tensor_map_e4m3(&map_w, g.w, g.N, g.K, BN);
+  if (rc) return rc;
+  TcGemmParams p;
+  p.T = g.T;
+  p.N = g.N;
+  p.K = g.K;
+  p.epi = g.epi;
+  const int tiles = ceil_div(g.T, TG_BM) * (g.N / BN);
+  MB_CHECK_CUDA(cudaFuncSetAttribute(gemm_wgmma_fp8_kernel<MODE, BN, TA>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmem));
+  gemm_wgmma_fp8_kernel<MODE, BN, TA><<<tiles < sms ? tiles : sms, Cfg::kThreads, Cfg::kSmem, stream>>>(map_a, map_w, p);
+  note_launch("gemm_wgmma_fp8_kernel<%d, %d, %d>", MODE, BN, TA);
+  MB_CHECK_LAUNCH("gemm_wgmma_fp8_kernel");
+  return MB200_OK;
+}
+
+template <int MODE, int TA>
+int launch_gemm_wgmma_fp8_small_ta(const GemmParams& g, int sms, cudaStream_t stream) {
+  switch (wgmma_small_bn(g.N, sms)) {
+    case 256: return launch_gemm_wgmma_fp8_bn<MODE, 256, TA>(g, sms, stream);
+    case 128: return launch_gemm_wgmma_fp8_bn<MODE, 128, TA>(g, sms, stream);
+    case 64: return launch_gemm_wgmma_fp8_bn<MODE, 64, TA>(g, sms, stream);
+    case 32: return launch_gemm_wgmma_fp8_bn<MODE, 32, TA>(g, sms, stream);
+    default: return fail(MB200_E_INVALID, "small-batch GEMM (fp8): N=%d is not a multiple of 32", g.N);
+  }
+}
+
+template <int MODE>
+int launch_gemm_wgmma_fp8(const GemmParams& g, cudaStream_t stream) {
+  int dev = 0, sms = 0;
+  MB_CHECK_CUDA(cudaGetDevice(&dev));
+  MB_CHECK_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  if (g.T <= 32) return launch_gemm_wgmma_fp8_small_ta<MODE, 32>(g, sms, stream);
+  if (g.T <= 64) return launch_gemm_wgmma_fp8_small_ta<MODE, 64>(g, sms, stream);
+  if (g.T < TG_BM) return launch_gemm_wgmma_fp8_small_ta<MODE, 128>(g, sms, stream);
+  // the bf16 launcher's BN rule, with the m units it would have used (clusters of two for T >= 512 unless switched off)
+  const bool pair = wgmma_cluster_enabled() && g.T >= 4 * TG_BM;
+  const int units = pair ? sms / 2 : sms, m_units = pair ? ceil_div(ceil_div(g.T, TG_BM), 2) : ceil_div(g.T, TG_BM);
+  int bn = 256;
+  if (g.N % 256 != 0 || (int64_t)m_units * (g.N / 256) < units) {
+    bn = g.N % 128 == 0 ? 128 : 192;
+  }
+  const int forced = wgmma_forced_bn();
+  if ((forced == 128 || forced == 192 || forced == 256) && g.N % forced == 0) bn = forced;
+  if (bn == 192) return launch_gemm_wgmma_fp8_bn<MODE, 192, TG_BM>(g, sms, stream);
+  return bn == 128 ? launch_gemm_wgmma_fp8_bn<MODE, 128, TG_BM>(g, sms, stream) : launch_gemm_wgmma_fp8_bn<MODE, 256, TG_BM>(g, sms, stream);
 }
 
 }  // namespace mb200

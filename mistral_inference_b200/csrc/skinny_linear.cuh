@@ -23,7 +23,10 @@ struct SkinnyParams {
   EpiParams epi;
 };
 
-template <int T, int MODE, bool NORM>
+// W8 (FP8 dense weights, launch_skinny_fp8): p.w is e4m3 [N, K] (K % 16 == 0) and MODE carries EPI_WSCALE (the row
+// scales in p.epi.w_scale).  Same CTA, x staging and row pairs; a 16-byte load is 16 weights (half the bytes of a bf16 load, still
+// 4 in flight per row per lane), each pair converted exactly (e4m3x2_to_float2) and fed to the same fp32 FMAs.
+template <int T, int MODE, bool NORM, bool W8 = false>
 __global__ void __launch_bounds__(kSkinnyThreads) skinny_linear_kernel(const SkinnyParams p) {
   extern __shared__ __align__(16) uint8_t smem_raw[];
   uint4* xs = reinterpret_cast<uint4*>(smem_raw);  // [T][K/8] 16-byte chunks
@@ -84,6 +87,63 @@ __global__ void __launch_bounds__(kSkinnyThreads) skinny_linear_kernel(const Ski
   // ---- stream the two rows of this warp ----
   const int n0 = (blockIdx.x * kSkinnyWarps + warp) * kSkinnyRowsPerWarp;
   if (n0 >= p.N) return;
+  if constexpr (W8) {
+    const int kq = p.K >> 4;  // e4m3 chunks of a weight row
+    const uint4* w0 = reinterpret_cast<const uint4*>(reinterpret_cast<const uint8_t*>(p.w) + (int64_t)n0 * p.K);
+    const uint4* w1 = w0 + kq;
+    float acc[2][T];
+#pragma unroll
+    for (int t = 0; t < T; ++t) acc[0][t] = acc[1][t] = 0.f;
+
+    // 16 weights of each row against x chunks 2c, 2c + 1
+    auto fma16 = [&](const uint4& a, const uint4& b, int c) {
+      const uint32_t aq[4] = {a.x, a.y, a.z, a.w}, bq[4] = {b.x, b.y, b.z, b.w};
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {  // weights 8h .. 8h + 7 against x chunk 2c + h
+        float2 af[4], bf[4];
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          af[j] = e4m3x2_to_float2(aq[2 * h + (j >> 1)] >> (16 * (j & 1)));
+          bf[j] = e4m3x2_to_float2(bq[2 * h + (j >> 1)] >> (16 * (j & 1)));
+        }
+#pragma unroll
+        for (int t = 0; t < T; ++t) {
+          const uint4 xv = xs[t * kc + 2 * c + h];
+          const uint32_t xw[4] = {xv.x, xv.y, xv.z, xv.w};
+#pragma unroll
+          for (int j = 0; j < 4; ++j) {
+            const float xl = bf16lo(xw[j]), xh = bf16hi(xw[j]);
+            acc[0][t] = fmaf(af[j].x, xl, acc[0][t]);
+            acc[0][t] = fmaf(af[j].y, xh, acc[0][t]);
+            acc[1][t] = fmaf(bf[j].x, xl, acc[1][t]);
+            acc[1][t] = fmaf(bf[j].y, xh, acc[1][t]);
+          }
+        }
+      }
+    };
+    constexpr int U = T == 4 ? 3 : 4;  // 16-byte loads in flight per row per lane (3 at T = 4: 4 would spill)
+    int c = lane;
+    for (; c + (U - 1) * 32 < kq; c += U * 32) {
+      uint4 a[U], b[U];
+#pragma unroll
+      for (int u = 0; u < U; ++u) {
+        a[u] = ldg_stream16(w0 + c + u * 32);
+        b[u] = ldg_stream16(w1 + c + u * 32);
+      }
+#pragma unroll
+      for (int u = 0; u < U; ++u) fma16(a[u], b[u], c + u * 32);
+    }
+    for (; c < kq; c += 32) fma16(ldg_stream16(w0 + c), ldg_stream16(w1 + c), c);  // tail (K/16 not a multiple of 128)
+#pragma unroll
+    for (int t = 0; t < T; ++t) {
+      acc[0][t] = warp_sum(acc[0][t]);
+      acc[1][t] = warp_sum(acc[1][t]);
+    }
+#pragma unroll
+    for (int t = 0; t < T; ++t)
+      if (lane == t) epi_pair<MODE>(p.epi, t, n0, acc[0][t], acc[1][t]);
+    return;
+  }
   const uint4* w0 = reinterpret_cast<const uint4*>(p.w) + (int64_t)n0 * kc;
   const uint4* w1 = w0 + kc;
 
@@ -145,6 +205,28 @@ __global__ void __launch_bounds__(kSkinnyThreads) skinny_linear_kernel(const Ski
 #pragma unroll
   for (int t = 0; t < T; ++t)
     if (lane == t) epi_pair<MODE>(p.epi, t, n0, acc[0][t], acc[1][t]);
+}
+
+template <int MODE, bool NORM>
+int launch_skinny_fp8(const SkinnyParams& p, int T, cudaStream_t stream) {
+  MB_CHECK_ARG(T >= 1 && T <= MB200_SKINNY_MAX_T, "skinny linear (fp8): T=%d out of range", T);
+  MB_CHECK_ARG(p.K % 16 == 0 && p.N % kSkinnyRowsPerWarp == 0, "skinny linear (fp8): K=%d must be a multiple of 16, N=%d even", p.K, p.N);
+  const size_t smem = (size_t)T * p.K * 2;
+  MB_CHECK_ARG(smem <= 200 * 1024, "skinny linear (fp8): T*K too large for shared memory (%zu B)", smem);
+  const dim3 grid(ceil_div(p.N, kSkinnyRowsPerCta));
+  auto go = [&](auto kernel) -> int {
+    if (smem > 48 * 1024) MB_CHECK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    kernel<<<grid, kSkinnyThreads, smem, stream>>>(p);
+    note_launch("skinny_linear_kernel<%d, %d, %s, true>", T, MODE, NORM ? "true" : "false");
+    MB_CHECK_LAUNCH("skinny_linear_kernel<fp8>");
+    return MB200_OK;
+  };
+  switch (T) {
+    case 1: return go(skinny_linear_kernel<1, MODE, NORM, true>);
+    case 2: return go(skinny_linear_kernel<2, MODE, NORM, true>);
+    case 3: return go(skinny_linear_kernel<3, MODE, NORM, true>);
+    default: return go(skinny_linear_kernel<4, MODE, NORM, true>);
+  }
 }
 
 template <int MODE, bool NORM>

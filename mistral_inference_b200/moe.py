@@ -81,9 +81,13 @@ class Fp8Expert(nn.Module):
 
     def quantize_(self, name: str, w: torch.Tensor) -> None:
         """Quantises the bf16 weight `w` of Linear `name` into place (one bf16 copy of `w` on the device while it runs)."""
-        q, s = self._slots(name)
-        assert tuple(w.shape) == tuple(q.shape), f"{name}: shape {tuple(w.shape)} != expected {tuple(q.shape)}"
-        _abi.quantize_e4m3_rows(w.to(device=q.device, dtype=torch.bfloat16).contiguous(), q, s)
+        quantize_rows_(name, w, *self._slots(name))
+
+
+def quantize_rows_(name: str, w: torch.Tensor, q: torch.Tensor, s: torch.Tensor) -> None:
+    """q, s (e4m3 rows as uint8 and fp32 row scales, both possibly strided views) of the bf16 weight `w` of Linear `name`."""
+    assert tuple(w.shape) == tuple(q.shape), f"{name}: shape {tuple(w.shape)} != expected {tuple(q.shape)}"
+    _abi.quantize_e4m3_rows(w.to(device=q.device, dtype=torch.bfloat16).contiguous(), q, s)
 
 
 class MoeBuffers:

@@ -57,18 +57,46 @@ class _OutputView:
         return self._m.output_weight
 
 
+DENSE_WEIGHTS = ("bf16", "fp8")
+
+
+def _check_dense_weights(args: TransformerArgs, dense_weights: str) -> None:
+    """The refusals of dense_weights="fp8", before anything is allocated."""
+    if dense_weights not in DENSE_WEIGHTS:
+        raise ValueError(f"dense_weights={dense_weights!r}: expected one of {DENSE_WEIGHTS}")
+    if dense_weights != "fp8":
+        return
+    if args.moe is not None:
+        raise ValueError("dense_weights='fp8' needs a dense model: FP8 attention Linears on mixture-of-experts models are not built "
+                         "(expert_weights='fp8' quantises the experts)")
+    if args.lora is not None:
+        raise NotImplementedError("un-merged LoRA on FP8 dense weights is not built (merge the adapter into a bf16 model instead)")
+    # every Linear must stay off the mma.sync GEMM at every token count: it has no e4m3 variant (include/mistral_b200.h)
+    q_dim, kv_dim = args.n_heads * args.head_dim, args.n_kv_heads * args.head_dim
+    for name, N, K in (("wqkv", q_dim + 2 * kv_dim, args.dim), ("wo", args.dim, q_dim), ("w13", 2 * args.hidden_dim, args.dim),
+                       ("w2", args.dim, args.hidden_dim)):
+        if K % 64 != 0 or (N % 128 != 0 and N % 192 != 0):
+            raise ValueError(f"dense_weights='fp8': {name} [{N}, {K}] would need the mma.sync GEMM, which has no FP8 variant "
+                             "(K must be a multiple of 64 and N of 128 or 192)")
+
+
 class Transformer(nn.Module):
     def __init__(self, args: TransformerArgs, pipeline_rank: int = 0, num_pipeline_ranks: int = 1, softmax_fp32: bool = True,
                  expert_parallel: Optional[Tuple[int, int]] = None, expert_group: Any = None, expert_weights: str = "bf16", *,
-                 kv_cache: str = "bf16"):
+                 kv_cache: str = "bf16", dense_weights: str = "bf16"):
         """Same signature as the reference (transformer.py:34-40) plus `expert_parallel = (rank, world)`: MoE experts sharded
         `e % world == rank` over the ranks of `expert_group` (default process group), everything else replicated, one
         all-reduce of [T, dim] per MoE layer (SURVEY.md 8e); and `expert_weights`: "bf16", or "fp8" to store every MoE expert
         matrix as e4m3 with one fp32 scale per row (moe.Fp8Expert; the model then computes exactly what the bf16 model computes
         with the dequantised weights W', see include/mistral_b200.h); and `kv_cache`: "bf16", or "fp8" to keep the KV cache as e4m3
         with one power-of-two exponent per (slot, kv head) row (cache.BufferCache; the model is then the bf16 model with k, v
-        replaced by their dequantised k', v' right after RoPE in every forward that has a cache, see include/mistral_b200.h)."""
+        replaced by their dequantised k', v' right after RoPE in every forward that has a cache, see include/mistral_b200.h); and
+        `dense_weights`: "bf16", or "fp8" to store wq, wk, wv, wo, w1, w2 and w3 of every text layer of a dense model as e4m3 with
+        one fp32 scale per row, applied after the dot product: y = bf16(s * sum_k x * q) (include/mistral_b200.h; the embedding,
+        the lm head, the norms and the vision tower stay bf16).  That model is not bit-identical to any bf16 model."""
         super().__init__()
+        _check_dense_weights(args, dense_weights)
+        self.dense_weights = dense_weights
         if kv_cache not in KV_CACHE_FORMATS:
             raise ValueError(f"kv_cache={kv_cache!r}: expected one of {KV_CACHE_FORMATS}")
         if kv_cache == "fp8" and args.head_dim != 128:
@@ -125,7 +153,8 @@ class Transformer(nn.Module):
         self.layers = nn.ModuleDict({
             str(i): TransformerBlock(dim=args.dim, hidden_dim=args.hidden_dim, n_heads=args.n_heads, n_kv_heads=args.n_kv_heads,
                                      head_dim=args.head_dim, norm_eps=args.norm_eps, lora=args.lora, moe=args.moe,
-                                     expert_shard=self.expert_parallel, expert_group=expert_group, expert_weights=expert_weights)
+                                     expert_shard=self.expert_parallel, expert_group=expert_group, expert_weights=expert_weights,
+                                     dense_weights=dense_weights)
             for i in range(offset, end)
         })
         self.n_local_layers = len(self.layers)
@@ -140,7 +169,7 @@ class Transformer(nn.Module):
     # ------------------------------------------------------------------ properties
     @property
     def dtype(self) -> torch.dtype:
-        return next(self.parameters()).dtype
+        return next(p.dtype for p in self.parameters() if p.is_floating_point())  # FP8 weights are stored as integers
 
     @property
     def device(self) -> torch.device:
@@ -328,7 +357,7 @@ class Transformer(nn.Module):
 
     def _megakernel_ok(self, B: int) -> bool:
         # the megakernel has no LoRA stage and reads bf16 experts and a bf16 KV cache only: with un-merged adapters, FP8 experts or
-        # an FP8 cache batch 1 takes the per-layer graph path
+        # an FP8 cache batch 1 takes the per-layer graph path (FP8 dense weights have a megakernel of their own: decode_step_fp8)
         # the shape limits (head ratio, K chunking, KV <= 8, MoE sizes, a shared-memory ring of >= 9 stages next to the
         # activations) are the library's, asked once per model: a model it refuses takes the per-layer path
         if not (B == 1 and self.num_pipeline_ranks == 1 and self.expert_parallel[1] == 1 and self.args.lora is None
@@ -336,9 +365,13 @@ class Transformer(nn.Module):
             return False
         if self._megakernel_refused is None:
             a, moe = self.args, self.args.moe
-            self._megakernel_refused = _abi.decode_step_unsupported(
-                a.dim, a.hidden_dim, a.n_heads, a.n_kv_heads, a.head_dim, self.vocab_size,
-                moe.num_experts if moe is not None else 0, moe.num_experts_per_tok if moe is not None else 0) or ""
+            if self.dense_weights == "fp8":
+                self._megakernel_refused = _abi.decode_step_fp8_unsupported(a.dim, a.hidden_dim, a.n_heads, a.n_kv_heads, a.head_dim,
+                                                                            self.vocab_size) or ""
+            else:
+                self._megakernel_refused = _abi.decode_step_unsupported(
+                    a.dim, a.hidden_dim, a.n_heads, a.n_kv_heads, a.head_dim, self.vocab_size,
+                    moe.num_experts if moe is not None else 0, moe.num_experts_per_tok if moe is not None else 0) or ""
         return self._megakernel_refused == ""
 
     def _decode_state(self, cache: BufferCache, key: Any) -> Dict[str, Any]:
@@ -361,9 +394,10 @@ class Transformer(nn.Module):
         a = self.args
         ws = self.workspace(1)
         st = self._decode_state(cache, "mk")
+        fp8 = self.dense_weights == "fp8"
         if "layers" not in st:
             blocks = list(self.layers.values())
-            desc = np.zeros((len(blocks), 8), dtype=np.uint64)
+            desc = np.zeros((len(blocks), 12 if fp8 else 8), dtype=np.uint64)  # mb200_layer_desc(_fp8)
             moe = self.args.moe
             E = moe.num_experts if moe is not None else 0
             gate_tab, w13_tab, w2_tab = [], [], []
@@ -376,9 +410,12 @@ class Transformer(nn.Module):
                     gate_tab.append(ff.gate_weight.data_ptr())
                     w13_tab += [ff.experts[str(e)].w13.data_ptr() for e in range(E)]
                     w2_tab += [ff.experts[str(e)].w2_weight.data_ptr() for e in range(E)]
-                desc[i] = [blk.attention.wqkv.data_ptr(), blk.attention.wo_weight.data_ptr(), w13p, w2p,
-                           blk.attention_norm.weight.data_ptr(), blk.ffn_norm.weight.data_ptr(), cache.cache_k[i].data_ptr(),
-                           cache.cache_v[i].data_ptr()]
+                desc[i, :8] = [blk.attention.wqkv.data_ptr(), blk.attention.wo_weight.data_ptr(), w13p, w2p,
+                               blk.attention_norm.weight.data_ptr(), blk.ffn_norm.weight.data_ptr(), cache.cache_k[i].data_ptr(),
+                               cache.cache_v[i].data_ptr()]
+                if fp8:
+                    desc[i, 8:] = [blk.attention.wqkv_scale.data_ptr(), blk.attention.wo_scale.data_ptr(), ff.w13_scale.data_ptr(),
+                                   ff.w2_scale.data_ptr()]
             tab = lambda v: torch.tensor(v, dtype=torch.int64, device=self.device) if v else None  # noqa: E731
             st.update({"E": E, "k": moe.num_experts_per_tok if moe is not None else 0,
                        "moe_gate": tab(gate_tab), "moe_w13": tab(w13_tab), "moe_w2": tab(w2_tab),
@@ -400,9 +437,15 @@ class Transformer(nn.Module):
             tok = st["token"]
         self.last_argmax = st["next"]
         with _nvtx("mb200.decode_megakernel"):
-            _abi.decode_step(st["layers"], st["windows"], self.n_local_layers, self.tok_embeddings.weight, self.norm.weight, self.output_weight,
-                             self.rope_table, tok, pos, 0, st["logits"], st["next"], a.dim, a.hidden_dim, a.n_heads, a.n_kv_heads, a.head_dim,
-                             self.vocab_size, a.norm_eps, ws, st["E"], st["k"], st["moe_gate"], st["moe_w13"], st["moe_w2"])
+            if fp8:
+                _abi.decode_step_fp8(st["layers"], st["windows"], self.n_local_layers, self.tok_embeddings.weight, self.norm.weight,
+                                     self.output_weight, self.rope_table, tok, pos, 0, st["logits"], st["next"], a.dim, a.hidden_dim,
+                                     a.n_heads, a.n_kv_heads, a.head_dim, self.vocab_size, a.norm_eps, ws)
+            else:
+                _abi.decode_step(st["layers"], st["windows"], self.n_local_layers, self.tok_embeddings.weight, self.norm.weight,
+                                 self.output_weight, self.rope_table, tok, pos, 0, st["logits"], st["next"], a.dim, a.hidden_dim, a.n_heads,
+                                 a.n_kv_heads, a.head_dim, self.vocab_size, a.norm_eps, ws, st["E"], st["k"], st["moe_gate"], st["moe_w13"],
+                                 st["moe_w2"])
         cache.update_seqlens([1])
         self._last_static_logits = st["logits"].data_ptr()
         return st["logits"]
@@ -569,6 +612,15 @@ class Transformer(nn.Module):
                 if part == "":  # a full checkpoint's plain weight: zero adapter (lora.py:76-89)
                     adapter.zero(seg)
                 rest = name + ".weight"
+        ff = blk.feed_forward
+        if getattr(att, "fp8", False):  # FP8 dense weights: the reference's bf16 weight, quantised into place
+            for mod, names in ((att, ("wq", "wk", "wv", "wo")), (ff, ("w1", "w2", "w3"))):
+                for name in names:
+                    if rest.startswith(f"{'attention' if mod is att else 'feed_forward'}.{name}."):
+                        if rest.rsplit(".", 1)[1] != "weight":
+                            raise ValueError(f"Unexpected key {k}")
+                        put(mod.weight_e4m3(name), lambda _seg, w, mod=mod, name=name: mod.quantize_(name, w))
+                        return True
         if rest == "attention.wq.weight":
             put(att.wqkv[: att.q_dim])
         elif rest == "attention.wk.weight":
@@ -711,11 +763,19 @@ class Transformer(nn.Module):
     @staticmethod
     def _block_state(out: Dict[str, torch.Tensor], p: str, blk: TransformerBlock) -> None:
         att = blk.attention
-        for n in ("wq", "wk", "wv", "wo"):
-            Transformer._linear_state(out, p, blk, "attention." + n, getattr(att, n).weight)
+        fp8 = getattr(att, "fp8", False)
+        if not fp8:
+            for n in ("wq", "wk", "wv", "wo"):
+                Transformer._linear_state(out, p, blk, "attention." + n, getattr(att, n).weight)
         out[p + "attention_norm.weight"] = blk.attention_norm.weight
         out[p + "ffn_norm.weight"] = blk.ffn_norm.weight
         ff = blk.feed_forward
+        if fp8:  # the stored format itself: no dequantised copies
+            for mod, prefix, names in ((att, "attention.", ("wq", "wk", "wv", "wo")), (ff, "feed_forward.", ("w1", "w2", "w3"))):
+                for n in names:
+                    out[p + prefix + n + ".weight_e4m3"] = mod.weight_e4m3(n)
+                    out[p + prefix + n + ".weight_scale"] = mod.weight_scale(n)
+            return
         if hasattr(ff, "experts"):
             out[p + "feed_forward.gate.weight"] = ff.gate_weight
             for e, ex in ff.experts.items():  # keyed by the global expert id; the local ones only when sharded
@@ -762,6 +822,9 @@ class Transformer(nn.Module):
         lora_dtype = lora_dtypes.pop()
         assert lora_dtype == self.dtype, f"LoRA weights dtype differs from model's dtype {lora_dtype} != {self.dtype}"
         assert all("lora" in key for key in lora_state_dict.keys())
+        if self.dense_weights == "fp8" and any(key.startswith("layers.") for key in lora_state_dict):
+            raise NotImplementedError("merging a LoRA adapter into FP8 dense weights is not built: the layer Linears are stored quantised "
+                                      "(load the adapter into a bf16 model)")
         if self.expert_weights == "fp8" and any(".experts." in key for key in lora_state_dict):
             raise NotImplementedError("merging a LoRA adapter into FP8 expert weights is not built: the experts are stored quantised "
                                       "(load the adapter into a bf16 model, or drop its expert Linears)")
@@ -805,11 +868,12 @@ class Transformer(nn.Module):
     def from_folder(folder: Union[Path, str], max_batch_size: int = 1, num_pipeline_ranks: int = 1,
                     device: Union[torch.device, str] = "cuda", dtype: Optional[torch.dtype] = None,
                     softmax_fp32: bool = True, expert_parallel: Optional[Tuple[int, int]] = None, expert_group: Any = None,
-                    expert_weights: str = "bf16", *, kv_cache: str = "bf16") -> "Transformer":
+                    expert_weights: str = "bf16", *, kv_cache: str = "bf16", dense_weights: str = "bf16") -> "Transformer":
         """transformer.py:297-338.  Tensors stream from disk straight into the packed device buffers; with `expert_parallel`
         the experts of other ranks are skipped (never read into device memory).  With expert_weights="fp8" each bf16 expert
         tensor is copied to the device and quantised into place: the peak is the FP8 model plus about one bf16 tensor.
-        `kv_cache` ("bf16" | "fp8") is the format of the KV cache that generate() builds (see Transformer)."""
+        `kv_cache` ("bf16" | "fp8") is the format of the KV cache that generate() builds (see Transformer).  With
+        dense_weights="fp8" every bf16 layer Linear is quantised into place the same way."""
         with open(Path(folder) / "params.json", "r") as f:
             model_args = TransformerArgs.from_dict(json.load(f))
         model_args.max_batch_size = max_batch_size
@@ -829,7 +893,7 @@ class Transformer(nn.Module):
             # on meta and assigns, transformer.py:321-331; a fp32 build followed by .to(bf16) would need 3x the model's bytes)
             return Transformer.empty(model_args, dev, dtype or ck_dtype, pipeline_rank=pipeline_rank, num_pipeline_ranks=num_pipeline_ranks,
                                      softmax_fp32=softmax_fp32, expert_parallel=expert_parallel, expert_group=expert_group,
-                                     expert_weights=expert_weights, kv_cache=kv_cache)
+                                     expert_weights=expert_weights, kv_cache=kv_cache, dense_weights=dense_weights)
 
         if pt_model_file.exists():
             loaded = torch.load(str(pt_model_file), mmap=True)

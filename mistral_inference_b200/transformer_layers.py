@@ -6,6 +6,8 @@ include/mistral_b200.h); weights are stored pre-packed for the fused kernels:
   FeedForward.w13 [2 * hidden, dim], row 2i = w1[i], row 2i+1 = w3[i]  (SiLU*mul in the epilogue)
 `wq/wk/wv/w1/w3` are exposed as zero-copy views for state-dict compatibility.
 With `lora` set (un-merged adapters) each fused call also owns a packed LoraAdapter and runs the `_lora` entry points.
+With `fp8` (FP8 dense weights, include/mistral_b200.h) the packed matrices hold e4m3 bytes (uint8, same packing) next to one fp32
+scale per row, and every call runs the `_fp8` entry points.
 """
 from typing import List, Optional, Tuple
 
@@ -15,7 +17,7 @@ from torch import nn
 from . import _abi
 from .args import LoraArgs, MoeArgs
 from .cache import CacheView
-from .moe import Fp8Expert, MoeLayer
+from .moe import Fp8Expert, MoeLayer, quantize_rows_
 
 
 class _WeightView:
@@ -85,6 +87,29 @@ class LoraAdapter(nn.Module):
         return st
 
 
+class _Fp8Rows:
+    """FP8 dense storage of a module's packed matrices: `<m>` is uint8 [N, K] (e4m3 bit patterns), `<m>_scale_bits` int32 [N] the
+    bit patterns of the fp32 row scales (`Module.to(dtype)` casts every floating tensor; these must keep their bits).  `_slots`
+    maps a reference Linear name to its (q rows, scale entries): zero-copy views, strided where rows interleave."""
+
+    def _fp8_params(self, name: str, n: int, k: int) -> nn.Parameter:
+        setattr(self, name + "_scale_bits", nn.Parameter(torch.empty(n, dtype=torch.int32), requires_grad=False))
+        return nn.Parameter(torch.empty(n, k, dtype=torch.uint8), requires_grad=False)
+
+    def _slots(self, name: str) -> Tuple[torch.Tensor, torch.Tensor]:
+        raise NotImplementedError
+
+    def weight_e4m3(self, name: str) -> torch.Tensor:
+        return self._slots(name)[0].view(torch.float8_e4m3fn)
+
+    def weight_scale(self, name: str) -> torch.Tensor:
+        return self._slots(name)[1]
+
+    def quantize_(self, name: str, w: torch.Tensor) -> None:
+        """Quantises the bf16 weight `w` of Linear `name` into place (one bf16 copy of `w` on the device while it runs)."""
+        quantize_rows_(name, w, *self._slots(name))
+
+
 class RMSNorm(nn.Module):
     """transformer_layers.py:109-120."""
 
@@ -97,10 +122,10 @@ class RMSNorm(nn.Module):
         return _abi.rmsnorm(x, self.weight, self.eps)
 
 
-class Attention(nn.Module):
+class Attention(nn.Module, _Fp8Rows):
     """transformer_layers.py:31-93."""
 
-    def __init__(self, dim: int, n_heads: int, head_dim: int, n_kv_heads: int, lora: Optional[LoraArgs] = None):
+    def __init__(self, dim: int, n_heads: int, head_dim: int, n_kv_heads: int, lora: Optional[LoraArgs] = None, fp8: bool = False):
         super().__init__()
         self.dim = dim
         self.n_heads = n_heads
@@ -110,8 +135,13 @@ class Attention(nn.Module):
         self.scale = head_dim ** -0.5
         self.q_dim = n_heads * head_dim
         self.kv_dim = n_kv_heads * head_dim
-        self.wqkv = nn.Parameter(torch.empty(self.q_dim + 2 * self.kv_dim, dim), requires_grad=False)
-        self.wo_weight = nn.Parameter(torch.empty(dim, self.q_dim), requires_grad=False)
+        self.fp8 = fp8
+        if fp8:
+            self.wqkv = self._fp8_params("wqkv", self.q_dim + 2 * self.kv_dim, dim)
+            self.wo_weight = self._fp8_params("wo", dim, self.q_dim)
+        else:
+            self.wqkv = nn.Parameter(torch.empty(self.q_dim + 2 * self.kv_dim, dim), requires_grad=False)
+            self.wo_weight = nn.Parameter(torch.empty(dim, self.q_dim), requires_grad=False)
         self.lora = lora
         if lora is not None:
             self.wqkv_lora = LoraAdapter(dim, [self.q_dim, self.kv_dim, self.kv_dim], lora)
@@ -133,6 +163,22 @@ class Attention(nn.Module):
     @property
     def wo(self) -> _WeightView:
         return _WeightView(lambda: self.wo_weight)
+
+    @property
+    def wqkv_scale(self) -> torch.Tensor:
+        return self.wqkv_scale_bits.view(torch.float32)
+
+    @property
+    def wo_scale(self) -> torch.Tensor:
+        return self.wo_scale_bits.view(torch.float32)
+
+    def _slots(self, name: str) -> Tuple[torch.Tensor, torch.Tensor]:
+        rows = {"wq": slice(0, self.q_dim), "wk": slice(self.q_dim, self.q_dim + self.kv_dim), "wv": slice(self.q_dim + self.kv_dim, None)}
+        if name in rows:
+            return self.wqkv[rows[name]], self.wqkv_scale[rows[name]]
+        if name == "wo":
+            return self.wo_weight, self.wo_scale
+        raise ValueError(f"attention Linear {name!r}")
 
     def attend(self, x: torch.Tensor, norm_w: torch.Tensor, eps: float, rope: torch.Tensor, positions: torch.Tensor,
                cache: Optional[CacheView], ws: "_abi.Workspace") -> torch.Tensor:
@@ -185,7 +231,9 @@ class Attention(nn.Module):
 
     def _qkv(self, x, norm_w, rope, positions, q, k, v, cache_k, cache_v, cache_rows, eps, ws) -> None:
         H, KV, hd = self.n_heads, self.n_kv_heads, self.head_dim
-        if self.lora is None:
+        if self.fp8:
+            _abi.attn_qkv_fp8(x, norm_w, self.wqkv, self.wqkv_scale, rope, positions, q, k, v, cache_k, cache_v, cache_rows, H, KV, hd, eps, ws)
+        elif self.lora is None:
             _abi.attn_qkv(x, norm_w, self.wqkv, rope, positions, q, k, v, cache_k, cache_v, cache_rows, H, KV, hd, eps, ws)
         else:
             _abi.attn_qkv_lora(x, norm_w, self.wqkv, rope, positions, q, k, v, cache_k, cache_v, cache_rows, H, KV, hd, eps, ws,
@@ -193,7 +241,9 @@ class Attention(nn.Module):
 
     def project_out(self, a: torch.Tensor, residual: torch.Tensor, out: torch.Tensor, ws: "_abi.Workspace") -> None:
         """out = residual + wo(a)."""
-        if self.lora is None:
+        if self.fp8:
+            _abi.linear_residual_fp8(a, self.wo_weight, self.wo_scale, residual, out, ws)
+        elif self.lora is None:
             _abi.linear_residual(a, self.wo_weight, residual, out, ws)
         else:
             _abi.linear_residual_lora(a, self.wo_weight, residual, out, ws, self.wo_lora.call(a.shape[0]))
@@ -207,15 +257,20 @@ def decode_splits(B: int, KV: int, W: int, n_sm: int = 132) -> int:
     return int(max(1, min(s, 64, (W + 63) // 64)))
 
 
-class FeedForward(nn.Module):
+class FeedForward(nn.Module, _Fp8Rows):
     """transformer_layers.py:96-106."""
 
-    def __init__(self, dim: int, hidden_dim: int, lora: Optional[LoraArgs] = None):
+    def __init__(self, dim: int, hidden_dim: int, lora: Optional[LoraArgs] = None, fp8: bool = False):
         super().__init__()
         self.dim = dim
         self.hidden_dim = hidden_dim
-        self.w13 = nn.Parameter(torch.empty(2 * hidden_dim, dim), requires_grad=False)
-        self.w2_weight = nn.Parameter(torch.empty(dim, hidden_dim), requires_grad=False)
+        self.fp8 = fp8
+        if fp8:
+            self.w13 = self._fp8_params("w13", 2 * hidden_dim, dim)
+            self.w2_weight = self._fp8_params("w2", dim, hidden_dim)
+        else:
+            self.w13 = nn.Parameter(torch.empty(2 * hidden_dim, dim), requires_grad=False)
+            self.w2_weight = nn.Parameter(torch.empty(dim, hidden_dim), requires_grad=False)
         self.lora = lora
         if lora is not None:
             self.w13_lora = LoraAdapter(dim, [hidden_dim, hidden_dim], lora, interleaved=True)
@@ -233,13 +288,33 @@ class FeedForward(nn.Module):
     def w2(self) -> _WeightView:
         return _WeightView(lambda: self.w2_weight)
 
+    @property
+    def w13_scale(self) -> torch.Tensor:
+        return self.w13_scale_bits.view(torch.float32)
+
+    @property
+    def w2_scale(self) -> torch.Tensor:
+        return self.w2_scale_bits.view(torch.float32)
+
+    def _slots(self, name: str) -> Tuple[torch.Tensor, torch.Tensor]:
+        h, d = self.hidden_dim, self.dim
+        if name in ("w1", "w3"):
+            seg = 0 if name == "w1" else 1
+            return self.w13.view(h, 2, d)[:, seg], self.w13_scale.view(h, 2)[:, seg]
+        if name == "w2":
+            return self.w2_weight, self.w2_scale
+        raise ValueError(f"feed-forward Linear {name!r}")
+
     def run(self, x: torch.Tensor, norm_w: Optional[torch.Tensor], eps: float, residual: Optional[torch.Tensor],
             ws: "_abi.Workspace") -> torch.Tensor:
         """[norm] -> gate/up -> silu*mul -> down [+ residual]."""
         T = x.shape[0]
         g = torch.empty(T, self.hidden_dim, dtype=x.dtype, device=x.device)
         out = torch.empty(T, self.dim, dtype=x.dtype, device=x.device)
-        if self.lora is None:
+        if self.fp8:
+            _abi.ffn_gateup_fp8(x, norm_w, self.w13, self.w13_scale, g, eps, ws)
+            _abi.linear_residual_fp8(g, self.w2_weight, self.w2_scale, residual, out, ws)
+        elif self.lora is None:
             _abi.ffn_gateup(x, norm_w, self.w13, g, eps, ws)
             _abi.linear_residual(g, self.w2_weight, residual, out, ws)
         else:
@@ -257,7 +332,7 @@ class TransformerBlock(nn.Module):
 
     def __init__(self, dim: int, hidden_dim: int, n_heads: int, n_kv_heads: int, head_dim: int, norm_eps: float,
                  lora: Optional[LoraArgs] = None, moe: Optional[MoeArgs] = None, expert_shard: Tuple[int, int] = (0, 1), expert_group=None,
-                 expert_weights: str = "bf16"):
+                 expert_weights: str = "bf16", dense_weights: str = "bf16"):
         super().__init__()
         if lora is not None and moe is not None:
             raise NotImplementedError("un-merged LoRA on mixture-of-experts layers is not built: the grouped expert GEMMs have no "
@@ -265,7 +340,9 @@ class TransformerBlock(nn.Module):
         self.n_heads = n_heads
         self.dim = dim
         self.norm_eps = norm_eps
-        self.attention = Attention(dim=dim, n_heads=n_heads, head_dim=head_dim, n_kv_heads=n_kv_heads, lora=lora)
+        fp8 = dense_weights == "fp8"
+        assert not fp8 or (moe is None and lora is None), "FP8 dense weights: dense layers without un-merged LoRA only"
+        self.attention = Attention(dim=dim, n_heads=n_heads, head_dim=head_dim, n_kv_heads=n_kv_heads, lora=lora, fp8=fp8)
         self.attention_norm = RMSNorm(dim, eps=norm_eps)
         self.ffn_norm = RMSNorm(dim, eps=norm_eps)
         self.feed_forward: nn.Module
@@ -276,7 +353,7 @@ class TransformerBlock(nn.Module):
                                          gate_weight=nn.Parameter(torch.empty(moe.num_experts, dim), requires_grad=False), moe_args=moe,
                                          expert_shard=expert_shard, expert_group=expert_group)
         else:
-            self.feed_forward = FeedForward(dim=dim, hidden_dim=hidden_dim, lora=lora)
+            self.feed_forward = FeedForward(dim=dim, hidden_dim=hidden_dim, lora=lora, fp8=fp8)
 
     def forward(self, x: torch.Tensor, rope: torch.Tensor, positions: torch.Tensor, cache: Optional[CacheView],
                 ws: "_abi.Workspace") -> torch.Tensor:
