@@ -468,6 +468,43 @@ int mb200_decode_step_fp8(const mb200_layer_desc_fp8* layers_dev, const int32_t*
 int mb200_decode_step_fp8_supported(int64_t dim, int64_t hidden, int64_t n_heads, int64_t n_kv_heads, int64_t head_dim, int64_t vocab,
                                     int64_t smem_optin);
 
+/* ---------------------------------------------------------------------------------------------
+ * INT4 dense weights (Python: Transformer(..., dense_weights="int4")).  Each layer Linear's weight W [N, K] (K % 128 == 0) is
+ * stored as symmetric 4-bit codes with one bf16 scale per group g of 128 consecutive k of a row, written by
+ * mb200_quantize_int4_groups:
+ *     a[n, g]  = max over k in group g of |W[n, k]|                                  (fp32)
+ *     s[n, g]  = 1 if a == 0, else bf16_rn(fp32(a / 7)), raised to the smallest positive bf16 (2^-133) if that rounds to 0
+ *     q[n, k]  = clamp(rint_even(fp32(W[n, k]) / fp32(s[n, g])), -8, 7)                 (IEEE division)
+ *     W'[n, k] = bf16_rn(fp32(q) * fp32(s))                                            (q * s is exact in fp32: one rounding)
+ * Storage: codes uint8 [N, K/2], byte j of a row holding q + 8 of k = 2j in its low nibble and of k = 2j + 1 in its high nibble;
+ * scales bf16 [N, K/128].  The packing is the bf16 one: wqkv rows cat(q, k, v), w13 rows interleaved w1 / w3.  W' is never
+ * materialised in memory: the kernels form it in registers or shared memory with two exact bf16x2 instructions per pair
+ * ((0x4300 | (q + 8)) - 136 = q, then one bf16 multiply by s).
+ * The INT4 model computes what the bf16 model computes with weights W': every Linear is bf16(x W'^T) with fp32 accumulation,
+ * followed by the mode's own epilogue exactly as in the bf16 entry points.  From 128 tokens on the kernels also keep the bf16
+ * kernels' tiles and k order, so their results equal the bf16 entry point on W' bit for bit.
+ *
+ * mb200_quantize_int4_groups: w bf16 [rows, K] contiguous; code row r at q + r * q_row_stride bytes, scale row r at
+ *     scale + r * scale_row_stride elements (strided rows: w1 / w3 land in the interleaved w13 rows).
+ * mb200_attn_qkv_int4, mb200_ffn_gateup_int4, mb200_linear_residual_int4: the counterpart's arguments with the weight replaced by
+ *     w_q (codes [N, K/2]) and w_gscale (bf16 scales [N, K/128]).  Kernel choice is that of the _fp8 trio (T <= 4: weight-streaming
+ *     GEMV; 5..128 tokens with N % 128 == 0: stream-K; else wgmma, single CTA at the bf16 tile width); K % 128 != 0, or a shape the
+ *     bf16 path would run on mma.sync, returns MB200_E_INVALID.
+ */
+int mb200_quantize_int4_groups(const void* w, int64_t rows, int64_t K, void* q, int64_t q_row_stride, void* scale, int64_t scale_row_stride,
+                               void* stream);
+int mb200_attn_qkv_int4(const void* x, const void* norm_w, const void* w_q, const void* w_gscale, const float* rope, const int32_t* positions,
+                        void* q_out, void* k_out, void* v_out, void* cache_k, void* cache_v, const int32_t* cache_rows, int64_t T, int64_t dim,
+                        int64_t n_heads, int64_t n_kv_heads, int64_t head_dim, float eps, void* workspace, size_t workspace_bytes, void* stream);
+int mb200_ffn_gateup_int4(const void* x, const void* norm_w, const void* w_q, const void* w_gscale, void* g_out, int64_t T, int64_t dim,
+                          int64_t hidden, float eps, void* workspace, size_t workspace_bytes, void* stream);
+int mb200_linear_residual_int4(const void* x, const void* w_q, const void* w_gscale, const void* residual, void* out, int64_t T, int64_t N,
+                               int64_t K, void* workspace, size_t workspace_bytes, void* stream);
+
+/* Debug: CTAs of attn_decode_tma_kernel<rep> (rep = H/KV) resident per SM on the current device, from
+ * cudaOccupancyMaxActiveBlocksPerMultiprocessor at the kernel's launch configuration. */
+int mb200_debug_attn_decode_occupancy(int64_t rep, int* blocks_per_sm);
+
 /* Test-only: CUDA-core fp32 GEMM c[T, N] = a[T, K] w[N, K]^T used to cross-check the tensor-core kernels. */
 int mb200_test_gemm_naive(const void* a, const void* w, float* c, int64_t T, int64_t N, int64_t K, void* stream);
 

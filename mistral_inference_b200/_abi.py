@@ -89,6 +89,14 @@ _SIGNATURES = {
                                       c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int64, c_int64, c_int64, c_float, c_void_p, c_size_t,
                                       c_void_p]),
     "mb200_decode_step_fp8_supported": (c_int, [c_int64] * 7),
+    "mb200_quantize_int4_groups": (c_int, [c_void_p, c_int64, c_int64, c_void_p, c_int64, c_void_p, c_int64, c_void_p]),
+    "mb200_attn_qkv_int4": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                    c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int64, c_int64, c_float, c_void_p, c_size_t, c_void_p]),
+    "mb200_ffn_gateup_int4": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_float, c_void_p,
+                                      c_size_t, c_void_p]),
+    "mb200_linear_residual_int4": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_void_p,
+                                           c_size_t, c_void_p]),
+    "mb200_debug_attn_decode_occupancy": (c_int, [c_int64, ctypes.POINTER(c_int)]),
     "mb200_test_gemm_naive": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_void_p]),
 }
 
@@ -321,6 +329,57 @@ def linear_residual_fp8(x, w_q, w_scale, residual, out, ws: Workspace) -> None:
     N = w_q.shape[0]
     _check(lib().mb200_linear_residual_fp8(_ptr(x), _ptr(w_q), _ptr(w_scale), _ptr(residual), _ptr(out), T, N, K, ws.ptr, ws.nbytes,
                                            _stream()), "mb200_linear_residual_fp8")
+
+
+# ---- INT4 dense weights (include/mistral_b200.h): w_q the packed codes uint8 [N, K/2], w_gscale the bf16 group scales [N, K/128] ----
+def _check_int4(w_q: torch.Tensor, w_gscale: torch.Tensor) -> None:
+    assert w_q.dtype == torch.uint8 and w_gscale.dtype == torch.bfloat16, (w_q.dtype, w_gscale.dtype)
+    assert w_q.is_contiguous() and w_gscale.is_contiguous() and w_gscale.shape == (w_q.shape[0], w_q.shape[1] // 64), \
+        (tuple(w_q.shape), tuple(w_gscale.shape))
+
+
+def attn_qkv_int4(x, norm_w, w_q, w_gscale, rope, positions, q_out, k_out, v_out, cache_k, cache_v, cache_rows, n_heads, n_kv_heads,
+                  head_dim, eps, ws: Workspace) -> None:
+    _check_int4(w_q, w_gscale)
+    T, dim = x.shape
+    _check(lib().mb200_attn_qkv_int4(_ptr(x), _ptr(norm_w), _ptr(w_q), _ptr(w_gscale), _ptr(rope), _ptr(positions), _ptr(q_out),
+                                     _ptr(k_out), _ptr(v_out), _ptr(cache_k), _ptr(cache_v), _ptr(cache_rows), T, dim, n_heads, n_kv_heads,
+                                     head_dim, eps, ws.ptr, ws.nbytes, _stream()), "mb200_attn_qkv_int4")
+
+
+def ffn_gateup_int4(x, norm_w, w_q, w_gscale, g_out, eps, ws: Workspace) -> None:
+    _check_int4(w_q, w_gscale)
+    T, dim = x.shape
+    hidden = w_q.shape[0] // 2
+    _check(lib().mb200_ffn_gateup_int4(_ptr(x), _ptr(norm_w), _ptr(w_q), _ptr(w_gscale), _ptr(g_out), T, dim, hidden, eps, ws.ptr,
+                                       ws.nbytes, _stream()), "mb200_ffn_gateup_int4")
+
+
+def linear_residual_int4(x, w_q, w_gscale, residual, out, ws: Workspace) -> None:
+    _check_int4(w_q, w_gscale)
+    T, K = x.shape
+    N = w_q.shape[0]
+    _check(lib().mb200_linear_residual_int4(_ptr(x), _ptr(w_q), _ptr(w_gscale), _ptr(residual), _ptr(out), T, N, K, ws.ptr, ws.nbytes,
+                                            _stream()), "mb200_linear_residual_int4")
+
+
+def attn_decode_occupancy(rep: int) -> int:
+    """CTAs of attn_decode_tma_kernel<rep> resident per SM on the current device."""
+    n = c_int(0)
+    _check(lib().mb200_debug_attn_decode_occupancy(rep, ctypes.byref(n)), "mb200_debug_attn_decode_occupancy")
+    return int(n.value)
+
+
+def quantize_int4_groups(w: torch.Tensor, q: torch.Tensor, gscale: torch.Tensor) -> None:
+    """q (uint8 [rows, K/2]) and gscale (bf16 [rows, K/128]) of the bf16 matrix w [rows, K]; both may be row-strided views."""
+    rows, K = w.shape
+    assert w.dtype == torch.bfloat16 and w.is_contiguous() and q.dtype == torch.uint8 and gscale.dtype == torch.bfloat16, \
+        (w.dtype, q.dtype, gscale.dtype)
+    assert q.shape == (rows, K // 2) and q.stride(1) == 1 and gscale.shape == (rows, K // 128) and gscale.stride(1) == 1, \
+        (tuple(q.shape), tuple(gscale.shape))
+    assert q.is_cuda and gscale.is_cuda and w.device == q.device == gscale.device
+    _check(lib().mb200_quantize_int4_groups(_ptr(w), rows, K, q.data_ptr(), q.stride(0), gscale.data_ptr(), gscale.stride(0), _stream()),
+           "mb200_quantize_int4_groups")
 
 
 class LoraStruct(ctypes.Structure):

@@ -12,6 +12,7 @@
 #include "gemm_mma.cuh"
 #include "gemm_streamk.cuh"
 #include "gemm_wgmma.cuh"
+#include "int4.cuh"
 #include "kv_fp8.cuh"
 #include "lora.cuh"
 #include "moe.cuh"
@@ -119,13 +120,22 @@ static int run_linear(const void* x, const void* norm_w, const void* w, const Ep
   return launch_gemm_mma<MODE>(g, st);
 }
 
-// FP8 dense weights (include/mistral_b200.h): w is e4m3 [N, K], epi.w_scale its fp32 row scales.  The bf16 dispatch, except that
-// a shape run_linear would give to gemm_mma_kernel is refused: that kernel has no e4m3 variant.
-template <int MODE>
-static int run_linear_fp8(const void* x, const void* norm_w, const void* w, const EpiParams& epi, int64_t T, int64_t N, int64_t K, float eps,
-                          void* workspace, size_t workspace_bytes, cudaStream_t st) {
-  MB_CHECK_ARG(T >= 1, "linear (fp8): T=%lld", (long long)T);
-  MB_CHECK_ARG(epi.w_scale != nullptr && ((uintptr_t)epi.w_scale & 7) == 0, "linear (fp8): w_scale must be an 8-byte aligned fp32 array");
+// Quantised dense weights (include/mistral_b200.h): the bf16 dispatch of run_linear, except that a shape it would give to
+// gemm_mma_kernel is refused (that kernel has no quantised variant).  One function for both formats, so the regime choice lives here
+// once.  FP8 (INT4 = false): w is e4m3 [N, K], epi.w_scale its fp32 row scales, applied by the epilogue (EPI_WSCALE).  INT4: w is
+// the packed code matrix [N, K/2], gscale its bf16 group scales [N, K/128]; the kernels convert to W' and keep the bf16 epilogue.
+template <int MODE, bool INT4>
+static int run_linear_quant(const void* x, const void* norm_w, const void* w, const uint16_t* gscale, const EpiParams& epi, int64_t T,
+                            int64_t N, int64_t K, float eps, void* workspace, size_t workspace_bytes, cudaStream_t st) {
+  const char* fmt = INT4 ? "int4" : "fp8";
+  constexpr int KMODE = INT4 ? MODE : (MODE | EPI_WSCALE);  // the kernels' epilogue mode
+  MB_CHECK_ARG(T >= 1, "linear (%s): T=%lld", fmt, (long long)T);
+  if constexpr (INT4) {
+    MB_CHECK_ARG(gscale != nullptr && ((uintptr_t)gscale & 1) == 0 && ((uintptr_t)w & 15) == 0, "linear (int4): misaligned or null weights");
+    MB_CHECK_ARG(K % kInt4Group == 0, "linear (int4): K=%lld must be a multiple of 128", (long long)K);
+  } else {
+    MB_CHECK_ARG(epi.w_scale != nullptr && ((uintptr_t)epi.w_scale & 7) == 0, "linear (fp8): w_scale must be an 8-byte aligned fp32 array");
+  }
   if (T <= MB200_SKINNY_MAX_T) {
     SkinnyParams p;
     p.x = x;
@@ -135,11 +145,18 @@ static int run_linear_fp8(const void* x, const void* norm_w, const void* w, cons
     p.K = (int)K;
     p.eps = eps;
     p.epi = epi;
-    return norm_w ? launch_skinny_fp8<MODE | EPI_WSCALE, true>(p, (int)T, st) : launch_skinny_fp8<MODE | EPI_WSCALE, false>(p, (int)T, st);
+    if constexpr (INT4) {
+      p.gscale = gscale;
+      // attn_qkv always norms its input: no un-normed QKV instantiation (it would spill 8 bytes at T = 4)
+      if constexpr (MODE == EPI_QKV_ROPE) return launch_skinny_int4<KMODE, true>(p, (int)T, st);
+      else return norm_w ? launch_skinny_int4<KMODE, true>(p, (int)T, st) : launch_skinny_int4<KMODE, false>(p, (int)T, st);
+    } else {
+      return norm_w ? launch_skinny_fp8<KMODE, true>(p, (int)T, st) : launch_skinny_fp8<KMODE, false>(p, (int)T, st);
+    }
   }
   const bool sk = streamk_eligible(T, N, K);
-  MB_CHECK_ARG(sk || wgmma_gemm_eligible(T, N, K), "linear (fp8): T=%lld N=%lld K=%lld needs the mma.sync GEMM, which has no e4m3 variant",
-               (long long)T, (long long)N, (long long)K);
+  MB_CHECK_ARG(sk || wgmma_gemm_eligible(T, N, K), "linear (%s): T=%lld N=%lld K=%lld needs the mma.sync GEMM, which has no %s variant", fmt,
+               (long long)T, (long long)N, (long long)K, INT4 ? "int4" : "e4m3");
   const void* a = x;
   if (norm_w) {
     const WsRegion nr = ws_normed(T, K);
@@ -156,8 +173,13 @@ static int run_linear_fp8(const void* x, const void* norm_w, const void* w, cons
   g.N = (int)N;
   g.K = (int)K;
   g.epi = epi;
-  if (sk) return launch_streamk_fp8<MODE | EPI_WSCALE>(g, workspace, workspace_bytes, st);
-  return launch_gemm_wgmma_fp8<MODE | EPI_WSCALE>(g, st);
+  if constexpr (INT4) {
+    if (sk) return launch_streamk_int4<KMODE>(g, gscale, workspace, workspace_bytes, st);
+    return launch_gemm_wgmma_int4<KMODE>(g, gscale, st);
+  } else {
+    if (sk) return launch_streamk_fp8<KMODE>(g, workspace, workspace_bytes, st);
+    return launch_gemm_wgmma_fp8<KMODE>(g, st);
+  }
 }
 
 // Un-merged LoRA around one fused Linear (include/mistral_b200.h): down projection -> up projection -> base GEMM whose epilogue
@@ -246,7 +268,7 @@ int mb200_rmsnorm(const void* x, const void* w, void* out, int64_t T, int64_t di
 static int attn_qkv_impl(const void* x, const void* norm_w, const void* wqkv, const float* rope, const int32_t* positions, void* q_out,
                          void* k_out, void* v_out, void* cache_k, void* cache_v, const int32_t* cache_rows, int64_t T, int64_t dim,
                          int64_t n_heads, int64_t n_kv_heads, int64_t head_dim, float eps, void* workspace, size_t workspace_bytes,
-                         void* stream, const mb200_lora* lora, const float* w_scale = nullptr) {
+                         void* stream, const mb200_lora* lora, const float* w_scale = nullptr, const uint16_t* w_gscale = nullptr) {
   MB_CHECK_ARG(x && norm_w && wqkv && rope && positions && q_out && k_out && v_out, "attn_qkv: null pointer");
   MB_CHECK_ARG(head_dim == kHeadDim || head_dim == 64, "attn_qkv: head_dim=%lld unsupported (64 or 128)", (long long)head_dim);
   MB_CHECK_ARG(cache_rows == nullptr || (cache_k && cache_v), "attn_qkv: cache_rows without cache pointers");
@@ -265,8 +287,10 @@ static int attn_qkv_impl(const void* x, const void* norm_w, const void* wqkv, co
   const int64_t N = (n_heads + 2 * n_kv_heads) * head_dim;
   if (w_scale) {
     e.w_scale = w_scale;
-    return run_linear_fp8<EPI_QKV_ROPE>(x, norm_w, wqkv, e, T, N, dim, eps, workspace, workspace_bytes, (cudaStream_t)stream);
+    return run_linear_quant<EPI_QKV_ROPE, false>(x, norm_w, wqkv, nullptr, e, T, N, dim, eps, workspace, workspace_bytes, (cudaStream_t)stream);
   }
+  if (w_gscale) return run_linear_quant<EPI_QKV_ROPE, true>(x, norm_w, wqkv, w_gscale, e, T, N, dim, eps, workspace, workspace_bytes,
+                                                                 (cudaStream_t)stream);
   if (lora) return run_linear_lora<EPI_QKV_ROPE>(x, norm_w, wqkv, e, lora, T, N, dim, eps, workspace, workspace_bytes, (cudaStream_t)stream);
   return run_linear<EPI_QKV_ROPE>(x, norm_w, wqkv, e, T, N, dim, eps, workspace, workspace_bytes, (cudaStream_t)stream);
 }
@@ -352,8 +376,26 @@ int mb200_attn_decode(const void* q, const void* cache_k, const void* cache_v, c
     case 4: return launch_attn_decode_tma<4>(p, B * W, st);
     case 6: return launch_attn_decode_tma<6>(p, B * W, st);
     case 8: return launch_attn_decode_tma<8>(p, B * W, st);
-    default: return fail(MB200_E_INVALID, "attn_decode: H/KV=%d unsupported (1,2,4,6,8)", rep);
+    case 12: return launch_attn_decode_tma<12>(p, B * W, st);
+    default: return fail(MB200_E_INVALID, "attn_decode: H/KV=%d unsupported (1,2,4,6,8,12)", rep);
   }
+}
+
+int mb200_debug_attn_decode_occupancy(int64_t rep, int* blocks_per_sm) {
+  MB_CHECK_ARG(blocks_per_sm, "debug_attn_decode_occupancy: null pointer");
+  const void* fn = nullptr;
+  switch (rep) {
+    case 1: fn = (const void*)attn_decode_tma_kernel<1>; break;
+    case 2: fn = (const void*)attn_decode_tma_kernel<2>; break;
+    case 4: fn = (const void*)attn_decode_tma_kernel<4>; break;
+    case 6: fn = (const void*)attn_decode_tma_kernel<6>; break;
+    case 8: fn = (const void*)attn_decode_tma_kernel<8>; break;
+    case 12: fn = (const void*)attn_decode_tma_kernel<12>; break;
+    default: return fail(MB200_E_INVALID, "debug_attn_decode_occupancy: H/KV=%lld not compiled", (long long)rep);
+  }
+  MB_CHECK_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, ADT_SMEM));
+  MB_CHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(blocks_per_sm, fn, ADT_THREADS, ADT_SMEM));
+  return MB200_OK;
 }
 
 int mb200_attn_prefill(const void* q, const void* k_new, const void* v_new, const void* cache_k, const void* cache_v, const int32_t* q_start,
@@ -528,8 +570,8 @@ int mb200_linear_residual_fp8(const void* x, const void* w_q, const float* w_sca
   e.residual = residual;
   e.ld_out = N;
   e.w_scale = w_scale;
-  if (residual) return run_linear_fp8<EPI_RESIDUAL>(x, nullptr, w_q, e, T, N, K, 0.f, workspace, workspace_bytes, (cudaStream_t)stream);
-  return run_linear_fp8<EPI_STORE>(x, nullptr, w_q, e, T, N, K, 0.f, workspace, workspace_bytes, (cudaStream_t)stream);
+  if (residual) return run_linear_quant<EPI_RESIDUAL, false>(x, nullptr, w_q, nullptr, e, T, N, K, 0.f, workspace, workspace_bytes, (cudaStream_t)stream);
+  return run_linear_quant<EPI_STORE, false>(x, nullptr, w_q, nullptr, e, T, N, K, 0.f, workspace, workspace_bytes, (cudaStream_t)stream);
 }
 
 int mb200_ffn_gateup_fp8(const void* x, const void* norm_w, const void* w_q, const float* w_scale, void* g_out, int64_t T, int64_t dim,
@@ -539,7 +581,53 @@ int mb200_ffn_gateup_fp8(const void* x, const void* norm_w, const void* w_q, con
   e.out = g_out;
   e.ld_out = hidden;
   e.w_scale = w_scale;
-  return run_linear_fp8<EPI_SWIGLU>(x, norm_w, w_q, e, T, 2 * hidden, dim, eps, workspace, workspace_bytes, (cudaStream_t)stream);
+  return run_linear_quant<EPI_SWIGLU, false>(x, norm_w, w_q, nullptr, e, T, 2 * hidden, dim, eps, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+int mb200_attn_qkv_int4(const void* x, const void* norm_w, const void* w_q, const void* w_gscale, const float* rope, const int32_t* positions,
+                        void* q_out, void* k_out, void* v_out, void* cache_k, void* cache_v, const int32_t* cache_rows, int64_t T, int64_t dim,
+                        int64_t n_heads, int64_t n_kv_heads, int64_t head_dim, float eps, void* workspace, size_t workspace_bytes, void* stream) {
+  MB_CHECK_ARG(w_gscale, "attn_qkv_int4: null group scales");
+  return attn_qkv_impl(x, norm_w, w_q, rope, positions, q_out, k_out, v_out, cache_k, cache_v, cache_rows, T, dim, n_heads, n_kv_heads,
+                       head_dim, eps, workspace, workspace_bytes, stream, nullptr, nullptr, (const uint16_t*)w_gscale);
+}
+
+int mb200_linear_residual_int4(const void* x, const void* w_q, const void* w_gscale, const void* residual, void* out, int64_t T, int64_t N,
+                               int64_t K, void* workspace, size_t workspace_bytes, void* stream) {
+  MB_CHECK_ARG(x && w_q && w_gscale && out, "linear_residual_int4: null pointer");
+  EpiParams e;
+  e.out = out;
+  e.residual = residual;
+  e.ld_out = N;
+  const uint16_t* gs = (const uint16_t*)w_gscale;
+  if (residual) return run_linear_quant<EPI_RESIDUAL, true>(x, nullptr, w_q, gs, e, T, N, K, 0.f, workspace, workspace_bytes, (cudaStream_t)stream);
+  return run_linear_quant<EPI_STORE, true>(x, nullptr, w_q, gs, e, T, N, K, 0.f, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+int mb200_ffn_gateup_int4(const void* x, const void* norm_w, const void* w_q, const void* w_gscale, void* g_out, int64_t T, int64_t dim,
+                          int64_t hidden, float eps, void* workspace, size_t workspace_bytes, void* stream) {
+  MB_CHECK_ARG(x && w_q && w_gscale && g_out, "ffn_gateup_int4: null pointer");
+  EpiParams e;
+  e.out = g_out;
+  e.ld_out = hidden;
+  return run_linear_quant<EPI_SWIGLU, true>(x, norm_w, w_q, (const uint16_t*)w_gscale, e, T, 2 * hidden, dim, eps, workspace, workspace_bytes,
+                                     (cudaStream_t)stream);
+}
+
+int mb200_quantize_int4_groups(const void* w, int64_t rows, int64_t K, void* q, int64_t q_row_stride, void* scale, int64_t scale_row_stride,
+                               void* stream) {
+  MB_CHECK_ARG(w && q && scale, "quantize_int4_groups: null pointer");
+  MB_CHECK_ARG(rows >= 1 && rows <= 0x7fffffff && K >= kInt4Group && K % kInt4Group == 0 && K <= (1 << 24),
+               "quantize_int4_groups: rows=%lld K=%lld (K a multiple of 128)", (long long)rows, (long long)K);
+  MB_CHECK_ARG(q_row_stride >= K / 2 && q_row_stride % 4 == 0 && scale_row_stride >= K / kInt4Group,
+               "quantize_int4_groups: q_row_stride=%lld (>= K/2, multiple of 4) scale_row_stride=%lld (>= K/128)", (long long)q_row_stride,
+               (long long)scale_row_stride);
+  MB_CHECK_ARG(((uintptr_t)w & 15) == 0 && ((uintptr_t)q & 3) == 0 && ((uintptr_t)scale & 1) == 0, "quantize_int4_groups: misaligned pointer");
+  quantize_int4_groups_kernel<<<(unsigned)rows, 256, 0, (cudaStream_t)stream>>>((const uint4*)w, (int)K, (uint8_t*)q, q_row_stride,
+                                                                                (uint16_t*)scale, scale_row_stride);
+  MB_CHECK_LAUNCH("quantize_int4_groups_kernel");
+  note_launch("quantize_int4_groups_kernel");
+  return MB200_OK;
 }
 
 int mb200_linear_residual_lora(const void* x, const void* w, const void* residual, void* out, int64_t T, int64_t N, int64_t K,

@@ -15,6 +15,9 @@
 // publishes its (m, l, acc) partial and the last CTA to arrive per (b, g) merges them.  Slots >= kv_len are uninitialised
 // memory in the reference (cache.py:166): their scores are masked by index and their V rows are zeroed in shared memory before
 // the PV product.
+// REP > 8 (H/KV = 12, Mistral Large 2): query heads 8 .. REP-1 of the group are MMA rows 8 .. REP-1 (the a1 / a3 halves of the Q
+// fragment, o[n][2..3], a second running (m, l) per thread).  Their merge arrays (sm_acc, cm, cl: 30 KB at REP = 12) live in the
+// K/V ring, which is idle once every tile is consumed, so the CTA keeps the shared-memory size that lets two of them share an SM.
 #pragma once
 #include "decode_megakernel.cuh"  // mbarrier helpers with the watchdog
 #include "gemm_mma.cuh"
@@ -136,10 +139,17 @@ __global__ void __launch_bounds__(ADT_THREADS, 2)
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + ADT_STAGES * ADT_STAGE_BYTES);
   uint64_t* empty = full + ADT_STAGES;
+  constexpr bool HI = REP > 8;  // query heads in MMA rows 8..15 too
+  static_assert(REP <= 16, "one m16 MMA tile of query heads");
   __shared__ float sm_m[ADT_CONSUMER_WARPS][REP], sm_l[ADT_CONSUMER_WARPS][REP];
-  __shared__ float sm_acc[ADT_CONSUMER_WARPS][REP][kHeadDim];
+  __shared__ float sm_acc_s[ADT_CONSUMER_WARPS][HI ? 1 : REP][kHeadDim];
   __shared__ int is_last;
-  __shared__ float cm[64 * REP], cl[64 * REP];
+  __shared__ float cm_s[64 * (HI ? 1 : REP)], cl_s[64 * (HI ? 1 : REP)];
+  typedef float AccArr[ADT_CONSUMER_WARPS][REP][kHeadDim];
+  AccArr& sm_acc = HI ? *reinterpret_cast<AccArr*>(smem) : *reinterpret_cast<AccArr*>(&sm_acc_s[0][0][0]);
+  float* cm = HI ? reinterpret_cast<float*>(smem + sizeof(AccArr)) : cm_s;
+  float* cl = HI ? cm + 64 * REP : cl_s;
+  static_assert(!HI || sizeof(AccArr) + 2 * 64 * REP * sizeof(float) <= ADT_STAGES * ADT_STAGE_BYTES, "merge arrays fit the ring");
 
   const int s = blockIdx.x, g = blockIdx.y, b = blockIdx.z;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -164,6 +174,7 @@ __global__ void __launch_bounds__(ADT_THREADS, 2)
   constexpr float kMasked = -1.0e30f;
   float o[16][4];
   float m_run = kMasked, l_run = 0.f;
+  float m_hi = kMasked, l_hi = 0.f;  // HI: MMA row + 8
   const int row = lane >> 2, cq = lane & 3;
 
   if (warp == ADT_CONSUMER_WARPS) {
@@ -192,6 +203,11 @@ __global__ void __launch_bounds__(ADT_THREADS, 2)
         const bf16* qp = p.q + ((int64_t)b * p.H + g * REP + row) * kHeadDim + ks * 16 + cq * 2;
         qa[ks][0] = *reinterpret_cast<const uint32_t*>(qp);
         qa[ks][2] = *reinterpret_cast<const uint32_t*>(qp + 8);
+      }
+      if (HI && row + 8 < REP) {
+        const bf16* qp = p.q + ((int64_t)b * p.H + g * REP + row + 8) * kHeadDim + ks * 16 + cq * 2;
+        qa[ks][1] = *reinterpret_cast<const uint32_t*>(qp);
+        qa[ks][3] = *reinterpret_cast<const uint32_t*>(qp + 8);
       }
     }
 #pragma unroll
@@ -251,6 +267,33 @@ __global__ void __launch_bounds__(ADT_THREADS, 2)
           o[n][0] *= corr;
           o[n][1] *= corr;
         }
+        if constexpr (HI) {  // the same online softmax for MMA row + 8 (accumulator elements 2, 3)
+          float mx2 = m_hi;
+#pragma unroll
+          for (int t = 0; t < 2; ++t)
+#pragma unroll
+            for (int c = 2; c < 4; ++c) {
+              const int key = t * 8 + cq * 2 + c - 2;
+              sc[t][c] = key < nk ? sc[t][c] * sl2 : kMasked;
+              mx2 = fmaxf(mx2, sc[t][c]);
+            }
+          mx2 = fmaxf(mx2, __shfl_xor_sync(0xffffffffu, mx2, 1));
+          mx2 = fmaxf(mx2, __shfl_xor_sync(0xffffffffu, mx2, 2));
+          const float corr2 = exp2f(m_hi - mx2);
+          m_hi = mx2;
+          l_hi *= corr2;
+#pragma unroll
+          for (int t = 0; t < 2; ++t) {
+            const float e2 = exp2f(sc[t][2] - mx2), e3 = exp2f(sc[t][3] - mx2);
+            l_hi += e2 + e3;
+            pa[2 * t + 1] = pack_bf16x2(e2, e3);
+          }
+#pragma unroll
+          for (int n = 0; n < 16; ++n) {
+            o[n][2] *= corr2;
+            o[n][3] *= corr2;
+          }
+        }
         const int vrow = 16 * warp + (lane & 7) + ((lane >> 3) & 1) * 8;
 #pragma unroll
         for (int n2 = 0; n2 < 8; ++n2) {
@@ -265,7 +308,10 @@ __global__ void __launch_bounds__(ADT_THREADS, 2)
     }
     l_run += __shfl_xor_sync(0xffffffffu, l_run, 1);
     l_run += __shfl_xor_sync(0xffffffffu, l_run, 2);
-    if (row < REP) {
+    if constexpr (HI) {
+      l_hi += __shfl_xor_sync(0xffffffffu, l_hi, 1);
+      l_hi += __shfl_xor_sync(0xffffffffu, l_hi, 2);
+    } else if (row < REP) {
 #pragma unroll
       for (int n = 0; n < 16; ++n) {
         sm_acc[warp][row][n * 8 + cq * 2] = o[n][0];
@@ -274,6 +320,31 @@ __global__ void __launch_bounds__(ADT_THREADS, 2)
       if (cq == 0) {
         sm_m[warp][row] = m_run;
         sm_l[warp][row] = l_run;
+      }
+    }
+  }
+  if constexpr (HI) {
+    __syncthreads();  // every warp is done with the ring: the merge arrays may overwrite it
+    if (warp < ADT_CONSUMER_WARPS) {
+#pragma unroll
+      for (int n = 0; n < 16; ++n) {
+        sm_acc[warp][row][n * 8 + cq * 2] = o[n][0];
+        sm_acc[warp][row][n * 8 + cq * 2 + 1] = o[n][1];
+      }
+      if (cq == 0) {
+        sm_m[warp][row] = m_run;
+        sm_l[warp][row] = l_run;
+      }
+      if (row + 8 < REP) {
+#pragma unroll
+        for (int n = 0; n < 16; ++n) {
+          sm_acc[warp][row + 8][n * 8 + cq * 2] = o[n][2];
+          sm_acc[warp][row + 8][n * 8 + cq * 2 + 1] = o[n][3];
+        }
+        if (cq == 0) {
+          sm_m[warp][row + 8] = m_hi;
+          sm_l[warp][row + 8] = l_hi;
+        }
       }
     }
   }

@@ -22,6 +22,8 @@
 // stored --, N = 128, fp32 accumulators in registers) and running the pair epilogues of epilogue.cuh on its fragment.  GROUPED: the mixture-of-experts variant -- m
 // tiles (expert segments of <= TA rows) come from the device-side plan of csrc/moe.cuh, each with its own weight tensor map.
 #pragma once
+#include <type_traits>
+
 #include "gemm_wgmma.cuh"
 #include "workspace.cuh"
 
@@ -55,20 +57,58 @@ struct SkParams {
   unsigned* flags;  // [gridDim], zero between launches
 };
 
+// W4 stages.  A 64-wide k-block of a 128-row INT4 tile is 4 KB of codes, and a weight stage must carry 16 KB to stream at the HBM
+// rate (above).  So the codes do not travel with the stages: one TMA brings a CHUNK of up to four consecutive k-blocks of one tile
+// ([128 rows x 128 B] = 16 KB) into a ring of its own, and warps 1-3 convert it k-block by k-block into the bf16 W' tiles of the
+// ordinary stages.  A chunk starts at the first unit of a CTA's range, at the first k-block of a tile, or after four k-blocks; a
+// chunk cut short by the range end reads up to three k-blocks it does not use (past K they read as zero).  The units, their
+// partition over the CTAs and every tile's k order stay the bf16 kernel's.
+constexpr int SK_W4_CHUNK_KB = 4, SK_W4_CHUNK_BYTES = SK_BN * SK_W4_CHUNK_KB * TG_BK / 2, SK_W4_SLOTS = 4;
+template <int TA>
+struct SkW4Cfg {  // the bf16 stage (A + W' tile) and, after the stages, the chunk ring
+  using B = TgCfg<SK_BN, TA>;
+  static constexpr int kABytes = B::kABytes, kBBytes = B::kBBytes, kStageBytes = B::kStageBytes, kSlack = B::kSlack;
+  static constexpr int kWG = B::kWG, kThreads = B::kThreads, kRawBytes = 0;
+  static constexpr int kRing = SK_W4_SLOTS * SK_W4_CHUNK_BYTES;
+  static constexpr int kFit = (227 * 1024 - 1024 - 512 - kSlack - kRing) / kStageBytes;
+  static constexpr int kStages = B::kStages < kFit ? B::kStages : kFit;
+  static constexpr int kSmem = kStages * kStageBytes + kSlack + kRing + 1024 + 512;
+  static_assert(kStages >= 3 && kSmem <= 227 * 1024, "W4 stream-K shared memory plan");
+};
+__device__ __forceinline__ bool mbar_test_wait(uint64_t* bar, uint32_t parity) {  // non-blocking probe
+  uint32_t ok;
+  asm volatile(
+      "{\n"
+      ".reg .pred p;\n"
+      "mbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\n"
+      "selp.u32 %0, 1, 0, p;\n"
+      "}\n"
+      : "=r"(ok)
+      : "r"(smem_u32(bar)), "r"(parity)
+      : "memory");
+  return ok != 0;
+}
+
 // W8: FP8 weights, converted per stage by warps 1-3 exactly as in tc_gemm_body (gemm_wgmma.cuh): the experts' W' tiles (grouped)
 // or the exact q tiles of a dense Linear, whose row scales the epilogue applies (MODE carries EPI_WSCALE).  The partition into
 // (tile, k-block) units is the bf16 kernel's, so an FP8 call splits and sums every tile the same way.
-template <int MODE, int TA, bool GROUPED, bool W8 = false>
+// W4: INT4 dense weights, the packed codes arriving in 16 KB chunks (SkW4Cfg above) and converted to the bf16 W' tile of each stage
+// by warps 1-3 (convert_w4_tile, gscale the group scales); same partition, same k-blocks, same split-tile sums as the bf16 kernel,
+// so the result is the bf16 kernel's on W'.
+template <int MODE, int TA, bool GROUPED, bool W8 = false, bool W4 = false>
 __device__ __forceinline__ void sk_gemm_body(const CUtensorMap& map_a, const CUtensorMap* map_w_base, const SkParams& p, const int32_t* plan,
-                                             const MoeWeightScales* scales = nullptr) {
+                                             const MoeWeightScales* scales = nullptr, const uint16_t* gscale = nullptr) {
   static_assert(!W8 || GROUPED || (MODE & EPI_WSCALE) != 0, "FP8 dense weights: the epilogue applies the row scales");
-  using Cfg = TgCfg<SK_BN, TA, W8>;
+  static_assert(!W4 || (!GROUPED && (MODE & EPI_WSCALE) == 0), "INT4 weights: dense variant, bf16 epilogue");
+  constexpr bool RAW = W8 || W4;
+  using Cfg = std::conditional_t<W4, SkW4Cfg<TA>, TgCfg<SK_BN, TA, W8>>;
   constexpr int STAGES = Cfg::kStages, STAGE_BYTES = Cfg::kStageBytes, A_BYTES = Cfg::kABytes, NCONS = 128 * Cfg::kWG;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint64_t* full = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES + Cfg::kSlack);
+  uint8_t* chunks = smem + STAGES * STAGE_BYTES + Cfg::kSlack;  // W4: the chunk ring
+  uint64_t* full = reinterpret_cast<uint64_t*>(chunks + (W4 ? SK_W4_SLOTS * SK_W4_CHUNK_BYTES : 0));
   uint64_t* empty = full + STAGES;
-  uint64_t* raw = empty + STAGES;  // W8 only
+  uint64_t* raw = empty + STAGES;  // W8: per stage; W4: chunk landed [SLOTS], chunk converted [SLOTS]
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int G = (int)gridDim.x, cta = (int)blockIdx.x;
@@ -84,9 +124,15 @@ __device__ __forceinline__ void sk_gemm_body(const CUtensorMap& map_a, const CUt
 
   if (threadIdx.x == 0) {
     for (int i = 0; i < STAGES; ++i) {
-      mbar_init(&full[i], W8 ? 1 + W8_CONVERTERS : 1);
+      mbar_init(&full[i], RAW ? 1 + W8_CONVERTERS : 1);
       mbar_init(&empty[i], Cfg::kWG);
       if (W8) mbar_init(&raw[i], 1);
+    }
+    if (W4) {
+      for (int i = 0; i < SK_W4_SLOTS; ++i) {
+        mbar_init(&raw[i], 1);
+        mbar_init(&raw[SK_W4_SLOTS + i], W8_CONVERTERS);
+      }
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&map_a) : "memory");
@@ -107,7 +153,42 @@ __device__ __forceinline__ void sk_gemm_body(const CUtensorMap& map_a, const CUt
     // Iteration `it` handles unit u_begin + it.  Weights are never written by any kernel: the W tiles of the first ring are
     // requested BEFORE the programmatic-dependent-launch wait (they stream in while the previous kernel drains); the A tiles of
     // those stages, which the previous kernel produced, follow after it.
-    if (lane == 0) {
+    if (W4 && lane == 0) {
+      const uint32_t n_it = (uint32_t)(u_end - u_begin);
+      uint32_t issued = 0, next_it = 0;  // chunks requested; the first iteration of the next chunk
+      auto issue_chunk = [&]() {
+        const uint32_t u = (uint32_t)u_begin + next_it, slot = issued % SK_W4_SLOTS;
+        const int tile = (int)(u / (uint32_t)num_k), kb = (int)(u % (uint32_t)num_k);
+        mbar_arrive_expect_tx(&raw[slot], SK_W4_CHUNK_BYTES);
+        tma_load_2d(chunks + slot * SK_W4_CHUNK_BYTES, map_w_base, &raw[slot], kb * (TG_BK / 2), tile * SK_BN);
+        next_it += (uint32_t)min(min(SK_W4_CHUNK_KB, num_k - kb), (int)(n_it - next_it));
+        ++issued;
+      };
+      auto chunk_free = [&](bool block) {  // slot of chunk `issued`: converted from its previous chunk
+        uint64_t* bar = &raw[SK_W4_SLOTS + issued % SK_W4_SLOTS];
+        const uint32_t par = ((issued / SK_W4_SLOTS) & 1) ^ 1;
+        if (!block) return mbar_test_wait(bar, par);
+        mbar_wait_quiet(bar, par);
+        return true;
+      };
+      while (issued < (uint32_t)SK_W4_SLOTS && next_it < n_it) issue_chunk();  // weights: before the programmatic-dependent wait
+      pdl_wait();
+      SK_STAMP(1);
+      for (uint32_t it = 0; it < n_it; ++it) {
+        // the chunk holding unit `it` must be requested before this thread blocks on a stage (its slot's previous chunk only needs
+        // units before `it`); later chunks as soon as their slots are free
+        while (next_it <= it) {
+          chunk_free(true);
+          issue_chunk();
+        }
+        while (next_it < n_it && chunk_free(false)) issue_chunk();
+        const uint32_t s = it % STAGES, par = (it / STAGES) & 1;
+        mbar_wait_quiet(&empty[s], par ^ 1);
+        mbar_arrive_expect_tx(&full[s], A_BYTES);
+        tma_load_2d(smem + s * STAGE_BYTES, &map_a, &full[s], (int)(((uint32_t)u_begin + it) % (uint32_t)num_k) * TG_BK, 0);
+      }
+      SK_STAMP(3);
+    } else if (lane == 0) {
       const uint32_t n_it = (uint32_t)(u_end - u_begin);
       auto issue = [&](uint32_t it, bool do_a, bool do_w) {
         const uint32_t u = (uint32_t)u_begin + it;
@@ -117,9 +198,9 @@ __device__ __forceinline__ void sk_gemm_body(const CUtensorMap& map_a, const CUt
         if (do_w) {
           const int n0 = (tile / num_m) * SK_BN;
           const CUtensorMap* wmap = GROUPED ? map_w_base + tile_expert[tile % num_m] : map_w_base;
-          if (W8) {
+          if (RAW) {
             mbar_arrive_expect_tx(&raw[s], Cfg::kRawBytes);
-            tma_load_2d(sa + A_BYTES + Cfg::kBBytes, wmap, &raw[s], kb * TG_BK, n0);
+            tma_load_2d(sa + A_BYTES + Cfg::kBBytes, wmap, &raw[s], kb * (W4 ? TG_BK / 2 : TG_BK), n0);
           } else {
             tma_load_2d(sa + A_BYTES, wmap, &full[s], kb * TG_BK, n0);
           }
@@ -128,7 +209,7 @@ __device__ __forceinline__ void sk_gemm_body(const CUtensorMap& map_a, const CUt
       };
       const uint32_t head = GROUPED ? 0u : (n_it < (uint32_t)STAGES ? n_it : (uint32_t)STAGES);  // (grouped: the tile list itself is the previous kernel's output)
       for (uint32_t it = 0; it < head; ++it) {
-        mbar_arrive_expect_tx(&full[it % STAGES], W8 ? A_BYTES : STAGE_BYTES);  // first lap: every slot is free
+        mbar_arrive_expect_tx(&full[it % STAGES], RAW ? A_BYTES : STAGE_BYTES);  // first lap: every slot is free
         issue(it, false, true);
       }
       pdl_wait();
@@ -137,10 +218,33 @@ __device__ __forceinline__ void sk_gemm_body(const CUtensorMap& map_a, const CUt
       for (uint32_t it = head; it < n_it; ++it) {
         const uint32_t s = it % STAGES, par = (it / STAGES) & 1;
         mbar_wait_quiet(&empty[s], par ^ 1);
-        mbar_arrive_expect_tx(&full[s], W8 ? A_BYTES : STAGE_BYTES);
+        mbar_arrive_expect_tx(&full[s], RAW ? A_BYTES : STAGE_BYTES);
         issue(it, true, true);
       }
       SK_STAMP(3);  // last tile requested
+    }
+  } else if (W4 && warp < 4) {
+    // ================= INT4: the chunks' k-blocks -> the bf16 W' tile of every stage, in the producer's order =================
+    const int ct = (int)threadIdx.x - 32, G = p.K / kInt4Group;
+    const uint32_t n_it = (uint32_t)(u_end - u_begin);
+    uint32_t chunk = 0, slot = 0;
+    int pos = SK_W4_CHUNK_KB;
+    for (uint32_t it = 0; it < n_it; ++it) {
+      const uint32_t u = (uint32_t)u_begin + it;
+      const int tile = (int)(u / (uint32_t)num_k), kb = (int)(u % (uint32_t)num_k);
+      if (kb == 0 || pos == SK_W4_CHUNK_KB || it == 0) {  // the chunk boundaries of the producer's issue_chunk
+        if (it != 0) mbar_arrive(&raw[SK_W4_SLOTS + slot]);
+        slot = chunk % SK_W4_SLOTS;
+        mbar_wait_quiet(&raw[slot], (chunk / SK_W4_SLOTS) & 1);
+        ++chunk;
+        pos = 0;
+      }
+      const uint32_t s = it % STAGES, par = (it / STAGES) & 1;
+      mbar_wait_quiet(&empty[s], par ^ 1);  // the stage's previous W' tile has been read
+      convert_w4_tile<SK_BN, SK_W4_CHUNK_KB * TG_BK / 2>(chunks + slot * SK_W4_CHUNK_BYTES + pos * (TG_BK / 2), smem + s * STAGE_BYTES + A_BYTES,
+                                                         gscale + (int64_t)tile * SK_BN * G + kb / 2, G, ct);
+      mbar_arrive(&full[s]);
+      ++pos;
     }
   } else if (W8 && warp < 4) {
     // ================= FP8: e4m3 -> bf16 W' tile of every stage, in the producer's order =================
@@ -271,6 +375,13 @@ __global__ void __launch_bounds__(TgCfg<SK_BN, TA, true>::kThreads, 1)
 }
 
 template <int MODE, int TA>
+__global__ void __launch_bounds__(TgCfg<SK_BN, TA, false, true>::kThreads, 1)
+    gemm_streamk_int4_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_w, const SkParams p,
+                             const uint16_t* __restrict__ gscale) {
+  sk_gemm_body<MODE, TA, false, false, true>(map_a, &map_w, p, nullptr, nullptr, gscale);
+}
+
+template <int MODE, int TA>
 __global__ void __launch_bounds__(TgCfg<SK_BN, TA, true>::kThreads, 1)
     gemm_streamk_grouped_fp8_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ MoeWeightMaps maps_w,
                                     const __grid_constant__ MoeWeightScales scales, const SkParams p, const int32_t* __restrict__ plan) {
@@ -353,6 +464,43 @@ int launch_streamk_fp8(const GemmParams& g, void* workspace, size_t workspace_by
   if (g.T <= 32) return launch_streamk_fp8_ta<MODE, 32>(g, workspace, workspace_bytes, stream);
   if (g.T <= 64) return launch_streamk_fp8_ta<MODE, 64>(g, workspace, workspace_bytes, stream);
   return launch_streamk_fp8_ta<MODE, 128>(g, workspace, workspace_bytes, stream);
+}
+
+// INT4 dense weights: the bf16 launcher's partition and workspace, a packed code map with chunk-wide boxes and the group scales
+template <int MODE, int TA>
+int launch_streamk_int4_ta(const GemmParams& g, const uint16_t* gscale, void* workspace, size_t workspace_bytes, cudaStream_t stream) {
+  using Cfg = SkW4Cfg<TA>;
+  int dev = 0, sms = 0;
+  MB_CHECK_CUDA(cudaGetDevice(&dev));
+  MB_CHECK_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  if (sms > SK_MAX_CTAS) sms = SK_MAX_CTAS;
+  if (workspace == nullptr || workspace_bytes < kWsSkPartials.end()) return fail(MB200_E_WORKSPACE, "stream-K gemm (int4): workspace %zu < %zu", workspace_bytes, kWsSkPartials.end());
+  CUtensorMap map_a, map_w;
+  int rc = make_tensor_map_2d(&map_a, g.a, g.T, g.K, TA);
+  if (rc) return rc;
+  rc = make_tensor_map_int4(&map_w, g.w, g.N, g.K, SK_BN, SK_W4_CHUNK_KB * TG_BK / 2);
+  if (rc) return rc;
+  SkParams p;
+  p.T = g.T;
+  p.N = g.N;
+  p.K = g.K;
+  p.epi = g.epi;
+  p.partials = reinterpret_cast<float*>((uint8_t*)workspace + kWsSkPartials.offset);
+  p.flags = reinterpret_cast<unsigned*>((uint8_t*)workspace + kWsSkFlags.offset);
+  const long long units = (long long)(g.N / SK_BN) * (g.K / TG_BK);
+  const int grid = (int)(units < sms ? units : sms);
+  MB_CHECK_CUDA(cudaFuncSetAttribute(gemm_streamk_int4_kernel<MODE, TA>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmem));
+  MB_CHECK_CUDA(launch_pdl(gemm_streamk_int4_kernel<MODE, TA>, dim3((unsigned)grid), dim3(Cfg::kThreads), (size_t)Cfg::kSmem, stream, map_a, map_w, p,
+                           gscale));
+  note_launch("gemm_streamk_int4_kernel<%d, %d>", MODE, TA);
+  return MB200_OK;
+}
+
+template <int MODE>
+int launch_streamk_int4(const GemmParams& g, const uint16_t* gscale, void* workspace, size_t workspace_bytes, cudaStream_t stream) {
+  if (g.T <= 32) return launch_streamk_int4_ta<MODE, 32>(g, gscale, workspace, workspace_bytes, stream);
+  if (g.T <= 64) return launch_streamk_int4_ta<MODE, 64>(g, gscale, workspace, workspace_bytes, stream);
+  return launch_streamk_int4_ta<MODE, 128>(g, gscale, workspace, workspace_bytes, stream);
 }
 
 }  // namespace mb200

@@ -21,6 +21,7 @@
 #include "decode_megakernel.cuh"  // mbarrier helpers with the watchdog
 #include "epilogue.cuh"
 #include "gemm_mma.cuh"
+#include "int4.cuh"
 #include "wgmma.cuh"
 
 namespace mb200 {
@@ -36,11 +37,13 @@ constexpr int TG_BM = 128, TG_BN = 256, TG_BK = 64;
 // weight-streaming GEMMs, bound by HBM, with BN chosen by the launcher to give every SM at most one (equal) tile per round.
 // W8 (FP8 expert weights, csrc/moe.cuh): a stage also holds the e4m3 [BN x 64] W tile as TMA delivered it (kRawBytes, unswizzled)
 // next to the bf16 tile the MMAs read, which the producer warpgroup's three idle warps write from it (convert_w8_tile).
-template <int BN, int TA = 128, bool W8 = false>
+// W4 (INT4 dense weights): the same arrangement with the packed [BN x 32-byte] code tile as the raw area (convert_w4_tile).
+template <int BN, int TA = 128, bool W8 = false, bool W4 = false>
 struct TgCfg {
+  static_assert(!(W8 && W4), "one weight format per stage");
   static constexpr int kABytes = TA * TG_BK * 2;
   static constexpr int kBBytes = BN * TG_BK * 2;
-  static constexpr int kRawBytes = W8 ? BN * TG_BK : 0;
+  static constexpr int kRawBytes = W8 ? BN * TG_BK : (W4 ? BN * TG_BK / 2 : 0);
   static constexpr int kStageBytes = kABytes + kBBytes + kRawBytes;
   static constexpr int kWG = TA > 64 ? 2 : 1;  // consumer warpgroups: 64 accumulator rows each
   static constexpr int kThreads = 128 * (1 + kWG);
@@ -51,9 +54,9 @@ struct TgCfg {
   // share of HBM) instead of the whole 227 KB: a successor's CTA, which starts when the predecessor's CTA on its SM exits, has its
   // first ring filled sooner, and other decode kernels' CTAs fit beside it.  W8: an e4m3 stage carries half the HBM bytes of a
   // bf16 one and needs the bf16 tile beside it, so its ring is twice as long to keep the same bytes in flight.
-  static constexpr int kShortRingStages = ((W8 ? 200 : 100) * 1024) / kStageBytes;
+  static constexpr int kShortRingStages = ((W8 || W4 ? 200 : 100) * 1024) / kStageBytes;
   static constexpr int kStages = (TA < 128 || BN < 128) ? (kShortRingStages < 3 ? 3 : (kShortRingStages > kMaxStages ? kMaxStages : kShortRingStages))
-                                                        : W8 ? kMaxStages : (BN == 128 ? 6 : 4);
+                                                        : (W8 || W4) ? kMaxStages : (BN == 128 ? 6 : 4);
   static constexpr int kSmem = kStages * kStageBytes + kSlack + 1024 /*align*/ + 512 /*barriers*/;
   static_assert(kSmem <= 227 * 1024, "shared memory plan exceeds the 227 KB of an sm_90 block");
 };
@@ -133,6 +136,30 @@ __device__ __forceinline__ void convert_w8_tile(const uint8_t* raw, uint8_t* wti
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy stores -> the wgmma (async proxy) reads
 }
 
+// ---- INT4 dense weights: packed code tile -> the bf16 W' tile of the stage -----------------------------------------------------
+// raw = [BN rows x 32 bytes] (64 codes of k-block kb per row, as stored; rows RS bytes apart: 32 for a one-k-block tile, 128 for a
+// k-block inside stream-K's four-k-block chunk), gs = the scale of row 0's group of this k-block, row r's at gs[r * G].  W' comes from int4x8_to_bf16x2 (int4.cuh), so the tile holds exactly the bf16 weights the contract names and the MMAs,
+// descriptors and epilogue are the bf16 kernel's.  Thread ct takes 16-byte code chunks ct, ct + W8_CONVERTERS, ... (32 codes: four
+// swizzled 16-byte bf16 chunks of one row); a quarter warp's stores hit 8 distinct chunk columns of four rows.
+template <int BN, int RS = TG_BK / 2>
+__device__ __forceinline__ void convert_w4_tile(const uint8_t* raw, uint8_t* wtile, const uint16_t* __restrict__ gs, int G, int ct) {
+#pragma unroll 2
+  for (int q = ct; q < BN * 2; q += W8_CONVERTERS) {
+    const int row = q >> 1, c = q & 1;
+    const uint4 v = *reinterpret_cast<const uint4*>(raw + row * RS + c * 16);
+    const uint32_t s2 = (uint32_t)__ldg(gs + (int64_t)row * G) * 0x10001u;
+    const uint32_t in[4] = {v.x, v.y, v.z, v.w};
+    uint8_t* dst = wtile + row * (TG_BK * 2);
+#pragma unroll
+    for (int h = 0; h < 4; ++h) {
+      uint32_t o[4];
+      int4x8_to_bf16x2<true>(in[h], s2, o);
+      *reinterpret_cast<uint4*>(dst + (((4 * c + h) ^ (row & 7)) << 4)) = make_uint4(o[0], o[1], o[2], o[3]);
+    }
+  }
+  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy stores -> the wgmma (async proxy) reads
+}
+
 // One consumer warpgroup's share of a k-block: the 64 tile rows starting at a_addr against the whole [BN x 64] W tile.
 template <int BN>
 __device__ __forceinline__ void wgmma_kblock(float (&acc)[BN / 2], uint32_t a_addr, uint32_t b_addr, bool first) {
@@ -178,19 +205,23 @@ struct MoeWeightScales {  // W8: per-row fp32 scales of each expert's matrix (nu
 // W8 (single CTA only): the producer thread loads the e4m3 W tile into the stage's raw area on raw[s]; warps 1-3 wait on raw[s],
 // write the bf16 tile and arrive on full[s] (W8_CONVERTERS arrivals next to the producer's expect_tx for the A tile).  Grouped:
 // the experts' W' tiles (§3.9); dense: the exact q tiles, the row scales applied by the epilogue (MODE carries EPI_WSCALE).
-template <int MODE, int CL, int BN, int TA, bool GROUPED, bool W8 = false>
+// W4 (dense, single CTA only): the same with the packed INT4 code tile and its group scales gscale (bf16 bits [N, K/128]); the
+// converter warps write W' itself, so the epilogue is the bf16 kernel's.
+template <int MODE, int CL, int BN, int TA, bool GROUPED, bool W8 = false, bool W4 = false>
 __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& map_a, const CUtensorMap* map_w_base, const TcGemmParams& p, const int32_t* plan,
-                                             const MoeWeightScales* scales = nullptr) {
+                                             const MoeWeightScales* scales = nullptr, const uint16_t* gscale = nullptr) {
   static_assert(TA == 128 || CL == 1, "small-batch variant is single-CTA");
   static_assert(!W8 || CL == 1, "FP8 weights: single-CTA variant only");
   static_assert(!W8 || GROUPED || (MODE & EPI_WSCALE) != 0, "FP8 dense weights: the epilogue applies the row scales");
-  using Cfg = TgCfg<BN, TA, W8>;
+  static_assert(!W4 || (CL == 1 && !GROUPED && (MODE & EPI_WSCALE) == 0), "INT4 weights: dense single-CTA variant, bf16 epilogue");
+  constexpr bool RAW = W8 || W4;  // W tiles land in the raw area and are converted by warps 1-3
+  using Cfg = TgCfg<BN, TA, W8, W4>;
   constexpr int STAGES = Cfg::kStages, B_BYTES = Cfg::kBBytes, STAGE_BYTES = Cfg::kStageBytes, A_BYTES = Cfg::kABytes;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);  // SW128 wants 1024-B tiles
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES + Cfg::kSlack);
   uint64_t* empty = full + STAGES;
-  uint64_t* raw = empty + STAGES;  // W8 only
+  uint64_t* raw = empty + STAGES;  // W8 / W4 only
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int rank = CL > 1 ? (int)cluster_ctarank() : 0;
@@ -253,9 +284,9 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& map_a, const CUt
 
   if (threadIdx.x == 0) {
     for (int i = 0; i < STAGES; ++i) {
-      mbar_init(&full[i], W8 ? 1 + W8_CONVERTERS : 1);
+      mbar_init(&full[i], RAW ? 1 + W8_CONVERTERS : 1);
       mbar_init(&empty[i], CL * Cfg::kWG);
-      if (W8) mbar_init(&raw[i], 1);
+      if (RAW) mbar_init(&raw[i], 1);
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&map_a) : "memory");
@@ -280,11 +311,11 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& map_a, const CUt
           const uint32_t s = it % STAGES, par = (it / STAGES) & 1;
           mbar_wait_quiet(&empty[s], par ^ 1);
           uint8_t* sa = smem + s * STAGE_BYTES;
-          if constexpr (W8) {
+          if constexpr (RAW) {
             mbar_arrive_expect_tx(&full[s], A_BYTES);
             tma_load_2d(sa, &map_a, &full[s], kb * TG_BK, m0);
             mbar_arrive_expect_tx(&raw[s], Cfg::kRawBytes);
-            tma_load_2d(sa + A_BYTES + B_BYTES, wmap, &raw[s], kb * TG_BK, n0);
+            tma_load_2d(sa + A_BYTES + B_BYTES, wmap, &raw[s], kb * (W4 ? TG_BK / 2 : TG_BK), n0);
             continue;
           }
           mbar_arrive_expect_tx(&full[s], STAGE_BYTES);  // A + both halves of W (the peer's half may land first: tx-count goes negative)
@@ -297,8 +328,8 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& map_a, const CUt
         }
       }
     }
-  } else if (W8 && warp < 4) {
-    // ================= FP8: e4m3 -> bf16 W' tile of every stage, in the producer's order =================
+  } else if (RAW && warp < 4) {
+    // ================= FP8 / INT4: raw W tile -> bf16 tile of every stage, in the producer's order =================
     const int ct = (int)threadIdx.x - 32;
     uint32_t it = 0;
     for (int tile = cta; tile < num_tiles; tile += n_cta) {
@@ -309,7 +340,12 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& map_a, const CUt
         const uint32_t s = it % STAGES, par = (it / STAGES) & 1;
         mbar_wait_quiet(&raw[s], par);
         uint8_t* sa = smem + s * STAGE_BYTES;
-        convert_w8_tile<BN, !GROUPED>(sa + A_BYTES + B_BYTES, sa + A_BYTES, srows, ct);
+        if constexpr (W4) {
+          const int G = p.K / kInt4Group;
+          convert_w4_tile<BN>(sa + A_BYTES + B_BYTES, sa + A_BYTES, gscale + (int64_t)nt * BN * G + kb / 2, G, ct);
+        } else {
+          convert_w8_tile<BN, !GROUPED>(sa + A_BYTES + B_BYTES, sa + A_BYTES, srows, ct);
+        }
         mbar_arrive(&full[s]);
       }
     }
@@ -374,6 +410,14 @@ __global__ void __launch_bounds__(TgCfg<BN, TA, true>::kThreads, 1)
   tc_gemm_body<MODE, 1, BN, TA, false, true>(map_a, &map_w, p, nullptr);
 }
 
+// INT4 dense weights: map_w is the packed code matrix as uint8 [N, K/2] (box [BN x 32] bytes, no swizzle), gscale its group scales.
+template <int MODE, int BN, int TA>
+__global__ void __launch_bounds__(TgCfg<BN, TA, false, true>::kThreads, 1)
+    gemm_wgmma_int4_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_w, const TcGemmParams p,
+                           const uint16_t* __restrict__ gscale) {
+  tc_gemm_body<MODE, 1, BN, TA, false, false, true>(map_a, &map_w, p, nullptr, nullptr, gscale);
+}
+
 // FP8 expert weights: maps_w are e4m3 [N, K] maps (box [BN x 64] bytes, no swizzle), scales the per-row fp32 scales.
 template <int MODE, int BN, int TA>
 __global__ void __launch_bounds__(TgCfg<BN, TA, true>::kThreads, 1)
@@ -425,6 +469,21 @@ inline int make_tensor_map_e4m3(CUtensorMap* map, const void* base, int64_t rows
   return MB200_OK;
 }
 
+// INT4 codes as uint8 [rows, K/2], box = [box_rows x box_bytes] (32: one k-block of 64 codes; 128: stream-K's chunk of four),
+// unswizzled: the raw tile that convert_w4_tile reads; columns past K/2 read as zero
+inline int make_tensor_map_int4(CUtensorMap* map, const void* base, int64_t rows, int64_t K, int box_rows, int box_bytes = TG_BK / 2) {
+  PFN_encodeTiled enc = get_encode_tiled();
+  if (enc == nullptr) return fail(MB200_E_CUDA, "cuTensorMapEncodeTiled entry point not available");
+  const cuuint64_t dims[2] = {(cuuint64_t)(K / 2), (cuuint64_t)rows};
+  const cuuint64_t strides[1] = {(cuuint64_t)(K / 2)};
+  const cuuint32_t box[2] = {(cuuint32_t)box_bytes, (cuuint32_t)box_rows};
+  const cuuint32_t estr[2] = {1, 1};
+  const CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                         CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) return fail(MB200_E_CUDA, "cuTensorMapEncodeTiled (int4) failed (%d) rows=%lld K=%lld", (int)r, (long long)rows, (long long)K);
+  return MB200_OK;
+}
+
 inline bool wgmma_gemm_eligible(int64_t T, int64_t N, int64_t K) {
   if (K % TG_BK != 0) return false;
   if (T >= TG_BM) return N % 128 == 0 || N % 192 == 0;
@@ -440,6 +499,21 @@ inline bool wgmma_cluster_enabled() {
 inline int wgmma_forced_bn() {
   const char* e = getenv("MB200_GEMM_BN");
   return e != nullptr ? atoi(e) : 0;
+}
+
+// The prefill tile width (T >= 128) for every weight format: the quantised launchers run single CTAs where bf16 runs clusters of
+// two (pair), but take the BN that bf16 takes, so each tile sums the same k-blocks in the same order.  128-wide tiles only when
+// 256-wide ones cannot fill the machine once (small T or N): per flop a narrow tile pulls 1.5x the bytes out of L2.  192-wide
+// tiles are used for N that is a multiple of 192 only (and by the tests).  MB200_GEMM_BN overrides when it divides N.
+inline int wgmma_prefill_bn(int T, int N, bool pair, int sms) {
+  const int units = pair ? sms / 2 : sms, m_units = pair ? ceil_div(ceil_div(T, TG_BM), 2) : ceil_div(T, TG_BM);
+  int bn = 256;
+  if (N % 256 != 0 || (int64_t)m_units * (N / 256) < units) {
+    bn = N % 128 == 0 ? 128 : 192;
+  }
+  const int forced = wgmma_forced_bn();
+  if ((forced == 128 || forced == 192 || forced == 256) && N % forced == 0) bn = forced;
+  return bn;
 }
 
 template <int MODE, int BN>
@@ -547,15 +621,7 @@ int launch_gemm_wgmma(const GemmParams& g, cudaStream_t stream) {
   if (g.T <= 32) return launch_gemm_wgmma_small_ta<MODE, 32>(g, sms, stream);
   if (g.T <= 64) return launch_gemm_wgmma_small_ta<MODE, 64>(g, sms, stream);
   if (g.T < TG_BM) return launch_gemm_wgmma_small_ta<MODE, 128>(g, sms, stream);
-  // 128-wide tiles only when 256-wide ones cannot fill the machine once (small T or N): per flop a narrow tile pulls 1.5x the
-  // bytes out of L2.  192-wide tiles are used for N that is a multiple of 192 only (and by the tests).
-  const int units = pair ? sms / 2 : sms, m_units = pair ? ceil_div(ceil_div(g.T, TG_BM), 2) : ceil_div(g.T, TG_BM);
-  int bn = 256;
-  if (g.N % 256 != 0 || (int64_t)m_units * (g.N / 256) < units) {
-    bn = g.N % 128 == 0 ? 128 : 192;
-  }
-  const int forced = wgmma_forced_bn();
-  if ((forced == 128 || forced == 192 || forced == 256) && g.N % forced == 0) bn = forced;
+  const int bn = wgmma_prefill_bn(g.T, g.N, pair, sms);
   if (bn == 192) return launch_gemm_wgmma_bn<MODE, 192>(g, pair, sms, stream);
   const bool narrow = bn == 128;
   return narrow ? launch_gemm_wgmma_bn<MODE, 128>(g, pair, sms, stream) : launch_gemm_wgmma_bn<MODE, 256>(g, pair, sms, stream);
@@ -604,17 +670,58 @@ int launch_gemm_wgmma_fp8(const GemmParams& g, cudaStream_t stream) {
   if (g.T <= 32) return launch_gemm_wgmma_fp8_small_ta<MODE, 32>(g, sms, stream);
   if (g.T <= 64) return launch_gemm_wgmma_fp8_small_ta<MODE, 64>(g, sms, stream);
   if (g.T < TG_BM) return launch_gemm_wgmma_fp8_small_ta<MODE, 128>(g, sms, stream);
-  // the bf16 launcher's BN rule, with the m units it would have used (clusters of two for T >= 512 unless switched off)
-  const bool pair = wgmma_cluster_enabled() && g.T >= 4 * TG_BM;
-  const int units = pair ? sms / 2 : sms, m_units = pair ? ceil_div(ceil_div(g.T, TG_BM), 2) : ceil_div(g.T, TG_BM);
-  int bn = 256;
-  if (g.N % 256 != 0 || (int64_t)m_units * (g.N / 256) < units) {
-    bn = g.N % 128 == 0 ? 128 : 192;
-  }
-  const int forced = wgmma_forced_bn();
-  if ((forced == 128 || forced == 192 || forced == 256) && g.N % forced == 0) bn = forced;
+  // the bf16 launcher's BN, with the m units it would have used (clusters of two for T >= 512 unless switched off)
+  const int bn = wgmma_prefill_bn(g.T, g.N, wgmma_cluster_enabled() && g.T >= 4 * TG_BM, sms);
   if (bn == 192) return launch_gemm_wgmma_fp8_bn<MODE, 192, TG_BM>(g, sms, stream);
   return bn == 128 ? launch_gemm_wgmma_fp8_bn<MODE, 128, TG_BM>(g, sms, stream) : launch_gemm_wgmma_fp8_bn<MODE, 256, TG_BM>(g, sms, stream);
+}
+
+// ---- INT4 dense weights: the tile choices of launch_gemm_wgmma_fp8 (single CTAs where bf16 runs clusters, same BN) ------------
+// Each tile's k order is the bf16 kernel's and its bf16 tile is W', so from 128 tokens on the result equals the bf16 launcher on W'.
+template <int MODE, int BN, int TA>
+int launch_gemm_wgmma_int4_bn(const GemmParams& g, const uint16_t* gscale, int sms, cudaStream_t stream) {
+  using Cfg = TgCfg<BN, TA, false, true>;
+  CUtensorMap map_a, map_w;
+  int rc = make_tensor_map_2d(&map_a, g.a, g.T, g.K, TA);
+  if (rc) return rc;
+  rc = make_tensor_map_int4(&map_w, g.w, g.N, g.K, BN);
+  if (rc) return rc;
+  TcGemmParams p;
+  p.T = g.T;
+  p.N = g.N;
+  p.K = g.K;
+  p.epi = g.epi;
+  const int tiles = ceil_div(g.T, TG_BM) * (g.N / BN);
+  MB_CHECK_CUDA(cudaFuncSetAttribute(gemm_wgmma_int4_kernel<MODE, BN, TA>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmem));
+  gemm_wgmma_int4_kernel<MODE, BN, TA><<<tiles < sms ? tiles : sms, Cfg::kThreads, Cfg::kSmem, stream>>>(map_a, map_w, p, gscale);
+  note_launch("gemm_wgmma_int4_kernel<%d, %d, %d>", MODE, BN, TA);
+  MB_CHECK_LAUNCH("gemm_wgmma_int4_kernel");
+  return MB200_OK;
+}
+
+template <int MODE, int TA>
+int launch_gemm_wgmma_int4_small_ta(const GemmParams& g, const uint16_t* gscale, int sms, cudaStream_t stream) {
+  switch (wgmma_small_bn(g.N, sms)) {
+    case 256: return launch_gemm_wgmma_int4_bn<MODE, 256, TA>(g, gscale, sms, stream);
+    case 128: return launch_gemm_wgmma_int4_bn<MODE, 128, TA>(g, gscale, sms, stream);
+    case 64: return launch_gemm_wgmma_int4_bn<MODE, 64, TA>(g, gscale, sms, stream);
+    case 32: return launch_gemm_wgmma_int4_bn<MODE, 32, TA>(g, gscale, sms, stream);
+    default: return fail(MB200_E_INVALID, "small-batch GEMM (int4): N=%d is not a multiple of 32", g.N);
+  }
+}
+
+template <int MODE>
+int launch_gemm_wgmma_int4(const GemmParams& g, const uint16_t* gscale, cudaStream_t stream) {
+  int dev = 0, sms = 0;
+  MB_CHECK_CUDA(cudaGetDevice(&dev));
+  MB_CHECK_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  if (g.T <= 32) return launch_gemm_wgmma_int4_small_ta<MODE, 32>(g, gscale, sms, stream);
+  if (g.T <= 64) return launch_gemm_wgmma_int4_small_ta<MODE, 64>(g, gscale, sms, stream);
+  if (g.T < TG_BM) return launch_gemm_wgmma_int4_small_ta<MODE, 128>(g, gscale, sms, stream);
+  const int bn = wgmma_prefill_bn(g.T, g.N, wgmma_cluster_enabled() && g.T >= 4 * TG_BM, sms);
+  if (bn == 192) return launch_gemm_wgmma_int4_bn<MODE, 192, TG_BM>(g, gscale, sms, stream);
+  return bn == 128 ? launch_gemm_wgmma_int4_bn<MODE, 128, TG_BM>(g, gscale, sms, stream)
+                   : launch_gemm_wgmma_int4_bn<MODE, 256, TG_BM>(g, gscale, sms, stream);
 }
 
 }  // namespace mb200

@@ -6,6 +6,7 @@
 // shared memory (optionally RMS-normalised in place by every CTA -- 8..28 KB, cheaper than a kernel boundary).
 #pragma once
 #include "epilogue.cuh"
+#include "int4.cuh"
 
 namespace mb200 {
 
@@ -21,12 +22,20 @@ struct SkinnyParams {
   int N, K;
   float eps;
   EpiParams epi;
+  const uint16_t* gscale = nullptr;  // W4: bf16 group scales [N, K/128]
 };
 
 // W8 (FP8 dense weights, launch_skinny_fp8): p.w is e4m3 [N, K] (K % 16 == 0) and MODE carries EPI_WSCALE (the row
 // scales in p.epi.w_scale).  Same CTA, x staging and row pairs; a 16-byte load is 16 weights (half the bytes of a bf16 load, still
 // 4 in flight per row per lane), each pair converted exactly (e4m3x2_to_float2) and fed to the same fp32 FMAs.
-template <int T, int MODE, bool NORM, bool W8 = false>
+// The staged x plus the kernel's static reduction array red[T][kSkinnyWarps] must fit the block's shared memory: past the default
+// 48 KB the launch needs the opt-in attribute (at T * K = 24576 the dynamic part alone is exactly 48 KB, e.g. Mistral Large's
+// dim 12288 at two tokens).
+inline bool skinny_needs_optin(size_t smem, int T) { return smem + (size_t)T * kSkinnyWarps * sizeof(float) > 48 * 1024; }
+
+// W4 (INT4 dense weights, launch_skinny_int4): p.w is the packed code matrix [N, K/2] (K % 128 == 0), p.gscale its group scales.
+// A 16-byte load is 32 weights of one group; the lane converts them to W' (int4x8_to_bf16x2) and feeds the same fp32 FMAs.
+template <int T, int MODE, bool NORM, bool W8 = false, bool W4 = false>
 __global__ void __launch_bounds__(kSkinnyThreads) skinny_linear_kernel(const SkinnyParams p) {
   extern __shared__ __align__(16) uint8_t smem_raw[];
   uint4* xs = reinterpret_cast<uint4*>(smem_raw);  // [T][K/8] 16-byte chunks
@@ -87,6 +96,64 @@ __global__ void __launch_bounds__(kSkinnyThreads) skinny_linear_kernel(const Ski
   // ---- stream the two rows of this warp ----
   const int n0 = (blockIdx.x * kSkinnyWarps + warp) * kSkinnyRowsPerWarp;
   if (n0 >= p.N) return;
+  if constexpr (W4) {
+    const int kq = p.K >> 5, G = p.K >> 7;  // 16-byte code chunks and scale groups of a row
+    const uint4* w0 = reinterpret_cast<const uint4*>(reinterpret_cast<const uint8_t*>(p.w) + (int64_t)n0 * (p.K >> 1));
+    const uint4* w1 = w0 + kq;
+    const uint16_t* s0 = p.gscale + (int64_t)n0 * G;
+    const uint16_t* s1 = s0 + G;
+    float acc[2][T];
+#pragma unroll
+    for (int t = 0; t < T; ++t) acc[0][t] = acc[1][t] = 0.f;
+
+    // 32 weights of each row (k = 32c ..) against x chunks 4c .. 4c + 3
+    auto fma32 = [&](const uint4& a, const uint4& b, int c) {
+      const uint32_t sa = (uint32_t)__ldg(s0 + (c >> 2)) * 0x10001u, sb = (uint32_t)__ldg(s1 + (c >> 2)) * 0x10001u;
+      const uint32_t aq[4] = {a.x, a.y, a.z, a.w}, bq[4] = {b.x, b.y, b.z, b.w};
+#pragma unroll
+      for (int h = 0; h < 4; ++h) {  // weights 8h .. 8h + 7: aw[i] = (W'[i], W'[i + 4])
+        uint32_t aw[4], bw[4];
+        int4x8_to_bf16x2<false>(aq[h], sa, aw);
+        int4x8_to_bf16x2<false>(bq[h], sb, bw);
+#pragma unroll
+        for (int t = 0; t < T; ++t) {
+          const uint4 xv = xs[t * kc + 4 * c + h];
+          const uint32_t xw[4] = {xv.x, xv.y, xv.z, xv.w};
+#pragma unroll
+          for (int i = 0; i < 4; ++i) {
+            const float xa = (i & 1) ? bf16hi(xw[i >> 1]) : bf16lo(xw[i >> 1]);            // x[i]
+            const float xb = (i & 1) ? bf16hi(xw[2 + (i >> 1)]) : bf16lo(xw[2 + (i >> 1)]);  // x[i + 4]
+            acc[0][t] = fmaf(bf16lo(aw[i]), xa, acc[0][t]);
+            acc[0][t] = fmaf(bf16hi(aw[i]), xb, acc[0][t]);
+            acc[1][t] = fmaf(bf16lo(bw[i]), xa, acc[1][t]);
+            acc[1][t] = fmaf(bf16hi(bw[i]), xb, acc[1][t]);
+          }
+        }
+      }
+    };
+    constexpr int U = T == 4 ? 3 : 4;  // 16-byte loads in flight per row per lane, as in W8
+    int c = lane;
+    for (; c + (U - 1) * 32 < kq; c += U * 32) {
+      uint4 a[U], b[U];
+#pragma unroll
+      for (int u = 0; u < U; ++u) {
+        a[u] = ldg_stream16(w0 + c + u * 32);
+        b[u] = ldg_stream16(w1 + c + u * 32);
+      }
+#pragma unroll
+      for (int u = 0; u < U; ++u) fma32(a[u], b[u], c + u * 32);
+    }
+    for (; c < kq; c += 32) fma32(ldg_stream16(w0 + c), ldg_stream16(w1 + c), c);  // tail
+#pragma unroll
+    for (int t = 0; t < T; ++t) {
+      acc[0][t] = warp_sum(acc[0][t]);
+      acc[1][t] = warp_sum(acc[1][t]);
+    }
+#pragma unroll
+    for (int t = 0; t < T; ++t)
+      if (lane == t) epi_pair<MODE>(p.epi, t, n0, acc[0][t], acc[1][t]);
+    return;
+  }
   if constexpr (W8) {
     const int kq = p.K >> 4;  // e4m3 chunks of a weight row
     const uint4* w0 = reinterpret_cast<const uint4*>(reinterpret_cast<const uint8_t*>(p.w) + (int64_t)n0 * p.K);
@@ -215,7 +282,7 @@ int launch_skinny_fp8(const SkinnyParams& p, int T, cudaStream_t stream) {
   MB_CHECK_ARG(smem <= 200 * 1024, "skinny linear (fp8): T*K too large for shared memory (%zu B)", smem);
   const dim3 grid(ceil_div(p.N, kSkinnyRowsPerCta));
   auto go = [&](auto kernel) -> int {
-    if (smem > 48 * 1024) MB_CHECK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    if (skinny_needs_optin(smem, T)) MB_CHECK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     kernel<<<grid, kSkinnyThreads, smem, stream>>>(p);
     note_launch("skinny_linear_kernel<%d, %d, %s, true>", T, MODE, NORM ? "true" : "false");
     MB_CHECK_LAUNCH("skinny_linear_kernel<fp8>");
@@ -229,6 +296,34 @@ int launch_skinny_fp8(const SkinnyParams& p, int T, cudaStream_t stream) {
   }
 }
 
+// x of up to 4 tokens is staged whole: 224 KB at Mistral Large's w2 (K = 28672), so the bound is the opt-in shared memory of the
+// device less the kernel's static reduction array, not the 200 KB of the bf16 and FP8 launchers.
+template <int MODE, bool NORM>
+int launch_skinny_int4(const SkinnyParams& p, int T, cudaStream_t stream) {
+  MB_CHECK_ARG(T >= 1 && T <= MB200_SKINNY_MAX_T, "skinny linear (int4): T=%d out of range", T);
+  MB_CHECK_ARG(p.K % kInt4Group == 0 && p.N % kSkinnyRowsPerWarp == 0 && p.gscale != nullptr,
+               "skinny linear (int4): K=%d must be a multiple of 128, N=%d even, group scales given", p.K, p.N);
+  int dev = 0, optin = 0;
+  MB_CHECK_CUDA(cudaGetDevice(&dev));
+  MB_CHECK_CUDA(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
+  const size_t smem = (size_t)T * p.K * 2;
+  MB_CHECK_ARG(smem + (size_t)T * kSkinnyWarps * sizeof(float) <= (size_t)optin, "skinny linear (int4): T*K too large for shared memory (%zu B)", smem);
+  const dim3 grid(ceil_div(p.N, kSkinnyRowsPerCta));
+  auto go = [&](auto kernel) -> int {
+    if (skinny_needs_optin(smem, T)) MB_CHECK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    kernel<<<grid, kSkinnyThreads, smem, stream>>>(p);
+    note_launch("skinny_linear_kernel<%d, %d, %s, false, true>", T, MODE, NORM ? "true" : "false");
+    MB_CHECK_LAUNCH("skinny_linear_kernel<int4>");
+    return MB200_OK;
+  };
+  switch (T) {
+    case 1: return go(skinny_linear_kernel<1, MODE, NORM, false, true>);
+    case 2: return go(skinny_linear_kernel<2, MODE, NORM, false, true>);
+    case 3: return go(skinny_linear_kernel<3, MODE, NORM, false, true>);
+    default: return go(skinny_linear_kernel<4, MODE, NORM, false, true>);
+  }
+}
+
 template <int MODE, bool NORM>
 int launch_skinny(const SkinnyParams& p, int T, cudaStream_t stream) {
   MB_CHECK_ARG(T >= 1 && T <= MB200_SKINNY_MAX_T, "skinny linear: T=%d out of range", T);
@@ -237,7 +332,7 @@ int launch_skinny(const SkinnyParams& p, int T, cudaStream_t stream) {
   MB_CHECK_ARG(smem <= 200 * 1024, "skinny linear: T*K too large for shared memory (%zu B)", smem);
   const dim3 grid(ceil_div(p.N, kSkinnyRowsPerCta));
   auto go = [&](auto kernel) -> int {
-    if (smem > 48 * 1024) MB_CHECK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    if (skinny_needs_optin(smem, T)) MB_CHECK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     kernel<<<grid, kSkinnyThreads, smem, stream>>>(p);
     note_launch("skinny_linear_kernel<%d, %d, %s>", T, MODE, NORM ? "true" : "false");
     MB_CHECK_LAUNCH("skinny_linear_kernel");

@@ -57,27 +57,31 @@ class _OutputView:
         return self._m.output_weight
 
 
-DENSE_WEIGHTS = ("bf16", "fp8")
+DENSE_WEIGHTS = ("bf16", "fp8", "int4")
 
 
 def _check_dense_weights(args: TransformerArgs, dense_weights: str) -> None:
-    """The refusals of dense_weights="fp8", before anything is allocated."""
+    """The refusals of dense_weights="fp8" / "int4", before anything is allocated."""
     if dense_weights not in DENSE_WEIGHTS:
         raise ValueError(f"dense_weights={dense_weights!r}: expected one of {DENSE_WEIGHTS}")
-    if dense_weights != "fp8":
+    if dense_weights == "bf16":
         return
+    fmt = dense_weights.upper()
     if args.moe is not None:
-        raise ValueError("dense_weights='fp8' needs a dense model: FP8 attention Linears on mixture-of-experts models are not built "
-                         "(expert_weights='fp8' quantises the experts)")
+        raise ValueError(f"dense_weights={dense_weights!r} needs a dense model: {fmt} attention Linears on mixture-of-experts models are "
+                         "not built (expert_weights='fp8' quantises the experts)")
     if args.lora is not None:
-        raise NotImplementedError("un-merged LoRA on FP8 dense weights is not built (merge the adapter into a bf16 model instead)")
-    # every Linear must stay off the mma.sync GEMM at every token count: it has no e4m3 variant (include/mistral_b200.h)
+        raise NotImplementedError(f"un-merged LoRA on {fmt} dense weights is not built (merge the adapter into a bf16 model instead)")
+    # every Linear must stay off the mma.sync GEMM at every token count: it has no e4m3 or int4 variant (include/mistral_b200.h);
+    # INT4 scale groups are 128 k wide
+    k_mult = 128 if dense_weights == "int4" else 64
     q_dim, kv_dim = args.n_heads * args.head_dim, args.n_kv_heads * args.head_dim
     for name, N, K in (("wqkv", q_dim + 2 * kv_dim, args.dim), ("wo", args.dim, q_dim), ("w13", 2 * args.hidden_dim, args.dim),
                        ("w2", args.dim, args.hidden_dim)):
-        if K % 64 != 0 or (N % 128 != 0 and N % 192 != 0):
-            raise ValueError(f"dense_weights='fp8': {name} [{N}, {K}] would need the mma.sync GEMM, which has no FP8 variant "
-                             "(K must be a multiple of 64 and N of 128 or 192)")
+        if K % k_mult != 0 or (N % 128 != 0 and N % 192 != 0):
+            groups = " or would split a 128-wide scale group" if dense_weights == "int4" else ""
+            raise ValueError(f"dense_weights={dense_weights!r}: {name} [{N}, {K}] would need the mma.sync GEMM, which has no {fmt} variant"
+                             f"{groups} (K must be a multiple of {k_mult} and N of 128 or 192)")
 
 
 class Transformer(nn.Module):
@@ -93,7 +97,9 @@ class Transformer(nn.Module):
         replaced by their dequantised k', v' right after RoPE in every forward that has a cache, see include/mistral_b200.h); and
         `dense_weights`: "bf16", or "fp8" to store wq, wk, wv, wo, w1, w2 and w3 of every text layer of a dense model as e4m3 with
         one fp32 scale per row, applied after the dot product: y = bf16(s * sum_k x * q) (include/mistral_b200.h; the embedding,
-        the lm head, the norms and the vision tower stay bf16).  That model is not bit-identical to any bf16 model."""
+        the lm head, the norms and the vision tower stay bf16).  That model is not bit-identical to any bf16 model.  "int4" stores the
+        same Linears as symmetric 4-bit codes with one bf16 scale per group of 128 k of a row; that model computes exactly what the
+        bf16 model computes with the dequantised weights W' (include/mistral_b200.h)."""
         super().__init__()
         _check_dense_weights(args, dense_weights)
         self.dense_weights = dense_weights
@@ -101,6 +107,9 @@ class Transformer(nn.Module):
             raise ValueError(f"kv_cache={kv_cache!r}: expected one of {KV_CACHE_FORMATS}")
         if kv_cache == "fp8" and args.head_dim != 128:
             raise ValueError(f"kv_cache='fp8' needs head_dim 128: the FP8 attention kernels read 128-byte rows (got {args.head_dim})")
+        if kv_cache == "fp8" and args.n_heads // args.n_kv_heads not in (1, 2, 4, 6, 8):
+            raise ValueError(f"kv_cache='fp8' supports 1, 2, 4, 6 or 8 query heads per kv head (got {args.n_heads // args.n_kv_heads}): "
+                             "the FP8-cache attention kernels hold a group's query heads in MMA rows 0-7")
         self.kv_cache = kv_cache
         if expert_weights not in EXPERT_WEIGHTS:
             raise ValueError(f"expert_weights={expert_weights!r}: expected one of {EXPERT_WEIGHTS}")
@@ -357,11 +366,13 @@ class Transformer(nn.Module):
 
     def _megakernel_ok(self, B: int) -> bool:
         # the megakernel has no LoRA stage and reads bf16 experts and a bf16 KV cache only: with un-merged adapters, FP8 experts or
-        # an FP8 cache batch 1 takes the per-layer graph path (FP8 dense weights have a megakernel of their own: decode_step_fp8)
+        # an FP8 cache batch 1 takes the per-layer graph path (FP8 dense weights have a megakernel of their own: decode_step_fp8;
+        # INT4 dense weights have none and take the graph path)
         # the shape limits (head ratio, K chunking, KV <= 8, MoE sizes, a shared-memory ring of >= 9 stages next to the
         # activations) are the library's, asked once per model: a model it refuses takes the per-layer path
         if not (B == 1 and self.num_pipeline_ranks == 1 and self.expert_parallel[1] == 1 and self.args.lora is None
-                and self.expert_weights == "bf16" and self.kv_cache == "bf16" and os.environ.get("MB200_MEGAKERNEL", "1") != "0"):
+                and self.expert_weights == "bf16" and self.kv_cache == "bf16" and self.dense_weights != "int4"
+                and os.environ.get("MB200_MEGAKERNEL", "1") != "0"):
             return False
         if self._megakernel_refused is None:
             a, moe = self.args, self.args.moe
@@ -621,6 +632,16 @@ class Transformer(nn.Module):
                             raise ValueError(f"Unexpected key {k}")
                         put(mod.weight_e4m3(name), lambda _seg, w, mod=mod, name=name: mod.quantize_(name, w))
                         return True
+        if getattr(att, "int4", False):  # INT4 dense weights: the reference's bf16 weight, quantised into place (the codes are [N, K/2])
+            for mod, names in ((att, ("wq", "wk", "wv", "wo")), (ff, ("w1", "w2", "w3"))):
+                for name in names:
+                    if rest.startswith(f"{'attention' if mod is att else 'feed_forward'}.{name}."):
+                        if rest.rsplit(".", 1)[1] != "weight":
+                            raise ValueError(f"Unexpected key {k}")
+                        q = mod.weight_int4(name)
+                        put(torch.empty(q.shape[0], 2 * q.shape[1], device="meta"),  # the bf16 shape, checked by put
+                            lambda _seg, w, mod=mod, name=name: mod.quantize_int4_(name, w))
+                        return True
         if rest == "attention.wq.weight":
             put(att.wqkv[: att.q_dim])
         elif rest == "attention.wk.weight":
@@ -727,8 +748,10 @@ class Transformer(nn.Module):
         adapters may be absent (they stay zero); the reference's post-hook clears every missing key (lora.py:66-69), this keeps
         the base weights strict."""
         if self.args.lora is None:
-            # an FP8 expert's `X.weight_e4m3` and `X.weight_scale` are both set by the reference's `X.weight`
-            have = set(loaded) | {k[: -len(".weight")] + sfx for k in loaded for sfx in (".weight_e4m3", ".weight_scale")}
+            # an FP8 Linear's `X.weight_e4m3` and `X.weight_scale`, an INT4 one's `X.weight_int4` and `X.weight_gscale`, are set by the
+            # reference's `X.weight`
+            have = set(loaded) | {k[: -len(".weight")] + sfx for k in loaded
+                                  for sfx in (".weight_e4m3", ".weight_scale", ".weight_int4", ".weight_gscale")}
             return set(self.reference_keys()) - have
         have = set(loaded) | {k[: -len(".weight")] + ".linear.weight" for k in loaded}
         return {k for k in self.reference_keys() if k not in have and not k.endswith((".lora_A.weight", ".lora_B.weight"))}
@@ -764,7 +787,8 @@ class Transformer(nn.Module):
     def _block_state(out: Dict[str, torch.Tensor], p: str, blk: TransformerBlock) -> None:
         att = blk.attention
         fp8 = getattr(att, "fp8", False)
-        if not fp8:
+        int4 = getattr(att, "int4", False)
+        if not (fp8 or int4):
             for n in ("wq", "wk", "wv", "wo"):
                 Transformer._linear_state(out, p, blk, "attention." + n, getattr(att, n).weight)
         out[p + "attention_norm.weight"] = blk.attention_norm.weight
@@ -775,6 +799,12 @@ class Transformer(nn.Module):
                 for n in names:
                     out[p + prefix + n + ".weight_e4m3"] = mod.weight_e4m3(n)
                     out[p + prefix + n + ".weight_scale"] = mod.weight_scale(n)
+            return
+        if int4:  # the stored format itself: no dequantised copies
+            for mod, prefix, names in ((att, "attention.", ("wq", "wk", "wv", "wo")), (ff, "feed_forward.", ("w1", "w2", "w3"))):
+                for n in names:
+                    out[p + prefix + n + ".weight_int4"] = mod.weight_int4(n)
+                    out[p + prefix + n + ".weight_gscale"] = mod.weight_gscale(n)
             return
         if hasattr(ff, "experts"):
             out[p + "feed_forward.gate.weight"] = ff.gate_weight
@@ -822,9 +852,9 @@ class Transformer(nn.Module):
         lora_dtype = lora_dtypes.pop()
         assert lora_dtype == self.dtype, f"LoRA weights dtype differs from model's dtype {lora_dtype} != {self.dtype}"
         assert all("lora" in key for key in lora_state_dict.keys())
-        if self.dense_weights == "fp8" and any(key.startswith("layers.") for key in lora_state_dict):
-            raise NotImplementedError("merging a LoRA adapter into FP8 dense weights is not built: the layer Linears are stored quantised "
-                                      "(load the adapter into a bf16 model)")
+        if self.dense_weights != "bf16" and any(key.startswith("layers.") for key in lora_state_dict):
+            raise NotImplementedError(f"merging a LoRA adapter into {self.dense_weights.upper()} dense weights is not built: the layer "
+                                      "Linears are stored quantised (load the adapter into a bf16 model)")
         if self.expert_weights == "fp8" and any(".experts." in key for key in lora_state_dict):
             raise NotImplementedError("merging a LoRA adapter into FP8 expert weights is not built: the experts are stored quantised "
                                       "(load the adapter into a bf16 model, or drop its expert Linears)")
@@ -873,7 +903,7 @@ class Transformer(nn.Module):
         the experts of other ranks are skipped (never read into device memory).  With expert_weights="fp8" each bf16 expert
         tensor is copied to the device and quantised into place: the peak is the FP8 model plus about one bf16 tensor.
         `kv_cache` ("bf16" | "fp8") is the format of the KV cache that generate() builds (see Transformer).  With
-        dense_weights="fp8" every bf16 layer Linear is quantised into place the same way."""
+        dense_weights="fp8" or "int4" every bf16 layer Linear is quantised into place the same way."""
         with open(Path(folder) / "params.json", "r") as f:
             model_args = TransformerArgs.from_dict(json.load(f))
         model_args.max_batch_size = max_batch_size

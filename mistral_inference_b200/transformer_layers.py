@@ -8,6 +8,8 @@ include/mistral_b200.h); weights are stored pre-packed for the fused kernels:
 With `lora` set (un-merged adapters) each fused call also owns a packed LoraAdapter and runs the `_lora` entry points.
 With `fp8` (FP8 dense weights, include/mistral_b200.h) the packed matrices hold e4m3 bytes (uint8, same packing) next to one fp32
 scale per row, and every call runs the `_fp8` entry points.
+With `int4` (INT4 dense weights, include/mistral_b200.h) they hold packed 4-bit codes (uint8 [N, K/2], same row packing) next to one
+bf16 scale per group of 128 k of a row, and every call runs the `_int4` entry points.
 """
 from typing import List, Optional, Tuple
 
@@ -110,6 +112,30 @@ class _Fp8Rows:
         quantize_rows_(name, w, *self._slots(name))
 
 
+class _Int4Rows:
+    """INT4 dense storage of a module's packed matrices: `<m>` is uint8 [N, K/2] (two codes per byte, low nibble = even k), and
+    `<m>_gscale_bits` int16 [N, K/128] the bit patterns of the bf16 group scales (`Module.to(dtype)` casts every floating tensor;
+    these must keep their bits).  The module's `_slots` maps a reference Linear name to its (code rows, scale rows): zero-copy views,
+    strided where rows interleave."""
+
+    def _int4_params(self, name: str, n: int, k: int) -> nn.Parameter:
+        assert k % 128 == 0, f"{name}: K={k} is not a multiple of the 128-wide scale groups"
+        setattr(self, name + "_gscale_bits", nn.Parameter(torch.empty(n, k // 128, dtype=torch.int16), requires_grad=False))
+        return nn.Parameter(torch.empty(n, k // 2, dtype=torch.uint8), requires_grad=False)
+
+    def weight_int4(self, name: str) -> torch.Tensor:
+        return self._slots(name)[0]
+
+    def weight_gscale(self, name: str) -> torch.Tensor:
+        return self._slots(name)[1]
+
+    def quantize_int4_(self, name: str, w: torch.Tensor) -> None:
+        """Quantises the bf16 weight `w` of Linear `name` into place (one bf16 copy of `w` on the device while it runs)."""
+        q, s = self._slots(name)
+        assert tuple(w.shape) == (q.shape[0], 2 * q.shape[1]), f"{name}: shape {tuple(w.shape)} != expected {(q.shape[0], 2 * q.shape[1])}"
+        _abi.quantize_int4_groups(w.to(device=q.device, dtype=torch.bfloat16).contiguous(), q, s)
+
+
 class RMSNorm(nn.Module):
     """transformer_layers.py:109-120."""
 
@@ -122,10 +148,11 @@ class RMSNorm(nn.Module):
         return _abi.rmsnorm(x, self.weight, self.eps)
 
 
-class Attention(nn.Module, _Fp8Rows):
+class Attention(nn.Module, _Fp8Rows, _Int4Rows):
     """transformer_layers.py:31-93."""
 
-    def __init__(self, dim: int, n_heads: int, head_dim: int, n_kv_heads: int, lora: Optional[LoraArgs] = None, fp8: bool = False):
+    def __init__(self, dim: int, n_heads: int, head_dim: int, n_kv_heads: int, lora: Optional[LoraArgs] = None, fp8: bool = False,
+                 int4: bool = False):
         super().__init__()
         self.dim = dim
         self.n_heads = n_heads
@@ -136,9 +163,14 @@ class Attention(nn.Module, _Fp8Rows):
         self.q_dim = n_heads * head_dim
         self.kv_dim = n_kv_heads * head_dim
         self.fp8 = fp8
+        self.int4 = int4
+        assert not (fp8 and int4)
         if fp8:
             self.wqkv = self._fp8_params("wqkv", self.q_dim + 2 * self.kv_dim, dim)
             self.wo_weight = self._fp8_params("wo", dim, self.q_dim)
+        elif int4:
+            self.wqkv = self._int4_params("wqkv", self.q_dim + 2 * self.kv_dim, dim)
+            self.wo_weight = self._int4_params("wo", dim, self.q_dim)
         else:
             self.wqkv = nn.Parameter(torch.empty(self.q_dim + 2 * self.kv_dim, dim), requires_grad=False)
             self.wo_weight = nn.Parameter(torch.empty(dim, self.q_dim), requires_grad=False)
@@ -172,12 +204,21 @@ class Attention(nn.Module, _Fp8Rows):
     def wo_scale(self) -> torch.Tensor:
         return self.wo_scale_bits.view(torch.float32)
 
+    @property
+    def wqkv_gscale(self) -> torch.Tensor:
+        return self.wqkv_gscale_bits.view(torch.bfloat16)
+
+    @property
+    def wo_gscale(self) -> torch.Tensor:
+        return self.wo_gscale_bits.view(torch.bfloat16)
+
     def _slots(self, name: str) -> Tuple[torch.Tensor, torch.Tensor]:
         rows = {"wq": slice(0, self.q_dim), "wk": slice(self.q_dim, self.q_dim + self.kv_dim), "wv": slice(self.q_dim + self.kv_dim, None)}
+        scale, wo_scale = (self.wqkv_gscale, self.wo_gscale) if self.int4 else (self.wqkv_scale, self.wo_scale)
         if name in rows:
-            return self.wqkv[rows[name]], self.wqkv_scale[rows[name]]
+            return self.wqkv[rows[name]], scale[rows[name]]
         if name == "wo":
-            return self.wo_weight, self.wo_scale
+            return self.wo_weight, wo_scale
         raise ValueError(f"attention Linear {name!r}")
 
     def attend(self, x: torch.Tensor, norm_w: torch.Tensor, eps: float, rope: torch.Tensor, positions: torch.Tensor,
@@ -233,6 +274,9 @@ class Attention(nn.Module, _Fp8Rows):
         H, KV, hd = self.n_heads, self.n_kv_heads, self.head_dim
         if self.fp8:
             _abi.attn_qkv_fp8(x, norm_w, self.wqkv, self.wqkv_scale, rope, positions, q, k, v, cache_k, cache_v, cache_rows, H, KV, hd, eps, ws)
+        elif self.int4:
+            _abi.attn_qkv_int4(x, norm_w, self.wqkv, self.wqkv_gscale, rope, positions, q, k, v, cache_k, cache_v, cache_rows, H, KV, hd, eps,
+                               ws)
         elif self.lora is None:
             _abi.attn_qkv(x, norm_w, self.wqkv, rope, positions, q, k, v, cache_k, cache_v, cache_rows, H, KV, hd, eps, ws)
         else:
@@ -243,6 +287,8 @@ class Attention(nn.Module, _Fp8Rows):
         """out = residual + wo(a)."""
         if self.fp8:
             _abi.linear_residual_fp8(a, self.wo_weight, self.wo_scale, residual, out, ws)
+        elif self.int4:
+            _abi.linear_residual_int4(a, self.wo_weight, self.wo_gscale, residual, out, ws)
         elif self.lora is None:
             _abi.linear_residual(a, self.wo_weight, residual, out, ws)
         else:
@@ -257,17 +303,22 @@ def decode_splits(B: int, KV: int, W: int, n_sm: int = 132) -> int:
     return int(max(1, min(s, 64, (W + 63) // 64)))
 
 
-class FeedForward(nn.Module, _Fp8Rows):
+class FeedForward(nn.Module, _Fp8Rows, _Int4Rows):
     """transformer_layers.py:96-106."""
 
-    def __init__(self, dim: int, hidden_dim: int, lora: Optional[LoraArgs] = None, fp8: bool = False):
+    def __init__(self, dim: int, hidden_dim: int, lora: Optional[LoraArgs] = None, fp8: bool = False, int4: bool = False):
         super().__init__()
         self.dim = dim
         self.hidden_dim = hidden_dim
         self.fp8 = fp8
+        self.int4 = int4
+        assert not (fp8 and int4)
         if fp8:
             self.w13 = self._fp8_params("w13", 2 * hidden_dim, dim)
             self.w2_weight = self._fp8_params("w2", dim, hidden_dim)
+        elif int4:
+            self.w13 = self._int4_params("w13", 2 * hidden_dim, dim)
+            self.w2_weight = self._int4_params("w2", dim, hidden_dim)
         else:
             self.w13 = nn.Parameter(torch.empty(2 * hidden_dim, dim), requires_grad=False)
             self.w2_weight = nn.Parameter(torch.empty(dim, hidden_dim), requires_grad=False)
@@ -296,13 +347,23 @@ class FeedForward(nn.Module, _Fp8Rows):
     def w2_scale(self) -> torch.Tensor:
         return self.w2_scale_bits.view(torch.float32)
 
+    @property
+    def w13_gscale(self) -> torch.Tensor:
+        return self.w13_gscale_bits.view(torch.bfloat16)
+
+    @property
+    def w2_gscale(self) -> torch.Tensor:
+        return self.w2_gscale_bits.view(torch.bfloat16)
+
     def _slots(self, name: str) -> Tuple[torch.Tensor, torch.Tensor]:
         h, d = self.hidden_dim, self.dim
         if name in ("w1", "w3"):
             seg = 0 if name == "w1" else 1
+            if self.int4:
+                return self.w13.view(h, 2, d // 2)[:, seg], self.w13_gscale.view(h, 2, d // 128)[:, seg]
             return self.w13.view(h, 2, d)[:, seg], self.w13_scale.view(h, 2)[:, seg]
         if name == "w2":
-            return self.w2_weight, self.w2_scale
+            return (self.w2_weight, self.w2_gscale) if self.int4 else (self.w2_weight, self.w2_scale)
         raise ValueError(f"feed-forward Linear {name!r}")
 
     def run(self, x: torch.Tensor, norm_w: Optional[torch.Tensor], eps: float, residual: Optional[torch.Tensor],
@@ -314,6 +375,9 @@ class FeedForward(nn.Module, _Fp8Rows):
         if self.fp8:
             _abi.ffn_gateup_fp8(x, norm_w, self.w13, self.w13_scale, g, eps, ws)
             _abi.linear_residual_fp8(g, self.w2_weight, self.w2_scale, residual, out, ws)
+        elif self.int4:
+            _abi.ffn_gateup_int4(x, norm_w, self.w13, self.w13_gscale, g, eps, ws)
+            _abi.linear_residual_int4(g, self.w2_weight, self.w2_gscale, residual, out, ws)
         elif self.lora is None:
             _abi.ffn_gateup(x, norm_w, self.w13, g, eps, ws)
             _abi.linear_residual(g, self.w2_weight, residual, out, ws)
@@ -340,9 +404,9 @@ class TransformerBlock(nn.Module):
         self.n_heads = n_heads
         self.dim = dim
         self.norm_eps = norm_eps
-        fp8 = dense_weights == "fp8"
-        assert not fp8 or (moe is None and lora is None), "FP8 dense weights: dense layers without un-merged LoRA only"
-        self.attention = Attention(dim=dim, n_heads=n_heads, head_dim=head_dim, n_kv_heads=n_kv_heads, lora=lora, fp8=fp8)
+        fp8, int4 = dense_weights == "fp8", dense_weights == "int4"
+        assert not (fp8 or int4) or (moe is None and lora is None), "quantised dense weights: dense layers without un-merged LoRA only"
+        self.attention = Attention(dim=dim, n_heads=n_heads, head_dim=head_dim, n_kv_heads=n_kv_heads, lora=lora, fp8=fp8, int4=int4)
         self.attention_norm = RMSNorm(dim, eps=norm_eps)
         self.ffn_norm = RMSNorm(dim, eps=norm_eps)
         self.feed_forward: nn.Module
@@ -353,7 +417,7 @@ class TransformerBlock(nn.Module):
                                          gate_weight=nn.Parameter(torch.empty(moe.num_experts, dim), requires_grad=False), moe_args=moe,
                                          expert_shard=expert_shard, expert_group=expert_group)
         else:
-            self.feed_forward = FeedForward(dim=dim, hidden_dim=hidden_dim, lora=lora, fp8=fp8)
+            self.feed_forward = FeedForward(dim=dim, hidden_dim=hidden_dim, lora=lora, fp8=fp8, int4=int4)
 
     def forward(self, x: torch.Tensor, rope: torch.Tensor, positions: torch.Tensor, cache: Optional[CacheView],
                 ws: "_abi.Workspace") -> torch.Tensor:

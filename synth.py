@@ -191,6 +191,9 @@ SHAPES: Dict[str, dict] = {
                          norm_eps=1e-5, vocab_size=32000, moe=dict(num_experts=8, num_experts_per_tok=2)),
     "mixtral-8x22b": dict(dim=6144, n_layers=56, head_dim=128, hidden_dim=16384, n_heads=48, n_kv_heads=8,
                           norm_eps=1e-5, vocab_size=32768, moe=dict(num_experts=8, num_experts_per_tok=2)),
+    # Mistral Large 2 (123B; also the text model of Pixtral Large): 96 query heads over 8 kv heads (H/KV = 12)
+    "mistral-large-2": dict(dim=12288, n_layers=88, head_dim=128, hidden_dim=28672, n_heads=96, n_kv_heads=8,
+                            norm_eps=1e-5, vocab_size=32768, rope_theta=1000000.0),
     # shapes small enough for the CPU oracle / golden fixtures (head_dim stays 128 like every real config)
     "tiny": dict(dim=256, n_layers=2, head_dim=128, hidden_dim=512, n_heads=4, n_kv_heads=2,
                  norm_eps=1e-5, vocab_size=512),
