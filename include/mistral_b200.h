@@ -328,6 +328,20 @@ int mb200_moe_grouped_ffn_fp8(const void* xs, const void* const* w13_host, const
                               const void* residual, void* g, void* yw, void* out, int64_t T, int64_t dim, int64_t hidden, int64_t n_experts,
                               int64_t top_k, const mb200_moe_comm* comm, void* workspace, size_t workspace_bytes, void* stream);
 
+/* INT4 expert weights: the INT4 format of the dense Linears (see mb200_quantize_int4_groups below) applied to every expert matrix;
+ * each expert's w1 / w3 fill the interleaved w13 rows (row 2i = w1[i], row 2i + 1 = w3[i]) through the quantiser's row strides.
+ * mb200_moe_grouped_ffn_int4: mb200_moe_grouped_ffn with INT4 experts: w13_host / w2_host are HOST arrays of E device pointers to
+ *     the codes (uint8 [2*hidden, dim/2] and [dim, hidden/2], 16-byte aligned), w13_gscale_host / w2_gscale_host HOST arrays of E
+ *     device pointers to their bf16 group scales ([2*hidden, dim/128] and [dim, hidden/128]); NULL for experts of other ranks.
+ *     dim and hidden must be multiples of 128 (else MB200_E_INVALID).  The grouped GEMMs form W' in shared memory; tile rows, tile
+ *     width and the stream-K partition are those of mb200_moe_grouped_ffn for the same plan, except that 128-row calls never run as
+ *     2-CTA clusters.  Every tile sums the same W' tiles in the same k order as the bf16 call, so the result equals
+ *     mb200_moe_grouped_ffn on W' bit for bit at every T. */
+int mb200_moe_grouped_ffn_int4(const void* xs, const void* const* w13_host, const void* const* w13_gscale_host, const void* const* w2_host,
+                               const void* const* w2_gscale_host, const int32_t* plan, const void* row_w, const int32_t* slot,
+                               const void* residual, void* g, void* yw, void* out, int64_t T, int64_t dim, int64_t hidden, int64_t n_experts,
+                               int64_t top_k, const mb200_moe_comm* comm, void* workspace, size_t workspace_bytes, void* stream);
+
 /* Buffers that other ranks (one process per GPU) can write: plain cudaMalloc + CUDA IPC.  alloc zero-fills and synchronises;
  * export writes the 64-byte IPC handle to pass to the other processes (e.g. torch.distributed.all_gather_object); open maps a
  * peer's buffer into this process (peer access over NVLink is enabled lazily).  These are the only entry points that allocate. */

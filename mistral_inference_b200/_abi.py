@@ -64,6 +64,8 @@ _SIGNATURES = {
     "mb200_quantize_e4m3_rows": (c_int, [c_void_p, c_int64, c_int64, c_void_p, c_int64, c_void_p, c_int64, c_void_p]),
     "mb200_moe_grouped_ffn_fp8": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                           c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int64, c_int64, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "mb200_moe_grouped_ffn_int4": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                           c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int64, c_int64, c_void_p, c_void_p, c_size_t, c_void_p]),
     "mb200_comm_alloc": (c_int, [c_size_t, ctypes.POINTER(c_void_p)]),
     "mb200_comm_free": (c_int, [c_void_p]),
     "mb200_comm_export": (c_int, [c_void_p, c_void_p]),
@@ -486,6 +488,16 @@ def moe_grouped_ffn_fp8(b, w13_host, s13_host, w2_host, s2_host, residual: Optio
                                            _ptr(b.slot), _ptr(residual), _ptr(b.g), b.yw_ptr, _ptr(out), T, dim, hidden, E, k,
                                            ctypes.cast(ctypes.pointer(comm), c_void_p) if comm is not None else None, ws.ptr, ws.nbytes,
                                            _stream()), "mb200_moe_grouped_ffn_fp8")
+
+
+def moe_grouped_ffn_int4(b, w13_host, s13_host, w2_host, s2_host, residual: Optional[torch.Tensor], out: torch.Tensor, T: int, dim: int,
+                         hidden: int, E: int, k: int, comm: Optional[MoeCommStruct], ws: "Workspace") -> None:
+    """moe_grouped_ffn with INT4 experts: host arrays of E device pointers to the packed codes and to their bf16 group scales."""
+    _check(lib().mb200_moe_grouped_ffn_int4(_ptr(b.xs), ctypes.cast(w13_host, c_void_p), ctypes.cast(s13_host, c_void_p),
+                                            ctypes.cast(w2_host, c_void_p), ctypes.cast(s2_host, c_void_p), _ptr(b.plan), _ptr(b.row_w),
+                                            _ptr(b.slot), _ptr(residual), _ptr(b.g), b.yw_ptr, _ptr(out), T, dim, hidden, E, k,
+                                            ctypes.cast(ctypes.pointer(comm), c_void_p) if comm is not None else None, ws.ptr, ws.nbytes,
+                                            _stream()), "mb200_moe_grouped_ffn_int4")
 
 
 def quantize_e4m3_rows(w: torch.Tensor, q: torch.Tensor, scale: torch.Tensor) -> None:

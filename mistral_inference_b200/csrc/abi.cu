@@ -803,15 +803,18 @@ int mb200_moe_route(const void* hn, const void* gate_w, int64_t T, int64_t dim, 
   return MB200_OK;
 }
 
-// s13 / s2: NULL for bf16 experts; for FP8 ones the host arrays of per-row fp32 scale pointers next to the e4m3 weights
-static int moe_grouped_ffn(const void* xs, const void* const* w13_host, const void* const* w2_host, const float* const* s13_host,
-                           const float* const* s2_host, const int32_t* plan, const void* row_w, const int32_t* slot, const void* residual, void* g,
+// s13 / s2: NULL for bf16 experts; the host arrays of per-row fp32 scale pointers next to e4m3 weights (FP8), or of bf16 group-scale
+// pointers next to INT4 codes
+static int moe_grouped_ffn(const void* xs, const void* const* w13_host, const void* const* w2_host, MoeFmt fmt, const void* const* s13_host,
+                           const void* const* s2_host, const int32_t* plan, const void* row_w, const int32_t* slot, const void* residual, void* g,
                            void* yw, void* out, int64_t T, int64_t dim, int64_t hidden, int64_t n_experts, int64_t top_k, const mb200_moe_comm* comm,
                            void* workspace, size_t workspace_bytes, void* stream) {
   MB_CHECK_ARG(xs && w13_host && w2_host && plan && row_w && slot && g && yw && out, "moe_grouped_ffn: null pointer");
   MB_CHECK_ARG(T >= 1 && top_k >= 1 && top_k <= MOE_MAX_TOPK && n_experts <= MOE_MAX_EXPERTS && dim % 64 == 0 && hidden % 64 == 0,
                "moe_grouped_ffn: T=%lld k=%lld E=%lld dim=%lld hidden=%lld", (long long)T, (long long)top_k, (long long)n_experts, (long long)dim,
                (long long)hidden);
+  MB_CHECK_ARG(fmt != MoeFmt::INT4 || (dim % kInt4Group == 0 && hidden % kInt4Group == 0),
+               "moe_grouped_ffn (int4): dim=%lld and hidden=%lld must be multiples of 128", (long long)dim, (long long)hidden);
   const int n_ranks = comm ? comm->n_ranks : 1, my_rank = comm ? comm->my_rank : 0;
   MB_CHECK_ARG(n_ranks >= 1 && n_ranks <= kMaxPeers && my_rank >= 0 && my_rank < n_ranks, "moe_grouped_ffn: rank %d of %d", my_rank, n_ranks);
   cudaStream_t st = (cudaStream_t)stream;
@@ -829,7 +832,7 @@ static int moe_grouped_ffn(const void* xs, const void* const* w13_host, const vo
   e1.out = g;
   e1.ld_out = hidden;
   int rc = launch_grouped<EPI_SWIGLU>(xs, rows_cap, dim, 2 * hidden, w13_host, (int)n_experts, est, tile_rows, plan, e1, workspace, workspace_bytes, st,
-                                      s13_host);
+                                      fmt, s13_host);
   if (rc) return rc;
   EpiParams e2;
   e2.out = yw;
@@ -841,7 +844,7 @@ static int moe_grouped_ffn(const void* xs, const void* const* w13_host, const vo
     e2.peer_out[r] = comm->peer_yw[r];
   }
   rc = launch_grouped<EPI_MOE_SCALE>(g, rows_cap, hidden, dim, w2_host, (int)n_experts, est, tile_rows, plan, e2, workspace, workspace_bytes, st,
-                                     s2_host);
+                                     fmt, s2_host);
   if (rc) return rc;
   MoeCombineParams c;
   c.yw = (const uint4*)yw;
@@ -876,7 +879,7 @@ static int moe_grouped_ffn(const void* xs, const void* const* w13_host, const vo
 int mb200_moe_grouped_ffn(const void* xs, const void* const* w13_host, const void* const* w2_host, const int32_t* plan, const void* row_w,
                           const int32_t* slot, const void* residual, void* g, void* yw, void* out, int64_t T, int64_t dim, int64_t hidden,
                           int64_t n_experts, int64_t top_k, const mb200_moe_comm* comm, void* workspace, size_t workspace_bytes, void* stream) {
-  return moe_grouped_ffn(xs, w13_host, w2_host, nullptr, nullptr, plan, row_w, slot, residual, g, yw, out, T, dim, hidden, n_experts, top_k, comm,
+  return moe_grouped_ffn(xs, w13_host, w2_host, MoeFmt::BF16, nullptr, nullptr, plan, row_w, slot, residual, g, yw, out, T, dim, hidden, n_experts, top_k, comm,
                          workspace, workspace_bytes, stream);
 }
 
@@ -885,8 +888,18 @@ int mb200_moe_grouped_ffn_fp8(const void* xs, const void* const* w13_host, const
                               void* g, void* yw, void* out, int64_t T, int64_t dim, int64_t hidden, int64_t n_experts, int64_t top_k,
                               const mb200_moe_comm* comm, void* workspace, size_t workspace_bytes, void* stream) {
   MB_CHECK_ARG(w13_scale_host && w2_scale_host, "moe_grouped_ffn_fp8: null scale table");
-  return moe_grouped_ffn(xs, w13_host, w2_host, w13_scale_host, w2_scale_host, plan, row_w, slot, residual, g, yw, out, T, dim, hidden, n_experts,
+  return moe_grouped_ffn(xs, w13_host, w2_host, MoeFmt::FP8, reinterpret_cast<const void* const*>(w13_scale_host),
+                         reinterpret_cast<const void* const*>(w2_scale_host), plan, row_w, slot, residual, g, yw, out, T, dim, hidden, n_experts,
                          top_k, comm, workspace, workspace_bytes, stream);
+}
+
+int mb200_moe_grouped_ffn_int4(const void* xs, const void* const* w13_host, const void* const* w13_gscale_host, const void* const* w2_host,
+                               const void* const* w2_gscale_host, const int32_t* plan, const void* row_w, const int32_t* slot, const void* residual,
+                               void* g, void* yw, void* out, int64_t T, int64_t dim, int64_t hidden, int64_t n_experts, int64_t top_k,
+                               const mb200_moe_comm* comm, void* workspace, size_t workspace_bytes, void* stream) {
+  MB_CHECK_ARG(w13_gscale_host && w2_gscale_host, "moe_grouped_ffn_int4: null scale table");
+  return moe_grouped_ffn(xs, w13_host, w2_host, MoeFmt::INT4, w13_gscale_host, w2_gscale_host, plan, row_w, slot, residual, g, yw, out, T, dim,
+                         hidden, n_experts, top_k, comm, workspace, workspace_bytes, stream);
 }
 
 int mb200_quantize_e4m3_rows(const void* w, int64_t rows, int64_t K, void* q, int64_t q_row_stride, float* scale, int64_t scale_stride, void* stream) {

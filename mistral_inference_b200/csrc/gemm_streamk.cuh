@@ -92,14 +92,16 @@ __device__ __forceinline__ bool mbar_test_wait(uint64_t* bar, uint32_t parity) {
 // W8: FP8 weights, converted per stage by warps 1-3 exactly as in tc_gemm_body (gemm_wgmma.cuh): the experts' W' tiles (grouped)
 // or the exact q tiles of a dense Linear, whose row scales the epilogue applies (MODE carries EPI_WSCALE).  The partition into
 // (tile, k-block) units is the bf16 kernel's, so an FP8 call splits and sums every tile the same way.
-// W4: INT4 dense weights, the packed codes arriving in 16 KB chunks (SkW4Cfg above) and converted to the bf16 W' tile of each stage
-// by warps 1-3 (convert_w4_tile, gscale the group scales); same partition, same k-blocks, same split-tile sums as the bf16 kernel,
-// so the result is the bf16 kernel's on W'.
+// W4: INT4 weights, the packed codes arriving in 16 KB chunks (SkW4Cfg above) and converted to the bf16 W' tile of each stage
+// by warps 1-3 (convert_w4_tile; group scales gscale when dense, gscales->s[expert] of the tile's expert when grouped); same
+// partition, same k-blocks, same split-tile sums as the bf16 kernel, so the result is the bf16 kernel's on W'.  A chunk never
+// crosses a tile, so each chunk belongs to one expert.
 template <int MODE, int TA, bool GROUPED, bool W8 = false, bool W4 = false>
 __device__ __forceinline__ void sk_gemm_body(const CUtensorMap& map_a, const CUtensorMap* map_w_base, const SkParams& p, const int32_t* plan,
-                                             const MoeWeightScales* scales = nullptr, const uint16_t* gscale = nullptr) {
+                                             const MoeWeightScales* scales = nullptr, const uint16_t* gscale = nullptr,
+                                             const MoeWeightGroupScales* gscales = nullptr) {
   static_assert(!W8 || GROUPED || (MODE & EPI_WSCALE) != 0, "FP8 dense weights: the epilogue applies the row scales");
-  static_assert(!W4 || (!GROUPED && (MODE & EPI_WSCALE) == 0), "INT4 weights: dense variant, bf16 epilogue");
+  static_assert(!W4 || (MODE & EPI_WSCALE) == 0, "INT4 weights: bf16 epilogue");
   constexpr bool RAW = W8 || W4;
   using Cfg = std::conditional_t<W4, SkW4Cfg<TA>, TgCfg<SK_BN, TA, W8>>;
   constexpr int STAGES = Cfg::kStages, STAGE_BYTES = Cfg::kStageBytes, A_BYTES = Cfg::kABytes, NCONS = 128 * Cfg::kWG;
@@ -152,7 +154,8 @@ __device__ __forceinline__ void sk_gemm_body(const CUtensorMap& map_a, const CUt
     // ================= TMA producer =================
     // Iteration `it` handles unit u_begin + it.  Weights are never written by any kernel: the W tiles of the first ring are
     // requested BEFORE the programmatic-dependent-launch wait (they stream in while the previous kernel drains); the A tiles of
-    // those stages, which the previous kernel produced, follow after it.
+    // those stages, which the previous kernel produced, follow after it.  Grouped: the tile list (and with it every weight
+    // address) is the previous kernel's output, so nothing is requested before the wait at the top of the body.
     if (W4 && lane == 0) {
       const uint32_t n_it = (uint32_t)(u_end - u_begin);
       uint32_t issued = 0, next_it = 0;  // chunks requested; the first iteration of the next chunk
@@ -160,7 +163,11 @@ __device__ __forceinline__ void sk_gemm_body(const CUtensorMap& map_a, const CUt
         const uint32_t u = (uint32_t)u_begin + next_it, slot = issued % SK_W4_SLOTS;
         const int tile = (int)(u / (uint32_t)num_k), kb = (int)(u % (uint32_t)num_k);
         mbar_arrive_expect_tx(&raw[slot], SK_W4_CHUNK_BYTES);
-        tma_load_2d(chunks + slot * SK_W4_CHUNK_BYTES, map_w_base, &raw[slot], kb * (TG_BK / 2), tile * SK_BN);
+        if constexpr (GROUPED)
+          tma_load_2d(chunks + slot * SK_W4_CHUNK_BYTES, map_w_base + tile_expert[tile % num_m], &raw[slot], kb * (TG_BK / 2),
+                      (tile / num_m) * SK_BN);
+        else
+          tma_load_2d(chunks + slot * SK_W4_CHUNK_BYTES, map_w_base, &raw[slot], kb * (TG_BK / 2), tile * SK_BN);
         next_it += (uint32_t)min(min(SK_W4_CHUNK_KB, num_k - kb), (int)(n_it - next_it));
         ++issued;
       };
@@ -185,7 +192,9 @@ __device__ __forceinline__ void sk_gemm_body(const CUtensorMap& map_a, const CUt
         const uint32_t s = it % STAGES, par = (it / STAGES) & 1;
         mbar_wait_quiet(&empty[s], par ^ 1);
         mbar_arrive_expect_tx(&full[s], A_BYTES);
-        tma_load_2d(smem + s * STAGE_BYTES, &map_a, &full[s], (int)(((uint32_t)u_begin + it) % (uint32_t)num_k) * TG_BK, 0);
+        const uint32_t u = (uint32_t)u_begin + it;
+        tma_load_2d(smem + s * STAGE_BYTES, &map_a, &full[s], (int)(u % (uint32_t)num_k) * TG_BK,
+                    GROUPED ? tile_row0[(u / (uint32_t)num_k) % (uint32_t)num_m] : 0);
       }
       SK_STAMP(3);
     } else if (lane == 0) {
@@ -241,8 +250,9 @@ __device__ __forceinline__ void sk_gemm_body(const CUtensorMap& map_a, const CUt
       }
       const uint32_t s = it % STAGES, par = (it / STAGES) & 1;
       mbar_wait_quiet(&empty[s], par ^ 1);  // the stage's previous W' tile has been read
+      const uint16_t* gs = GROUPED ? gscales->s[tile_expert[tile % num_m]] + (int64_t)(tile / num_m) * SK_BN * G : gscale + (int64_t)tile * SK_BN * G;
       convert_w4_tile<SK_BN, SK_W4_CHUNK_KB * TG_BK / 2>(chunks + slot * SK_W4_CHUNK_BYTES + pos * (TG_BK / 2), smem + s * STAGE_BYTES + A_BYTES,
-                                                         gscale + (int64_t)tile * SK_BN * G + kb / 2, G, ct);
+                                                         gs + kb / 2, G, ct);
       mbar_arrive(&full[s]);
       ++pos;
     }
@@ -386,6 +396,15 @@ __global__ void __launch_bounds__(TgCfg<SK_BN, TA, true>::kThreads, 1)
     gemm_streamk_grouped_fp8_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ MoeWeightMaps maps_w,
                                     const __grid_constant__ MoeWeightScales scales, const SkParams p, const int32_t* __restrict__ plan) {
   sk_gemm_body<MODE, TA, true, true>(map_a, maps_w.m, p, plan, &scales);
+}
+
+// INT4 expert weights: maps_w are the experts' code matrices as uint8 [N, K/2] (box [128 x 128] bytes: one chunk), gscales their
+// bf16 group scales [N, K/128].
+template <int MODE, int TA>
+__global__ void __launch_bounds__(TgCfg<SK_BN, TA, false, true>::kThreads, 1)
+    gemm_streamk_grouped_int4_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ MoeWeightMaps maps_w,
+                                     const __grid_constant__ MoeWeightGroupScales gscales, const SkParams p, const int32_t* __restrict__ plan) {
+  sk_gemm_body<MODE, TA, true, false, true>(map_a, maps_w.m, p, plan, nullptr, nullptr, &gscales);
 }
 
 inline bool streamk_eligible(int64_t T, int64_t N, int64_t K) {

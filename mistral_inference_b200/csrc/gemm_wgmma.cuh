@@ -37,7 +37,7 @@ constexpr int TG_BM = 128, TG_BN = 256, TG_BK = 64;
 // weight-streaming GEMMs, bound by HBM, with BN chosen by the launcher to give every SM at most one (equal) tile per round.
 // W8 (FP8 expert weights, csrc/moe.cuh): a stage also holds the e4m3 [BN x 64] W tile as TMA delivered it (kRawBytes, unswizzled)
 // next to the bf16 tile the MMAs read, which the producer warpgroup's three idle warps write from it (convert_w8_tile).
-// W4 (INT4 dense weights): the same arrangement with the packed [BN x 32-byte] code tile as the raw area (convert_w4_tile).
+// W4 (INT4 dense and expert weights): the same arrangement with the packed [BN x 32-byte] code tile as the raw area (convert_w4_tile).
 template <int BN, int TA = 128, bool W8 = false, bool W4 = false>
 struct TgCfg {
   static_assert(!(W8 && W4), "one weight format per stage");
@@ -201,19 +201,23 @@ struct MoeWeightMaps {
 struct MoeWeightScales {  // W8: per-row fp32 scales of each expert's matrix (null for experts of other ranks)
   const float* s[MOE_MAX_EXPERTS];
 };
+struct MoeWeightGroupScales {  // W4: bf16 group scales [N, K/128] of each expert's code matrix (null for experts of other ranks)
+  const uint16_t* s[MOE_MAX_EXPERTS];
+};
 
 // W8 (single CTA only): the producer thread loads the e4m3 W tile into the stage's raw area on raw[s]; warps 1-3 wait on raw[s],
 // write the bf16 tile and arrive on full[s] (W8_CONVERTERS arrivals next to the producer's expect_tx for the A tile).  Grouped:
 // the experts' W' tiles (§3.9); dense: the exact q tiles, the row scales applied by the epilogue (MODE carries EPI_WSCALE).
-// W4 (dense, single CTA only): the same with the packed INT4 code tile and its group scales gscale (bf16 bits [N, K/128]); the
-// converter warps write W' itself, so the epilogue is the bf16 kernel's.
+// W4 (single CTA only): the same with the packed INT4 code tile and its group scales (bf16 bits [N, K/128]: gscale when dense,
+// gscales->s[expert] of the tile's expert when grouped); the converter warps write W' itself, so the epilogue is the bf16 kernel's.
 template <int MODE, int CL, int BN, int TA, bool GROUPED, bool W8 = false, bool W4 = false>
 __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& map_a, const CUtensorMap* map_w_base, const TcGemmParams& p, const int32_t* plan,
-                                             const MoeWeightScales* scales = nullptr, const uint16_t* gscale = nullptr) {
+                                             const MoeWeightScales* scales = nullptr, const uint16_t* gscale = nullptr,
+                                             const MoeWeightGroupScales* gscales = nullptr) {
   static_assert(TA == 128 || CL == 1, "small-batch variant is single-CTA");
   static_assert(!W8 || CL == 1, "FP8 weights: single-CTA variant only");
   static_assert(!W8 || GROUPED || (MODE & EPI_WSCALE) != 0, "FP8 dense weights: the epilogue applies the row scales");
-  static_assert(!W4 || (CL == 1 && !GROUPED && (MODE & EPI_WSCALE) == 0), "INT4 weights: dense single-CTA variant, bf16 epilogue");
+  static_assert(!W4 || (CL == 1 && (MODE & EPI_WSCALE) == 0), "INT4 weights: single-CTA variant, bf16 epilogue");
   constexpr bool RAW = W8 || W4;  // W tiles land in the raw area and are converted by warps 1-3
   using Cfg = TgCfg<BN, TA, W8, W4>;
   constexpr int STAGES = Cfg::kStages, B_BYTES = Cfg::kBBytes, STAGE_BYTES = Cfg::kStageBytes, A_BYTES = Cfg::kABytes;
@@ -335,12 +339,15 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& map_a, const CUt
     for (int tile = cta; tile < num_tiles; tile += n_cta) {
       int mu, nt;
       tile_mn(tile, mu, nt);
-      const float* srows = GROUPED ? scales->s[tile_expert[mu]] + nt * BN : nullptr;
+      const float* srows = GROUPED && W8 ? scales->s[tile_expert[mu]] + nt * BN : nullptr;
       for (int kb = 0; kb < num_k; ++kb, ++it) {
         const uint32_t s = it % STAGES, par = (it / STAGES) & 1;
         mbar_wait_quiet(&raw[s], par);
         uint8_t* sa = smem + s * STAGE_BYTES;
-        if constexpr (W4) {
+        if constexpr (W4 && GROUPED) {
+          const int G = p.K / kInt4Group;
+          convert_w4_tile<BN>(sa + A_BYTES + B_BYTES, sa + A_BYTES, gscales->s[tile_expert[mu]] + (int64_t)nt * BN * G + kb / 2, G, ct);
+        } else if constexpr (W4) {
           const int G = p.K / kInt4Group;
           convert_w4_tile<BN>(sa + A_BYTES + B_BYTES, sa + A_BYTES, gscale + (int64_t)nt * BN * G + kb / 2, G, ct);
         } else {
@@ -424,6 +431,15 @@ __global__ void __launch_bounds__(TgCfg<BN, TA, true>::kThreads, 1)
     gemm_wgmma_grouped_fp8_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ MoeWeightMaps maps_w,
                                   const __grid_constant__ MoeWeightScales scales, const TcGemmParams p, const int32_t* __restrict__ plan) {
   tc_gemm_body<MODE, 1, BN, TA, true, true>(map_a, maps_w.m, p, plan, &scales);
+}
+
+// INT4 expert weights: maps_w are the experts' packed code matrices as uint8 [N, K/2] (box [BN x 32] bytes, no swizzle), gscales
+// their bf16 group scales [N, K/128].
+template <int MODE, int BN, int TA>
+__global__ void __launch_bounds__(TgCfg<BN, TA, false, true>::kThreads, 1)
+    gemm_wgmma_grouped_int4_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ MoeWeightMaps maps_w,
+                                   const __grid_constant__ MoeWeightGroupScales gscales, const TcGemmParams p, const int32_t* __restrict__ plan) {
+  tc_gemm_body<MODE, 1, BN, TA, true, false, true>(map_a, maps_w.m, p, plan, nullptr, nullptr, &gscales);
 }
 
 // ---- host: tensor maps (driver API through the runtime's entry-point lookup, no libcuda link dependency) ----

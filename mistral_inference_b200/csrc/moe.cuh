@@ -389,48 +389,69 @@ inline int64_t moe_tile_cap(int64_t pairs, int64_t E, int tile_rows) { return (p
 inline int64_t moe_plan_words(int64_t pairs, int64_t E, int tile_rows) { return MOE_PLAN_HEADER + 4 * moe_tile_cap(pairs, E, tile_rows); }
 inline int64_t moe_row_cap(int64_t pairs, int64_t E, int tile_rows) { return moe_tile_cap(pairs, E, tile_rows) * tile_rows; }
 
-// Tensor maps of the experts' weights (bf16, or e4m3 when `scales` is given) and their scale table; an expert of another rank
-// (NULL) gets a placeholder that this rank's tiles never reference.
-inline int moe_weight_maps(MoeWeightMaps* maps, MoeWeightScales* sc, const CUtensorMap& placeholder, const void* const* w_host,
-                           const float* const* scales, int E, int64_t N, int64_t K, int box_rows) {
+// Weight format of a grouped call's experts.  FP8: `scales` holds E per-row fp32 scale arrays; INT4: E bf16 group-scale arrays.
+enum class MoeFmt { BF16, FP8, INT4 };
+
+// Tensor maps of the experts' weights (bf16, e4m3, or INT4 codes with boxes of int4_box_bytes) and their scale tables; an expert
+// of another rank (NULL) gets a placeholder that this rank's tiles never reference.
+inline int moe_weight_maps(MoeWeightMaps* maps, MoeWeightScales* sc, MoeWeightGroupScales* gsc, const CUtensorMap& placeholder,
+                           const void* const* w_host, MoeFmt fmt, const void* const* scales, int E, int64_t N, int64_t K, int box_rows,
+                           int int4_box_bytes = TG_BK / 2) {
   for (int e = 0; e < MOE_MAX_EXPERTS; ++e) {
     const void* w = e < E && w_host[e] != nullptr ? w_host[e] : nullptr;
-    sc->s[e] = w != nullptr && scales != nullptr ? scales[e] : nullptr;
+    const void* s = w != nullptr && fmt != MoeFmt::BF16 ? scales[e] : nullptr;
+    sc->s[e] = fmt == MoeFmt::FP8 ? static_cast<const float*>(s) : nullptr;
+    gsc->s[e] = fmt == MoeFmt::INT4 ? static_cast<const uint16_t*>(s) : nullptr;
     if (w == nullptr) {
       maps->m[e] = placeholder;
       continue;
     }
-    if (scales != nullptr && scales[e] == nullptr) return fail(MB200_E_INVALID, "grouped gemm: expert %d has e4m3 weights but no scales", e);
-    const int rc = scales ? make_tensor_map_e4m3(&maps->m[e], w, N, K, box_rows) : make_tensor_map_2d(&maps->m[e], w, N, K, box_rows);
+    if (fmt != MoeFmt::BF16 && s == nullptr) return fail(MB200_E_INVALID, "grouped gemm: expert %d has quantised weights but no scales", e);
+    if (fmt == MoeFmt::INT4 && (((uintptr_t)w & 15) != 0 || ((uintptr_t)s & 1) != 0))
+      return fail(MB200_E_INVALID, "grouped gemm (int4): expert %d: misaligned codes or scales", e);
+    const int rc = fmt == MoeFmt::FP8    ? make_tensor_map_e4m3(&maps->m[e], w, N, K, box_rows)
+                   : fmt == MoeFmt::INT4 ? make_tensor_map_int4(&maps->m[e], w, N, K, box_rows, int4_box_bytes)
+                                         : make_tensor_map_2d(&maps->m[e], w, N, K, box_rows);
     if (rc) return rc;
   }
   return MB200_OK;
 }
 
-// FP8 (`scales` given): gemm_wgmma_grouped_fp8_kernel, always one CTA per tile (CL = 1): in a cluster pair each CTA would have to
-// convert the whole multicast tile, and the e4m3 tile already halves the L2 -> SM bytes that the multicast saves a third of.
+// FP8 and INT4: gemm_wgmma_grouped_fp8_kernel / gemm_wgmma_grouped_int4_kernel, always one CTA per tile (CL = 1): in a cluster pair
+// each CTA would have to convert the whole multicast tile, and the quantised tile already cuts the L2 -> SM bytes that the
+// multicast saves a third of.  The tile's k order is the bf16 kernel's at the same BN, so the result is too.
 template <int MODE, int BN, int TA, int CL = 1>
 int launch_grouped_bn(const void* a, int64_t rows_cap, int64_t K, int64_t N, const void* const* w_host, int E, const int32_t* plan, const EpiParams& epi,
-                      int sms, cudaStream_t stream, const float* const* scales = nullptr) {
+                      int sms, cudaStream_t stream, MoeFmt fmt, const void* const* scales) {
   using Cfg = TgCfg<BN, TA>;
   CUtensorMap map_a;
   MoeWeightMaps maps;
   MoeWeightScales sc;
+  MoeWeightGroupScales gsc;
   int rc = make_tensor_map_2d(&map_a, a, rows_cap, K, TA);
   if (rc) return rc;
-  rc = moe_weight_maps(&maps, &sc, map_a, w_host, scales, E, N, K, scales ? BN : BN / CL);  // cluster pairs: each CTA fetches half of the W tile and multicasts it
+  // cluster pairs: each CTA fetches half of the W tile and multicasts it
+  rc = moe_weight_maps(&maps, &sc, &gsc, map_a, w_host, fmt, scales, E, N, K, fmt != MoeFmt::BF16 ? BN : BN / CL);
   if (rc) return rc;
   TcGemmParams p;
   p.T = (int)rows_cap;
   p.N = (int)N;
   p.K = (int)K;
   p.epi = epi;
-  if (scales != nullptr) {
+  if (fmt == MoeFmt::FP8) {
     using Cfg8 = TgCfg<BN, TA, true>;
     MB_CHECK_CUDA(cudaFuncSetAttribute(gemm_wgmma_grouped_fp8_kernel<MODE, BN, TA>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg8::kSmem));
     gemm_wgmma_grouped_fp8_kernel<MODE, BN, TA><<<sms, Cfg8::kThreads, Cfg8::kSmem, stream>>>(map_a, maps, sc, p, plan);
     MB_CHECK_LAUNCH("gemm_wgmma_grouped_fp8_kernel");
     note_launch("gemm_wgmma_grouped_fp8_kernel<%d, 1, %d, %d>", MODE, BN, TA);
+    return MB200_OK;
+  }
+  if (fmt == MoeFmt::INT4) {
+    using Cfg4 = TgCfg<BN, TA, false, true>;
+    MB_CHECK_CUDA(cudaFuncSetAttribute(gemm_wgmma_grouped_int4_kernel<MODE, BN, TA>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg4::kSmem));
+    gemm_wgmma_grouped_int4_kernel<MODE, BN, TA><<<sms, Cfg4::kThreads, Cfg4::kSmem, stream>>>(map_a, maps, gsc, p, plan);
+    MB_CHECK_LAUNCH("gemm_wgmma_grouped_int4_kernel");
+    note_launch("gemm_wgmma_grouped_int4_kernel<%d, %d, %d>", MODE, BN, TA);
     return MB200_OK;
   }
   MB_CHECK_CUDA(cudaFuncSetAttribute(gemm_wgmma_grouped_kernel<MODE, CL, BN, TA>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmem));
@@ -463,17 +484,18 @@ int launch_grouped_bn(const void* a, int64_t rows_cap, int64_t K, int64_t N, con
 // decode-sized calls: the stream-K weight-streaming kernel over (expert segment, n tile, k block) units
 template <int MODE, int TA>
 int launch_grouped_streamk(const void* a, int64_t rows_cap, int64_t K, int64_t N, const void* const* w_host, int E, const int32_t* plan,
-                           const EpiParams& epi, void* workspace, size_t workspace_bytes, int sms, cudaStream_t stream,
-                           const float* const* scales = nullptr) {
+                           const EpiParams& epi, void* workspace, size_t workspace_bytes, int sms, cudaStream_t stream, MoeFmt fmt,
+                           const void* const* scales) {
   using Cfg = TgCfg<SK_BN, TA>;
   if (sms > SK_MAX_CTAS) sms = SK_MAX_CTAS;
   if (workspace == nullptr || workspace_bytes < kWsSkPartials.end()) return fail(MB200_E_WORKSPACE, "grouped stream-K gemm: workspace %zu < %zu", workspace_bytes, kWsSkPartials.end());
   CUtensorMap map_a;
   MoeWeightMaps maps;
   MoeWeightScales sc;
+  MoeWeightGroupScales gsc;
   int rc = make_tensor_map_2d(&map_a, a, rows_cap, K, TA);
   if (rc) return rc;
-  rc = moe_weight_maps(&maps, &sc, map_a, w_host, scales, E, N, K, SK_BN);
+  rc = moe_weight_maps(&maps, &sc, &gsc, map_a, w_host, fmt, scales, E, N, K, SK_BN, SK_W4_CHUNK_KB * TG_BK / 2);
   if (rc) return rc;
   SkParams p;
   p.T = (int)rows_cap;
@@ -482,12 +504,20 @@ int launch_grouped_streamk(const void* a, int64_t rows_cap, int64_t K, int64_t N
   p.epi = epi;
   p.partials = reinterpret_cast<float*>((uint8_t*)workspace + kWsSkPartials.offset);
   p.flags = reinterpret_cast<unsigned*>((uint8_t*)workspace + kWsSkFlags.offset);
-  if (scales != nullptr) {
+  if (fmt == MoeFmt::FP8) {
     using Cfg8 = TgCfg<SK_BN, TA, true>;
     MB_CHECK_CUDA(cudaFuncSetAttribute(gemm_streamk_grouped_fp8_kernel<MODE, TA>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg8::kSmem));
     MB_CHECK_CUDA(launch_pdl(gemm_streamk_grouped_fp8_kernel<MODE, TA>, dim3((unsigned)sms), dim3(Cfg8::kThreads), (size_t)Cfg8::kSmem, stream, map_a, maps,
                              sc, p, plan));
     note_launch("gemm_streamk_grouped_fp8_kernel<%d, %d>", MODE, TA);
+    return MB200_OK;
+  }
+  if (fmt == MoeFmt::INT4) {  // (the grouped body waits for the plan before it requests any chunk)
+    using Cfg4 = SkW4Cfg<TA>;
+    MB_CHECK_CUDA(cudaFuncSetAttribute(gemm_streamk_grouped_int4_kernel<MODE, TA>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg4::kSmem));
+    MB_CHECK_CUDA(launch_pdl(gemm_streamk_grouped_int4_kernel<MODE, TA>, dim3((unsigned)sms), dim3(Cfg4::kThreads), (size_t)Cfg4::kSmem, stream, map_a,
+                             maps, gsc, p, plan));
+    note_launch("gemm_streamk_grouped_int4_kernel<%d, %d>", MODE, TA);
     return MB200_OK;
   }
   MB_CHECK_CUDA(cudaFuncSetAttribute(gemm_streamk_grouped_kernel<MODE, TA>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmem));
@@ -498,24 +528,25 @@ int launch_grouped_streamk(const void* a, int64_t rows_cap, int64_t K, int64_t N
 
 template <int MODE>
 int launch_grouped(const void* a, int64_t rows_cap, int64_t K, int64_t N, const void* const* w_host, int E, int est_mtiles, int tile_rows,
-                   const int32_t* plan, const EpiParams& epi, void* workspace, size_t workspace_bytes, cudaStream_t stream,
-                   const float* const* scales = nullptr) {
+                   const int32_t* plan, const EpiParams& epi, void* workspace, size_t workspace_bytes, cudaStream_t stream, MoeFmt fmt,
+                   const void* const* scales) {
   int dev = 0, sms = 0;
   MB_CHECK_CUDA(cudaGetDevice(&dev));
   MB_CHECK_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   MB_CHECK_ARG(K % TG_BK == 0 && N % 32 == 0, "grouped gemm: K=%lld must be a multiple of 64, N=%lld of 32", (long long)K, (long long)N);
+  MB_CHECK_ARG(fmt != MoeFmt::INT4 || K % kInt4Group == 0, "grouped gemm (int4): K=%lld must be a multiple of 128", (long long)K);
   if (tile_rows < 128 && streamk_eligible(tile_rows, N, K)) {
-    if (tile_rows == 32) return launch_grouped_streamk<MODE, 32>(a, rows_cap, K, N, w_host, E, plan, epi, workspace, workspace_bytes, sms, stream, scales);
-    return launch_grouped_streamk<MODE, 64>(a, rows_cap, K, N, w_host, E, plan, epi, workspace, workspace_bytes, sms, stream, scales);
+    if (tile_rows == 32) return launch_grouped_streamk<MODE, 32>(a, rows_cap, K, N, w_host, E, plan, epi, workspace, workspace_bytes, sms, stream, fmt, scales);
+    return launch_grouped_streamk<MODE, 64>(a, rows_cap, K, N, w_host, E, plan, epi, workspace, workspace_bytes, sms, stream, fmt, scales);
   }
   if (tile_rows == 128) {
     // enough rows per expert for vertically adjacent tile pairs: the 2-CTA cluster kernel (W tile multicast, 2/3 of the L2 -> SM traffic)
-    if (N % 256 == 0 && scales == nullptr && wgmma_cluster_enabled() && rows_cap >= (int64_t)E * 512)
-      return launch_grouped_bn<MODE, 256, 128, 2>(a, rows_cap, K, N, w_host, E, plan, epi, sms, stream, scales);
-    if (N % 256 == 0) return launch_grouped_bn<MODE, 256, 128>(a, rows_cap, K, N, w_host, E, plan, epi, sms, stream, scales);
-    if (N % 128 == 0) return launch_grouped_bn<MODE, 128, 128>(a, rows_cap, K, N, w_host, E, plan, epi, sms, stream, scales);
-    if (N % 64 == 0) return launch_grouped_bn<MODE, 64, 128>(a, rows_cap, K, N, w_host, E, plan, epi, sms, stream, scales);
-    return launch_grouped_bn<MODE, 32, 128>(a, rows_cap, K, N, w_host, E, plan, epi, sms, stream, scales);
+    if (N % 256 == 0 && fmt == MoeFmt::BF16 && wgmma_cluster_enabled() && rows_cap >= (int64_t)E * 512)
+      return launch_grouped_bn<MODE, 256, 128, 2>(a, rows_cap, K, N, w_host, E, plan, epi, sms, stream, fmt, scales);
+    if (N % 256 == 0) return launch_grouped_bn<MODE, 256, 128>(a, rows_cap, K, N, w_host, E, plan, epi, sms, stream, fmt, scales);
+    if (N % 128 == 0) return launch_grouped_bn<MODE, 128, 128>(a, rows_cap, K, N, w_host, E, plan, epi, sms, stream, fmt, scales);
+    if (N % 64 == 0) return launch_grouped_bn<MODE, 64, 128>(a, rows_cap, K, N, w_host, E, plan, epi, sms, stream, fmt, scales);
+    return launch_grouped_bn<MODE, 32, 128>(a, rows_cap, K, N, w_host, E, plan, epi, sms, stream, fmt, scales);
   }
   int best = 32;
   double best_score = -1.0;
@@ -537,17 +568,17 @@ int launch_grouped(const void* a, int64_t rows_cap, int64_t K, int64_t N, const 
   }
   if (tile_rows == 64) {
     switch (best) {
-      case 256: return launch_grouped_bn<MODE, 256, 64>(a, rows_cap, K, N, w_host, E, plan, epi, sms, stream, scales);
-      case 128: return launch_grouped_bn<MODE, 128, 64>(a, rows_cap, K, N, w_host, E, plan, epi, sms, stream, scales);
-      case 64: return launch_grouped_bn<MODE, 64, 64>(a, rows_cap, K, N, w_host, E, plan, epi, sms, stream, scales);
-      default: return launch_grouped_bn<MODE, 32, 64>(a, rows_cap, K, N, w_host, E, plan, epi, sms, stream, scales);
+      case 256: return launch_grouped_bn<MODE, 256, 64>(a, rows_cap, K, N, w_host, E, plan, epi, sms, stream, fmt, scales);
+      case 128: return launch_grouped_bn<MODE, 128, 64>(a, rows_cap, K, N, w_host, E, plan, epi, sms, stream, fmt, scales);
+      case 64: return launch_grouped_bn<MODE, 64, 64>(a, rows_cap, K, N, w_host, E, plan, epi, sms, stream, fmt, scales);
+      default: return launch_grouped_bn<MODE, 32, 64>(a, rows_cap, K, N, w_host, E, plan, epi, sms, stream, fmt, scales);
     }
   }
   switch (best) {
-    case 256: return launch_grouped_bn<MODE, 256, 32>(a, rows_cap, K, N, w_host, E, plan, epi, sms, stream, scales);
-    case 128: return launch_grouped_bn<MODE, 128, 32>(a, rows_cap, K, N, w_host, E, plan, epi, sms, stream, scales);
-    case 64: return launch_grouped_bn<MODE, 64, 32>(a, rows_cap, K, N, w_host, E, plan, epi, sms, stream, scales);
-    default: return launch_grouped_bn<MODE, 32, 32>(a, rows_cap, K, N, w_host, E, plan, epi, sms, stream, scales);
+    case 256: return launch_grouped_bn<MODE, 256, 32>(a, rows_cap, K, N, w_host, E, plan, epi, sms, stream, fmt, scales);
+    case 128: return launch_grouped_bn<MODE, 128, 32>(a, rows_cap, K, N, w_host, E, plan, epi, sms, stream, fmt, scales);
+    case 64: return launch_grouped_bn<MODE, 64, 32>(a, rows_cap, K, N, w_host, E, plan, epi, sms, stream, fmt, scales);
+    default: return launch_grouped_bn<MODE, 32, 32>(a, rows_cap, K, N, w_host, E, plan, epi, sms, stream, fmt, scales);
   }
 }
 

@@ -37,7 +37,7 @@ class _GateView:
         return self._layer.gate_weight
 
 
-EXPERT_WEIGHTS = ("bf16", "fp8")
+EXPERT_WEIGHTS = ("bf16", "fp8", "int4")
 
 
 class Fp8Expert(nn.Module):
@@ -88,6 +88,62 @@ def quantize_rows_(name: str, w: torch.Tensor, q: torch.Tensor, s: torch.Tensor)
     """q, s (e4m3 rows as uint8 and fp32 row scales, both possibly strided views) of the bf16 weight `w` of Linear `name`."""
     assert tuple(w.shape) == tuple(q.shape), f"{name}: shape {tuple(w.shape)} != expected {tuple(q.shape)}"
     _abi.quantize_e4m3_rows(w.to(device=q.device, dtype=torch.bfloat16).contiguous(), q, s)
+
+
+class _Int4Rows:
+    """INT4 storage of a module's packed matrices: `<m>` is uint8 [N, K/2] (two codes per byte, low nibble = even k), and
+    `<m>_gscale_bits` int16 [N, K/128] the bit patterns of the bf16 group scales (`Module.to(dtype)` casts every floating tensor;
+    these must keep their bits).  The module's `_slots` maps a reference Linear name to its (code rows, scale rows): zero-copy views,
+    strided where rows interleave."""
+
+    def _int4_params(self, name: str, n: int, k: int) -> nn.Parameter:
+        assert k % 128 == 0, f"{name}: K={k} is not a multiple of the 128-wide scale groups"
+        setattr(self, name + "_gscale_bits", nn.Parameter(torch.empty(n, k // 128, dtype=torch.int16), requires_grad=False))
+        return nn.Parameter(torch.empty(n, k // 2, dtype=torch.uint8), requires_grad=False)
+
+    def weight_int4(self, name: str) -> torch.Tensor:
+        return self._slots(name)[0]
+
+    def weight_gscale(self, name: str) -> torch.Tensor:
+        return self._slots(name)[1]
+
+    def quantize_int4_(self, name: str, w: torch.Tensor) -> None:
+        """Quantises the bf16 weight `w` of Linear `name` into place (one bf16 copy of `w` on the device while it runs)."""
+        q, s = self._slots(name)
+        assert tuple(w.shape) == (q.shape[0], 2 * q.shape[1]), f"{name}: shape {tuple(w.shape)} != expected {(q.shape[0], 2 * q.shape[1])}"
+        _abi.quantize_int4_groups(w.to(device=q.device, dtype=torch.bfloat16).contiguous(), q, s)
+
+
+class Int4Expert(nn.Module, _Int4Rows):
+    """One expert with INT4 weights, the format of the INT4 dense Linears (include/mistral_b200.h): `w13` uint8 [2*hidden, dim/2]
+    (row 2i = w1[i], row 2i + 1 = w3[i], like FeedForward.w13) and `w2_weight` uint8 [dim, hidden/2] hold the packed codes, with one
+    bf16 scale per group of 128 k of a row in `w13_gscale_bits` / `w2_gscale_bits` (int16 bit patterns; `w13_gscale` / `w2_gscale`
+    are the bf16 views).  Weights arrive as bf16 and are quantised in place on the device."""
+
+    def __init__(self, dim: int, hidden_dim: int):
+        super().__init__()
+        self.dim = dim
+        self.hidden_dim = hidden_dim
+        self.w13 = self._int4_params("w13", 2 * hidden_dim, dim)
+        self.w2_weight = self._int4_params("w2", dim, hidden_dim)
+
+    @property
+    def w13_gscale(self) -> torch.Tensor:
+        return self.w13_gscale_bits.view(torch.bfloat16)
+
+    @property
+    def w2_gscale(self) -> torch.Tensor:
+        return self.w2_gscale_bits.view(torch.bfloat16)
+
+    def _slots(self, name: str) -> Tuple[torch.Tensor, torch.Tensor]:
+        """(code rows, scale rows) of the reference Linear `name` (w1, w2 or w3): zero-copy, strided for w1 / w3."""
+        h, d = self.hidden_dim, self.dim
+        if name in ("w1", "w3"):
+            seg = 0 if name == "w1" else 1
+            return self.w13.view(h, 2, d // 2)[:, seg], self.w13_gscale.view(h, 2, d // 128)[:, seg]
+        if name == "w2":
+            return self.w2_weight, self.w2_gscale
+        raise ValueError(f"expert Linear {name!r}")
 
 
 class MoeBuffers:
@@ -177,6 +233,9 @@ class MoeLayer(nn.Module):
         self.expert_shard = expert_shard
         self.expert_group = expert_group
         self.layer_parity = 0  # set by the model: consecutive MoE layers alternate the exchange buffer
+        first = self.experts[str(self.local_expert_ids[0])]
+        # the experts' storage format, one of EXPERT_WEIGHTS: which grouped entry point runs and which tensors it reads
+        self.expert_weights = "fp8" if isinstance(first, Fp8Expert) else ("int4" if isinstance(first, Int4Expert) else "bf16")
         self._ptrs = None
 
     @property
@@ -193,14 +252,16 @@ class MoeLayer(nn.Module):
 
     @property
     def fp8(self) -> bool:
-        return isinstance(self.experts[str(self.local_expert_ids[0])], Fp8Expert)
+        return self.expert_weights == "fp8"
 
     def _weight_tables(self):
-        """HOST arrays of E device pointers (NULL for experts of other ranks), rebuilt when a weight moved: (w13, w2), and for FP8
-        experts (w13_q, w13 scales, w2_q, w2 scales)."""
+        """HOST arrays of E device pointers (NULL for experts of other ranks), rebuilt when a weight moved: (w13, w2), for FP8
+        experts (w13_q, w13 scales, w2_q, w2 scales), for INT4 experts (w13 codes, w13 group scales, w2 codes, w2 group scales)."""
         E = self.args.num_experts
-        if self.fp8:
+        if self.expert_weights == "fp8":
             tensors = lambda ex: (ex.w13_q, ex.w13_scale_bits, ex.w2_q, ex.w2_scale_bits)  # noqa: E731
+        elif self.expert_weights == "int4":
+            tensors = lambda ex: (ex.w13, ex.w13_gscale_bits, ex.w2_weight, ex.w2_gscale_bits)  # noqa: E731
         else:
             tensors = lambda ex: (ex.w13, ex.w2_weight)  # noqa: E731
         key = tuple((e, *(t.data_ptr() for t in tensors(self.experts[str(e)]))) for e in self.local_expert_ids)
@@ -229,8 +290,10 @@ class MoeLayer(nn.Module):
             _abi.moe_route(hn[r0:r1], self.gate_weight, E, k, g, G, b)
             res = residual[r0:r1] if residual is not None else None
             cs = comm.struct(self.layer_parity) if comm is not None else None
-            if len(tables) == 4:
+            if self.expert_weights == "fp8":
                 _abi.moe_grouped_ffn_fp8(b, *tables, res, out[r0:r1], n, dim, first.hidden_dim, E, k, cs, ws)
+            elif self.expert_weights == "int4":
+                _abi.moe_grouped_ffn_int4(b, *tables, res, out[r0:r1], n, dim, first.hidden_dim, E, k, cs, ws)
             else:
                 _abi.moe_grouped_ffn(b, *tables, res, out[r0:r1], n, dim, first.hidden_dim, E, k, cs, ws)
         return out

@@ -18,7 +18,7 @@ from . import _abi
 from .args import PATCH_MERGE, TransformerArgs
 from .cache import KV_CACHE_FORMATS, BufferCache, CacheInputMetadata
 from .rope import precompute_freqs_cis
-from .moe import EXPERT_WEIGHTS, Fp8Expert
+from .moe import EXPERT_WEIGHTS, Fp8Expert, Int4Expert
 from .transformer_layers import LoraAdapter, RMSNorm, TransformerBlock
 from .vision_encoder import PatchMerger, VisionLanguageAdapter, VisionTransformer
 
@@ -60,24 +60,31 @@ class _OutputView:
 DENSE_WEIGHTS = ("bf16", "fp8", "int4")
 
 
-def _check_dense_weights(args: TransformerArgs, dense_weights: str) -> None:
+def _check_dense_weights(args: TransformerArgs, dense_weights: str, expert_weights: str) -> None:
     """The refusals of dense_weights="fp8" / "int4", before anything is allocated."""
     if dense_weights not in DENSE_WEIGHTS:
         raise ValueError(f"dense_weights={dense_weights!r}: expected one of {DENSE_WEIGHTS}")
     if dense_weights == "bf16":
         return
     fmt = dense_weights.upper()
-    if args.moe is not None:
-        raise ValueError(f"dense_weights={dense_weights!r} needs a dense model: {fmt} attention Linears on mixture-of-experts models are "
-                         "not built (expert_weights='fp8' quantises the experts)")
+    if args.moe is not None and dense_weights == "fp8":
+        raise ValueError("dense_weights='fp8' needs a dense model: FP8 attention Linears on mixture-of-experts models are not built "
+                         "(dense_weights='int4' quantises their attention Linears, expert_weights='fp8' or 'int4' the experts)")
+    if args.moe is not None and expert_weights == "bf16":
+        # the attention Linears are a few per cent of a MoE model's bytes (Mixtral-8x22B: 9.9 of 281 GB): INT4 ones are only worth
+        # their T <= 4 rounding differences next to quantised experts
+        raise ValueError("dense_weights='int4' on a mixture-of-experts model quantises its attention Linears only and is built with "
+                         "quantised experts: pass expert_weights='int4' (or 'fp8') as well")
     if args.lora is not None:
         raise NotImplementedError(f"un-merged LoRA on {fmt} dense weights is not built (merge the adapter into a bf16 model instead)")
     # every Linear must stay off the mma.sync GEMM at every token count: it has no e4m3 or int4 variant (include/mistral_b200.h);
-    # INT4 scale groups are 128 k wide
+    # INT4 scale groups are 128 k wide.  On a MoE model only the attention Linears are dense (the experts follow expert_weights).
     k_mult = 128 if dense_weights == "int4" else 64
     q_dim, kv_dim = args.n_heads * args.head_dim, args.n_kv_heads * args.head_dim
-    for name, N, K in (("wqkv", q_dim + 2 * kv_dim, args.dim), ("wo", args.dim, q_dim), ("w13", 2 * args.hidden_dim, args.dim),
-                       ("w2", args.dim, args.hidden_dim)):
+    linears = [("wqkv", q_dim + 2 * kv_dim, args.dim), ("wo", args.dim, q_dim)]
+    if args.moe is None:
+        linears += [("w13", 2 * args.hidden_dim, args.dim), ("w2", args.dim, args.hidden_dim)]
+    for name, N, K in linears:
         if K % k_mult != 0 or (N % 128 != 0 and N % 192 != 0):
             groups = " or would split a 128-wide scale group" if dense_weights == "int4" else ""
             raise ValueError(f"dense_weights={dense_weights!r}: {name} [{N}, {K}] would need the mma.sync GEMM, which has no {fmt} variant"
@@ -92,16 +99,18 @@ class Transformer(nn.Module):
         `e % world == rank` over the ranks of `expert_group` (default process group), everything else replicated, one
         all-reduce of [T, dim] per MoE layer (SURVEY.md 8e); and `expert_weights`: "bf16", or "fp8" to store every MoE expert
         matrix as e4m3 with one fp32 scale per row (moe.Fp8Expert; the model then computes exactly what the bf16 model computes
-        with the dequantised weights W', see include/mistral_b200.h); and `kv_cache`: "bf16", or "fp8" to keep the KV cache as e4m3
+        with the dequantised weights W', see include/mistral_b200.h), or "int4" to store them in the format of the INT4 dense
+        Linears below (moe.Int4Expert; again exactly the bf16 model on W'); and `kv_cache`: "bf16", or "fp8" to keep the KV cache as e4m3
         with one power-of-two exponent per (slot, kv head) row (cache.BufferCache; the model is then the bf16 model with k, v
         replaced by their dequantised k', v' right after RoPE in every forward that has a cache, see include/mistral_b200.h); and
         `dense_weights`: "bf16", or "fp8" to store wq, wk, wv, wo, w1, w2 and w3 of every text layer of a dense model as e4m3 with
         one fp32 scale per row, applied after the dot product: y = bf16(s * sum_k x * q) (include/mistral_b200.h; the embedding,
         the lm head, the norms and the vision tower stay bf16).  That model is not bit-identical to any bf16 model.  "int4" stores the
         same Linears as symmetric 4-bit codes with one bf16 scale per group of 128 k of a row; that model computes exactly what the
-        bf16 model computes with the dequantised weights W' (include/mistral_b200.h)."""
+        bf16 model computes with the dequantised weights W' (include/mistral_b200.h).  On a mixture-of-experts model "int4" stores
+        wq, wk, wv and wo only, and needs quantised experts (`expert_weights` "int4" or "fp8")."""
         super().__init__()
-        _check_dense_weights(args, dense_weights)
+        _check_dense_weights(args, dense_weights, expert_weights)
         self.dense_weights = dense_weights
         if kv_cache not in KV_CACHE_FORMATS:
             raise ValueError(f"kv_cache={kv_cache!r}: expected one of {KV_CACHE_FORMATS}")
@@ -113,8 +122,12 @@ class Transformer(nn.Module):
         self.kv_cache = kv_cache
         if expert_weights not in EXPERT_WEIGHTS:
             raise ValueError(f"expert_weights={expert_weights!r}: expected one of {EXPERT_WEIGHTS}")
-        if expert_weights == "fp8" and args.moe is None:
-            raise ValueError("expert_weights='fp8' needs a mixture-of-experts model: only the grouped expert GEMMs read FP8 weights")
+        if expert_weights != "bf16" and args.moe is None:
+            raise ValueError(f"expert_weights={expert_weights!r} needs a mixture-of-experts model: only the grouped expert GEMMs read "
+                             f"{expert_weights.upper()} weights")
+        if expert_weights == "int4" and (args.dim % 128 != 0 or args.hidden_dim % 128 != 0):
+            raise ValueError(f"expert_weights='int4': dim={args.dim} and hidden_dim={args.hidden_dim} must be multiples of 128, the width "
+                             "of the scale groups")
         self.expert_weights = expert_weights
         if args.lora is not None and args.moe is not None:
             raise NotImplementedError("un-merged LoRA on mixture-of-experts layers is not built: the grouped expert GEMMs have no "
@@ -633,7 +646,8 @@ class Transformer(nn.Module):
                         put(mod.weight_e4m3(name), lambda _seg, w, mod=mod, name=name: mod.quantize_(name, w))
                         return True
         if getattr(att, "int4", False):  # INT4 dense weights: the reference's bf16 weight, quantised into place (the codes are [N, K/2])
-            for mod, names in ((att, ("wq", "wk", "wv", "wo")), (ff, ("w1", "w2", "w3"))):
+            dense = ((att, ("wq", "wk", "wv", "wo")),) + (() if hasattr(ff, "experts") else ((ff, ("w1", "w2", "w3")),))
+            for mod, names in dense:
                 for name in names:
                     if rest.startswith(f"{'attention' if mod is att else 'feed_forward'}.{name}."):
                         if rest.rsplit(".", 1)[1] != "weight":
@@ -672,6 +686,15 @@ class Transformer(nn.Module):
                     name = parts[1]
                     put(ff.weight_e4m3(name), lambda _seg, w: ff.quantize_(name, w))
                     return True
+                if isinstance(ff, Int4Expert):  # the reference's bf16 weight, quantised into place (the codes are [N, K/2])
+                    if parts[2:] != ["weight"] or parts[1] not in ("w1", "w2", "w3"):
+                        raise ValueError(f"Unexpected key {k}")
+                    name = parts[1]
+                    q = ff.weight_int4(name)
+                    put(torch.empty(q.shape[0], 2 * q.shape[1], device="meta"), lambda _seg, w: ff.quantize_int4_(name, w))
+                    return True
+            elif hasattr(ff, "experts"):  # a MoE block has no dense feed_forward.w1/w2/w3
+                raise ValueError(f"Unexpected key {k}")
             name = parts[1]
             if name == "w1":
                 put(ff.w13.view(ff.hidden_dim, 2, ff.dim)[:, 0])
@@ -800,12 +823,15 @@ class Transformer(nn.Module):
                     out[p + prefix + n + ".weight_e4m3"] = mod.weight_e4m3(n)
                     out[p + prefix + n + ".weight_scale"] = mod.weight_scale(n)
             return
-        if int4:  # the stored format itself: no dequantised copies
-            for mod, prefix, names in ((att, "attention.", ("wq", "wk", "wv", "wo")), (ff, "feed_forward.", ("w1", "w2", "w3"))):
+        if int4:  # the stored format itself: no dequantised copies (on a MoE block the attention Linears only)
+            moe = hasattr(ff, "experts")
+            dense = ((att, "attention.", ("wq", "wk", "wv", "wo")),) + (() if moe else ((ff, "feed_forward.", ("w1", "w2", "w3")),))
+            for mod, prefix, names in dense:
                 for n in names:
                     out[p + prefix + n + ".weight_int4"] = mod.weight_int4(n)
                     out[p + prefix + n + ".weight_gscale"] = mod.weight_gscale(n)
-            return
+            if not moe:
+                return
         if hasattr(ff, "experts"):
             out[p + "feed_forward.gate.weight"] = ff.gate_weight
             for e, ex in ff.experts.items():  # keyed by the global expert id; the local ones only when sharded
@@ -813,6 +839,9 @@ class Transformer(nn.Module):
                     if isinstance(ex, Fp8Expert):  # the stored format itself: no dequantised copies
                         out[p + f"feed_forward.experts.{e}.{n}.weight_e4m3"] = ex.weight_e4m3(n)
                         out[p + f"feed_forward.experts.{e}.{n}.weight_scale"] = ex.weight_scale(n)
+                    elif isinstance(ex, Int4Expert):
+                        out[p + f"feed_forward.experts.{e}.{n}.weight_int4"] = ex.weight_int4(n)
+                        out[p + f"feed_forward.experts.{e}.{n}.weight_gscale"] = ex.weight_gscale(n)
                     else:
                         out[p + f"feed_forward.experts.{e}.{n}.weight"] = getattr(ex, n).weight
         else:
@@ -855,9 +884,9 @@ class Transformer(nn.Module):
         if self.dense_weights != "bf16" and any(key.startswith("layers.") for key in lora_state_dict):
             raise NotImplementedError(f"merging a LoRA adapter into {self.dense_weights.upper()} dense weights is not built: the layer "
                                       "Linears are stored quantised (load the adapter into a bf16 model)")
-        if self.expert_weights == "fp8" and any(".experts." in key for key in lora_state_dict):
-            raise NotImplementedError("merging a LoRA adapter into FP8 expert weights is not built: the experts are stored quantised "
-                                      "(load the adapter into a bf16 model, or drop its expert Linears)")
+        if self.expert_weights != "bf16" and any(".experts." in key for key in lora_state_dict):
+            raise NotImplementedError(f"merging a LoRA adapter into {self.expert_weights.upper()} expert weights is not built: the experts "
+                                      "are stored quantised (load the adapter into a bf16 model, or drop its expert Linears)")
         lora_state_dict = {k: v.to(self.device) for k, v in lora_state_dict.items()}
         if self.args.lora is not None:
             with torch.no_grad():
@@ -900,8 +929,8 @@ class Transformer(nn.Module):
                     softmax_fp32: bool = True, expert_parallel: Optional[Tuple[int, int]] = None, expert_group: Any = None,
                     expert_weights: str = "bf16", *, kv_cache: str = "bf16", dense_weights: str = "bf16") -> "Transformer":
         """transformer.py:297-338.  Tensors stream from disk straight into the packed device buffers; with `expert_parallel`
-        the experts of other ranks are skipped (never read into device memory).  With expert_weights="fp8" each bf16 expert
-        tensor is copied to the device and quantised into place: the peak is the FP8 model plus about one bf16 tensor.
+        the experts of other ranks are skipped (never read into device memory).  With expert_weights="fp8" or "int4" each bf16
+        expert tensor is copied to the device and quantised into place: the peak is the quantised model plus about one bf16 tensor.
         `kv_cache` ("bf16" | "fp8") is the format of the KV cache that generate() builds (see Transformer).  With
         dense_weights="fp8" or "int4" every bf16 layer Linear is quantised into place the same way."""
         with open(Path(folder) / "params.json", "r") as f:

@@ -19,7 +19,7 @@ from torch import nn
 from . import _abi
 from .args import LoraArgs, MoeArgs
 from .cache import CacheView
-from .moe import Fp8Expert, MoeLayer, quantize_rows_
+from .moe import Fp8Expert, Int4Expert, MoeLayer, _Int4Rows, quantize_rows_
 
 
 class _WeightView:
@@ -110,30 +110,6 @@ class _Fp8Rows:
     def quantize_(self, name: str, w: torch.Tensor) -> None:
         """Quantises the bf16 weight `w` of Linear `name` into place (one bf16 copy of `w` on the device while it runs)."""
         quantize_rows_(name, w, *self._slots(name))
-
-
-class _Int4Rows:
-    """INT4 dense storage of a module's packed matrices: `<m>` is uint8 [N, K/2] (two codes per byte, low nibble = even k), and
-    `<m>_gscale_bits` int16 [N, K/128] the bit patterns of the bf16 group scales (`Module.to(dtype)` casts every floating tensor;
-    these must keep their bits).  The module's `_slots` maps a reference Linear name to its (code rows, scale rows): zero-copy views,
-    strided where rows interleave."""
-
-    def _int4_params(self, name: str, n: int, k: int) -> nn.Parameter:
-        assert k % 128 == 0, f"{name}: K={k} is not a multiple of the 128-wide scale groups"
-        setattr(self, name + "_gscale_bits", nn.Parameter(torch.empty(n, k // 128, dtype=torch.int16), requires_grad=False))
-        return nn.Parameter(torch.empty(n, k // 2, dtype=torch.uint8), requires_grad=False)
-
-    def weight_int4(self, name: str) -> torch.Tensor:
-        return self._slots(name)[0]
-
-    def weight_gscale(self, name: str) -> torch.Tensor:
-        return self._slots(name)[1]
-
-    def quantize_int4_(self, name: str, w: torch.Tensor) -> None:
-        """Quantises the bf16 weight `w` of Linear `name` into place (one bf16 copy of `w` on the device while it runs)."""
-        q, s = self._slots(name)
-        assert tuple(w.shape) == (q.shape[0], 2 * q.shape[1]), f"{name}: shape {tuple(w.shape)} != expected {(q.shape[0], 2 * q.shape[1])}"
-        _abi.quantize_int4_groups(w.to(device=q.device, dtype=torch.bfloat16).contiguous(), q, s)
 
 
 class RMSNorm(nn.Module):
@@ -405,14 +381,17 @@ class TransformerBlock(nn.Module):
         self.dim = dim
         self.norm_eps = norm_eps
         fp8, int4 = dense_weights == "fp8", dense_weights == "int4"
-        assert not (fp8 or int4) or (moe is None and lora is None), "quantised dense weights: dense layers without un-merged LoRA only"
+        assert not (fp8 or int4) or lora is None, "quantised dense weights: layers without un-merged LoRA only"
+        assert not fp8 or moe is None, "FP8 dense weights: dense layers only"
+        # on a MoE block INT4 dense weights are the attention Linears only; the experts follow expert_weights
         self.attention = Attention(dim=dim, n_heads=n_heads, head_dim=head_dim, n_kv_heads=n_kv_heads, lora=lora, fp8=fp8, int4=int4)
         self.attention_norm = RMSNorm(dim, eps=norm_eps)
         self.ffn_norm = RMSNorm(dim, eps=norm_eps)
         self.feed_forward: nn.Module
         if moe is not None:
             g, G = expert_shard  # this rank allocates only the experts it owns (e % G == g): SURVEY.md 8(e)
-            expert = (lambda: Fp8Expert(dim, hidden_dim)) if expert_weights == "fp8" else (lambda: FeedForward(dim=dim, hidden_dim=hidden_dim, lora=lora))
+            expert = {"fp8": lambda: Fp8Expert(dim, hidden_dim), "int4": lambda: Int4Expert(dim, hidden_dim)}.get(
+                expert_weights, lambda: FeedForward(dim=dim, hidden_dim=hidden_dim, lora=lora))
             self.feed_forward = MoeLayer(experts={e: expert() for e in range(moe.num_experts) if e % G == g},
                                          gate_weight=nn.Parameter(torch.empty(moe.num_experts, dim), requires_grad=False), moe_args=moe,
                                          expert_shard=expert_shard, expert_group=expert_group)
