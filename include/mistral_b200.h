@@ -264,6 +264,37 @@ int mb200_sample_top_p(const float* logits, const float* uniform_dev, int64_t* o
                        float temperature, float top_p, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * Speculative decoding: a draft model proposes k tokens per sequence, the target scores the S = k + 1 tokens
+ * [last, d_1 .. d_k] of every sequence in one forward (the verify step), and an acceptance rule keeps a prefix.
+ *
+ * mb200_spec_meta: the metadata block BufferCache.build_metadata_host builds for seqlens = [S] * B at the positions
+ *   seqpos_dev, for the chunked-prefill layout (T = B * S):
+ *     positions[T] | q_start[B+1] | seqpos[B] | per distinct window W: cache_rows[T], kv_len[B]
+ *   seqpos_dev [B] int32 (DEVICE, read only); meta_dev [T + 2B + 1 + n_windows * (T + B)] int32 (DEVICE, out);
+ *   windows_host as in mb200_decode_meta.  With it a CUDA graph of the verify step replays without host writes.
+ *
+ * mb200_spec_accept_greedy / mb200_spec_accept_sample, one CTA per sequence b:
+ *   logits [B * S, vocab] fp32: the verify step's rows, row b * S + j scores the token after input j;
+ *   tokens_dev [B, S] int64: the verify step's input [last, d_1 .. d_k];
+ *   out_dev [B, S] int64 (out): d_1 .. d_n, then the target's token, then -1;  n_dev [B] int32 (out): n, the accepted proposals;
+ *   seqpos_dev [B] int32 (in/out): advanced by n + 1 (the cached prefix [last, d_1 .. d_n]).
+ *   greedy: a_j = argmax of row j with the first index on ties (as mb200_argmax_rows); n = the longest prefix with d_{j+1} == a_j;
+ *           the last token is a_n.
+ *   sample: standard speculative sampling (Leviathan et al. 2023; Chen et al. 2023) on the nucleus distributions
+ *           mb200_sample_top_p draws from at (temperature, top_p): P_j of target row j, Q_j of draft_logits [B * k, vocab]
+ *           row b * k + j.  d_{j+1} is accepted iff u[b, j] * Q_j(d) < P_j(d); at the first rejection the last token is drawn
+ *           from max(0, P_j - Q_j) renormalised, after k acceptances from P_k, both with u[b, k]; uniform_dev [B, S] fp32 in [0, 1).
+ *   The emitted tokens' log-probabilities are mb200_logprob_gather over (logits, out_dev): rows with -1 are skipped.
+ */
+int mb200_spec_meta(const int32_t* seqpos_dev, int32_t* meta_dev, int64_t B, int64_t S, const int32_t* windows_host, int64_t n_windows,
+                    void* stream);
+int mb200_spec_accept_greedy(const float* logits, const int64_t* tokens_dev, int64_t* out_dev, int32_t* n_dev, int32_t* seqpos_dev, int64_t B,
+                             int64_t S, int64_t vocab, void* stream);
+int mb200_spec_accept_sample(const float* logits, const float* draft_logits, const int64_t* tokens_dev, const float* uniform_dev, int64_t* out_dev,
+                             int32_t* n_dev, int32_t* seqpos_dev, int64_t B, int64_t S, int64_t vocab, float temperature, float top_p,
+                             void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * Mixture of experts for T > 1 tokens (prefill, batched decode).  Replaces MoeLayer.forward (moe.py:24-32): the gate Linear,
  * torch.topk on the bf16 router logits, the fp32 softmax over the k selected, and the per-expert torch.where / gather /
  * FeedForward / weighted `results[idx] +=` loop (one host sync per expert) -- with no host round trip at all.
@@ -410,7 +441,8 @@ int mb200_decode_step(const mb200_layer_desc* layers_dev, const int32_t* windows
 int mb200_debug_set_decode_timeline(void* device_buffer);
 /* Debug: [n_sm][n_layers][6][2] uint64 arrive/leave stamps of every CTA at every grid barrier (NULL = off). */
 int mb200_debug_set_barrier_timeline(void* device_buffer);
-/* Debug, per calling thread: the attention, dense GEMM, mixture-of-experts and vision data-movement kernels launched since the last call, one line each, named like the
+/* Debug, per calling thread: the attention, dense GEMM, mixture-of-experts, vision data-movement and speculative-decoding (spec_meta, spec_accept_*)
+ * kernels launched since the last call, one line each, named like the
  * kernel with its template arguments (e.g. "attn_decode_tma_kernel<8>", "gemm_wgmma_kernel<0, 1, 32, 64>").  Copies the log
  * into `out` (NUL-terminated; NULL discards it), clears it, and switches recording on (enable != 0) or off.  MB200_E_INVALID
  * when `out` is too small or launches were dropped because the log filled up.  Tests use it to check which kernel a call chose. */

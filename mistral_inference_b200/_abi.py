@@ -56,6 +56,10 @@ _SIGNATURES = {
     "mb200_argmax_rows": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_void_p]),
     "mb200_logprob_gather": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_void_p]),
     "mb200_sample_top_p": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_float, c_float, c_void_p]),
+    "mb200_spec_meta": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_void_p, c_int64, c_void_p]),
+    "mb200_spec_accept_greedy": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_void_p]),
+    "mb200_spec_accept_sample": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64,
+                                         c_float, c_float, c_void_p]),
     "mb200_moe_sizes": (c_int, [c_int64, c_int64, c_int64, ctypes.POINTER(c_int64), ctypes.POINTER(c_int64), ctypes.POINTER(c_int64)]),
     "mb200_moe_route": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int64, c_int64, c_int64, c_void_p, c_void_p, c_void_p, c_void_p,
                                 c_void_p, c_void_p, c_void_p]),
@@ -453,6 +457,46 @@ def sample_top_p(logits: torch.Tensor, uniform: torch.Tensor, temperature: float
     return out
 
 
+# ---- speculative decoding (include/mistral_b200.h): the verify step's metadata and the acceptance kernels ----
+def spec_meta_words(B: int, S: int, n_windows: int) -> int:
+    """int32 words of the metadata block of a verify step of S tokens per sequence."""
+    return B * S + 2 * B + 1 + n_windows * (B * S + B)
+
+
+def spec_meta(seqpos_dev: torch.Tensor, meta_dev: torch.Tensor, S: int, windows) -> None:
+    """Device-side metadata of a verify step of S tokens per sequence at the positions `seqpos_dev` (read, not advanced)."""
+    B = seqpos_dev.shape[0]
+    arr = (ctypes.c_int32 * len(windows))(*[int(w) for w in windows])
+    assert seqpos_dev.dtype == torch.int32 and meta_dev.dtype == torch.int32 and meta_dev.numel() >= spec_meta_words(B, S, len(windows))
+    _check(lib().mb200_spec_meta(_ptr(seqpos_dev), _ptr(meta_dev), B, S, ctypes.cast(arr, c_void_p), len(windows), _stream()), "mb200_spec_meta")
+
+
+def _check_accept(logits: torch.Tensor, tokens: torch.Tensor, out: torch.Tensor, n: torch.Tensor, seqpos: torch.Tensor):
+    B, S = tokens.shape
+    assert logits.dtype == torch.float32 and logits.shape[0] == B * S and tokens.dtype == torch.long
+    assert out.dtype == torch.long and out.shape == (B, S) and n.dtype == torch.int32 and n.shape == (B,)
+    assert seqpos.dtype == torch.int32 and seqpos.shape == (B,)
+    return B, S, logits.shape[1]
+
+
+def spec_accept_greedy(logits: torch.Tensor, tokens: torch.Tensor, out: torch.Tensor, n: torch.Tensor, seqpos: torch.Tensor) -> None:
+    """Greedy acceptance of the proposals tokens[:, 1:] against the verify logits [B * S, V]; advances `seqpos` by n + 1."""
+    B, S, V = _check_accept(logits, tokens, out, n, seqpos)
+    _check(lib().mb200_spec_accept_greedy(_ptr(logits), _ptr(tokens), _ptr(out), _ptr(n), _ptr(seqpos), B, S, V, _stream()),
+           "mb200_spec_accept_greedy")
+
+
+def spec_accept_sample(logits: torch.Tensor, draft_logits: torch.Tensor, tokens: torch.Tensor, uniform: torch.Tensor, out: torch.Tensor,
+                       n: torch.Tensor, seqpos: torch.Tensor, temperature: float, top_p: float) -> None:
+    """Speculative sampling on the nucleus distributions: draft_logits [B * (S - 1), V] are the rows the proposals were drawn from,
+    uniform [B, S] fp32; advances `seqpos` by n + 1."""
+    B, S, V = _check_accept(logits, tokens, out, n, seqpos)
+    assert draft_logits.dtype == torch.float32 and draft_logits.shape == (B * (S - 1), V)
+    assert uniform.dtype == torch.float32 and uniform.shape == (B, S)
+    _check(lib().mb200_spec_accept_sample(_ptr(logits), _ptr(draft_logits), _ptr(tokens), _ptr(uniform), _ptr(out), _ptr(n), _ptr(seqpos), B, S,
+                                          V, temperature, top_p, _stream()), "mb200_spec_accept_sample")
+
+
 class MoeCommStruct(ctypes.Structure):
     """mb200_moe_comm (include/mistral_b200.h)."""
     _fields_ = [("n_ranks", ctypes.c_int32), ("my_rank", ctypes.c_int32), ("peer_yw", c_void_p * 8), ("my_flags", c_void_p),
@@ -579,7 +623,7 @@ def set_barrier_timeline(buf: Optional[torch.Tensor]) -> None:
 
 
 def launch_log(enable: bool) -> list:
-    """Names of the attention / GEMM / MoE kernels launched from this thread since the last call (empty while recording is off);
+    """Names of the attention / GEMM / MoE / speculative-decoding kernels launched from this thread since the last call (empty while recording is off);
     clears the log and switches recording on or off (include/mistral_b200.h)."""
     buf = ctypes.create_string_buffer(32768)
     _check(lib().mb200_debug_launch_log(int(enable), ctypes.cast(buf, c_void_p), len(buf)), "mb200_debug_launch_log")

@@ -18,6 +18,7 @@
 #include "moe.cuh"
 #include "sampling.cuh"
 #include "skinny_linear.cuh"
+#include "speculative.cuh"
 #include "vision.cuh"
 #include "workspace.cuh"
 
@@ -326,6 +327,56 @@ int mb200_decode_meta(int32_t* seqpos_dev, int32_t* meta_dev, int64_t B, const i
   }
   decode_meta_kernel<<<(unsigned)ceil_div(B + 1, 128), 128, 0, (cudaStream_t)stream>>>(p);
   MB_CHECK_LAUNCH("decode_meta_kernel");
+  return MB200_OK;
+}
+
+int mb200_spec_meta(const int32_t* seqpos_dev, int32_t* meta_dev, int64_t B, int64_t S, const int32_t* windows_host, int64_t n_windows,
+                    void* stream) {
+  MB_CHECK_ARG(seqpos_dev && meta_dev && windows_host, "spec_meta: null pointer");
+  MB_CHECK_ARG(B >= 1 && S >= 1 && B * S <= (1 << 24) && n_windows >= 1 && n_windows <= kMaxWindows,
+               "spec_meta: B=%lld, S=%lld, n_windows=%lld (max %d)", (long long)B, (long long)S, (long long)n_windows, kMaxWindows);
+  SpecMetaParams p;
+  p.seqpos = seqpos_dev;
+  p.meta = meta_dev;
+  p.B = (int)B;
+  p.S = (int)S;
+  p.n_w = (int)n_windows;
+  for (int j = 0; j < (int)n_windows; ++j) {
+    MB_CHECK_ARG(windows_host[j] >= 1, "spec_meta: window %d", (int)windows_host[j]);
+    p.windows[j] = windows_host[j];
+  }
+  const int64_t threads = B * S > B + 1 ? B * S : B + 1;
+  spec_meta_kernel<<<(unsigned)ceil_div(threads, 128), 128, 0, (cudaStream_t)stream>>>(p);
+  note_launch("spec_meta_kernel");
+  MB_CHECK_LAUNCH("spec_meta_kernel");
+  return MB200_OK;
+}
+
+int mb200_spec_accept_greedy(const float* logits, const int64_t* tokens_dev, int64_t* out_dev, int32_t* n_dev, int32_t* seqpos_dev, int64_t B,
+                             int64_t S, int64_t vocab, void* stream) {
+  MB_CHECK_ARG(logits && tokens_dev && out_dev && n_dev && seqpos_dev, "spec_accept_greedy: null pointer");
+  MB_CHECK_ARG(B >= 1 && S >= 2 && vocab >= 1 && vocab <= 0x7fffffff, "spec_accept_greedy: B=%lld S=%lld vocab=%lld", (long long)B, (long long)S,
+               (long long)vocab);
+  spec_accept_greedy_kernel<<<(unsigned)B, SP_THREADS, 0, (cudaStream_t)stream>>>(logits, (const long long*)tokens_dev, (long long*)out_dev,
+                                                                                 n_dev, seqpos_dev, (int)S, (int)vocab);
+  note_launch("spec_accept_greedy_kernel");
+  MB_CHECK_LAUNCH("spec_accept_greedy_kernel");
+  return MB200_OK;
+}
+
+int mb200_spec_accept_sample(const float* logits, const float* draft_logits, const int64_t* tokens_dev, const float* uniform_dev, int64_t* out_dev,
+                             int32_t* n_dev, int32_t* seqpos_dev, int64_t B, int64_t S, int64_t vocab, float temperature, float top_p,
+                             void* stream) {
+  MB_CHECK_ARG(logits && draft_logits && tokens_dev && uniform_dev && out_dev && n_dev && seqpos_dev, "spec_accept_sample: null pointer");
+  MB_CHECK_ARG(B >= 1 && S >= 2 && vocab >= 1 && vocab <= 0x7fffffff, "spec_accept_sample: B=%lld S=%lld vocab=%lld", (long long)B, (long long)S,
+               (long long)vocab);
+  MB_CHECK_ARG(temperature > 0.f && top_p >= 0.f && top_p <= 1.f, "spec_accept_sample: temperature=%g must be > 0 and top_p=%g in [0, 1]",
+               (double)temperature, (double)top_p);
+  spec_accept_sample_kernel<<<(unsigned)B, SP_THREADS, 0, (cudaStream_t)stream>>>(logits, draft_logits, (const long long*)tokens_dev, uniform_dev,
+                                                                                 (long long*)out_dev, n_dev, seqpos_dev, (int)S, (int)vocab,
+                                                                                 1.0f / temperature, top_p);
+  note_launch("spec_accept_sample_kernel");
+  MB_CHECK_LAUNCH("spec_accept_sample_kernel");
   return MB200_OK;
 }
 

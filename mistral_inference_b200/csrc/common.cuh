@@ -38,7 +38,7 @@ inline int fail(int code, const char* fmt, ...) {
     if (e__ != cudaSuccess) return ::mb200::fail(MB200_E_CUDA, "%s: %s", #expr, cudaGetErrorString(e__)); \
   } while (0)
 
-// ---- launch log (mb200_debug_launch_log): which attention / GEMM / MoE kernel each call chose ------------------
+// ---- launch log (mb200_debug_launch_log): which attention / GEMM / MoE / speculative kernel each call chose --------
 // Off unless switched on: one thread-local flag test per launch.  One line per launch, named like the kernel with its template
 // arguments ("attn_decode_tma_kernel<8>", "gemm_wgmma_kernel<0, 1, 32, 64>").
 constexpr size_t kLaunchLogBytes = 16384;

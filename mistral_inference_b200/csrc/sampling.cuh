@@ -3,6 +3,7 @@
 //   argmax_rows_kernel      greedy pick: torch.argmax(logits, -1) (generate.py:156), first index on ties
 //   logprob_gather_kernel   log_softmax(logits, -1)[t, target[t]] (generate.py:101-117,134-135) without materialising [T, V]
 //   sample_top_p_kernel     softmax(logits / temperature) -> nucleus (top-p) filter -> one draw (generate.py:151-170)
+// The row argmax, the nucleus and the draw are device functions that the speculative acceptance kernels share.
 //
 // All three are one CTA per row over fp32 logits [T, V] (the lm head's output).  Roofline: HBM/L2 -- V * 4 bytes per row and
 // pass; argmax and logprob are single-pass (online log-sum-exp), top-p re-reads its row (L2 resident) during the threshold
@@ -43,8 +44,9 @@ __device__ __forceinline__ float block_max(float v, float* scratch) {
   return t;
 }
 
-__global__ void __launch_bounds__(SP_THREADS) argmax_rows_kernel(const float* __restrict__ logits, long long* __restrict__ out, int V) {
-  const float* row = logits + (int64_t)blockIdx.x * V;
+// argmax of one row with the first index on ties; the result is valid in thread 0 (the shared partials may be reused once
+// every thread has passed a __syncthreads after the call)
+__device__ __forceinline__ int block_argmax(const float* __restrict__ row, int V) {
   unsigned long long best = 0ull;
   for (int i = threadIdx.x; i < V; i += SP_THREADS) best = max(best, argmax_key(row[i], i));
 #pragma unroll
@@ -56,8 +58,13 @@ __global__ void __launch_bounds__(SP_THREADS) argmax_rows_kernel(const float* __
     best = sm[threadIdx.x];
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) best = max(best, __shfl_xor_sync(0xffffffffu, best, o));
-    if (threadIdx.x == 0) out[blockIdx.x] = (long long)(0x7fffffff - (int)(best & 0xffffffffull));
   }
+  return 0x7fffffff - (int)(best & 0xffffffffull);
+}
+
+__global__ void __launch_bounds__(SP_THREADS) argmax_rows_kernel(const float* __restrict__ logits, long long* __restrict__ out, int V) {
+  const int best = block_argmax(logits + (int64_t)blockIdx.x * V, V);
+  if (threadIdx.x == 0) out[blockIdx.x] = (long long)best;
 }
 
 // out[t] = logits[t, target[t]] - max - log(sum(exp(logits[t, :] - max)))   (fp32, like torch.log_softmax on fp32 logits)
@@ -86,19 +93,28 @@ __global__ void __launch_bounds__(SP_THREADS) logprob_gather_kernel(const float*
 // inverse CDF over the kept tokens in index order with the caller's uniform u[row] in [0, 1) -- the same distribution as
 // multinomial over the sorted, renormalised vector (order is irrelevant).  Tokens with EQUAL probability at the cut are kept or
 // dropped together, where the reference's unstable sort keeps an arbitrary subset of them.
-__global__ void __launch_bounds__(SP_THREADS) sample_top_p_kernel(const float* __restrict__ logits, const float* __restrict__ uniform,
-                                                                  long long* __restrict__ out, int V, float inv_temperature, float top_p) {
-  const float* row = logits + (int64_t)blockIdx.x * V;
-  __shared__ float scratch[SP_WARPS];
-  __shared__ float warp_mass[SP_WARPS];
+//
+// The pieces are shared with the speculative-sampling acceptance (speculative.cuh), which needs the same nucleus of two rows:
+//   NucleusRow   softmax(row / temperature): the row maximum m and 1/Z, prob(i) = exp(row[i] / T - m) / Z
+//   nucleus_tau  the threshold tau of the kept set {i : prob(i) >= tau}
+//   block_draw   inverse-CDF draw over nonnegative weights w(i) in index order
+struct NucleusRow {
+  const float* row;
+  float inv_temperature, m, inv_z;
+  __device__ __forceinline__ float prob(int i) const { return expf(row[i] * inv_temperature - m) * inv_z; }
+};
+
+__device__ __forceinline__ NucleusRow nucleus_row(const float* __restrict__ row, int V, float inv_temperature, float* scratch) {
   float m = -INFINITY;
   for (int i = threadIdx.x; i < V; i += SP_THREADS) m = fmaxf(m, row[i] * inv_temperature);
   m = block_max(m, scratch);
   float z = 0.f;
   for (int i = threadIdx.x; i < V; i += SP_THREADS) z += expf(row[i] * inv_temperature - m);
   z = block_sum(z, scratch);
-  const float inv_z = 1.0f / z;
-  auto prob = [&](int i) { return expf(row[i] * inv_temperature - m) * inv_z; };
+  return NucleusRow{row, inv_temperature, m, 1.0f / z};
+}
+
+__device__ __forceinline__ float nucleus_tau(const NucleusRow& r, int V, float top_p, float* scratch) {
   // bisection on the bit pattern of tau in (0, 1]: invariant S(hi) <= top_p (S(1.0) = 0), S(lo) > top_p or lo = 0
   unsigned lo = 0u, hi = __float_as_uint(1.0f);
   while (hi - lo > 1u) {
@@ -106,7 +122,7 @@ __global__ void __launch_bounds__(SP_THREADS) sample_top_p_kernel(const float* _
     const float q = __uint_as_float(mid);
     float s = 0.f;
     for (int i = threadIdx.x; i < V; i += SP_THREADS) {
-      const float p = prob(i);
+      const float p = r.prob(i);
       s += p > q ? p : 0.f;
     }
     s = block_sum(s, scratch);
@@ -118,15 +134,19 @@ __global__ void __launch_bounds__(SP_THREADS) sample_top_p_kernel(const float* _
   // kept set: p_i >= tau where tau = the smallest ACTUAL probability > lo's value ... any p in (value(lo), value(hi)] equals
   // value(hi) (adjacent floats), so "p >= value(hi)" is exact.  If even the largest probability alone exceeds top_p the first
   // token is still kept (its preceding mass is 0 <= p), which S(p_max) = 0 <= top_p guarantees here too.
-  const float tau = __uint_as_float(hi);
-  // mass of the kept set, then the draw: thread-contiguous chunks so that a prefix over threads is a prefix over indices
+  return __uint_as_float(hi);
+}
+
+// One draw from the weights w(i) >= 0, i < V: the token where u * sum(w) falls in the prefix sums over index order (u in
+// [0, 1)).  Every thread returns the token.  -1 only when every weight is 0.
+template <typename Weight>
+__device__ __forceinline__ int block_draw(const Weight& weight, int V, float u) {
+  __shared__ float warp_mass[SP_WARPS];
+  // mass of the weights, then the draw: thread-contiguous chunks so that a prefix over threads is a prefix over indices
   const int per = (V + SP_THREADS - 1) / SP_THREADS;
   const int i0 = threadIdx.x * per, i1 = min(V, i0 + per);
   float mine = 0.f;
-  for (int i = i0; i < i1; ++i) {
-    const float p = prob(i);
-    mine += p >= tau ? p : 0.f;
-  }
+  for (int i = i0; i < i1; ++i) mine += weight(i);
   // inclusive scan over threads: within the warp, then over the warps
   float incl = mine;
 #pragma unroll
@@ -157,33 +177,43 @@ __global__ void __launch_bounds__(SP_THREADS) sample_top_p_kernel(const float* _
   __syncthreads();
   const float lower = threadIdx.x ? upper_sm[threadIdx.x - 1] : 0.f;
   total = upper_sm[SP_THREADS - 1];
-  const float target = uniform[blockIdx.x] * total;
+  const float target = u * total;
   if (mine > 0.f && target >= lower && target < upper) atomicMin(&winner_tid, (int)threadIdx.x);
   __syncthreads();
   if ((int)threadIdx.x == winner_tid) {
     float run = lower;
     int pick = -1;
     for (int i = i0; i < i1; ++i) {
-      const float p = prob(i);
-      if (p >= tau) {
-        pick = i;  // last kept token so far: the fallback when rounding pushes the target past the chunk's sum
-        run += p;
+      const float w = weight(i);
+      if (w > 0.f) {
+        pick = i;  // last weighted token so far: the fallback when rounding pushes the target past the chunk's sum
+        run += w;
         if (target < run) break;
       }
     }
     winner = pick;
   }
   __syncthreads();
-  if (threadIdx.x == 0) {
-    if (winner < 0) {  // target == total after rounding: the last kept token overall
-      for (int i = V - 1; i >= 0; --i)
-        if (prob(i) >= tau) {
-          winner = i;
-          break;
-        }
-    }
-    out[blockIdx.x] = winner;
+  if (threadIdx.x == 0 && winner < 0) {  // target == total after rounding: the last weighted token overall
+    for (int i = V - 1; i >= 0; --i)
+      if (weight(i) > 0.f) {
+        winner = i;
+        break;
+      }
   }
+  __syncthreads();
+  const int out = winner;
+  __syncthreads();  // winner may be reused by the caller's next draw
+  return out;
+}
+
+__global__ void __launch_bounds__(SP_THREADS) sample_top_p_kernel(const float* __restrict__ logits, const float* __restrict__ uniform,
+                                                                  long long* __restrict__ out, int V, float inv_temperature, float top_p) {
+  __shared__ float scratch[SP_WARPS];
+  const NucleusRow r = nucleus_row(logits + (int64_t)blockIdx.x * V, V, inv_temperature, scratch);
+  const float tau = nucleus_tau(r, V, top_p, scratch);
+  const int winner = block_draw([&](int i) { const float p = r.prob(i); return p >= tau ? p : 0.f; }, V, uniform[blockIdx.x]);
+  if (threadIdx.x == 0) out[blockIdx.x] = winner;
 }
 
 }  // namespace mb200

@@ -54,8 +54,16 @@ class _PromptPlan:
 
 @torch.inference_mode()
 def generate(encoded_prompts: List[List[int]], model: Transformer, images: List[List] = [], *, max_tokens: int,  # noqa: B006
-             temperature: float, chunk_size: Optional[int] = None, eos_id: Optional[int] = None
-             ) -> Tuple[List[List[int]], List[List[float]]]:
+             temperature: float, chunk_size: Optional[int] = None, eos_id: Optional[int] = None,
+             draft: Optional[Transformer] = None, draft_tokens: int = 4) -> Tuple[List[List[int]], List[List[float]]]:
+    """`draft`: another Transformer with the same vocabulary that proposes `draft_tokens` tokens per round for the model to verify
+    (speculative decoding, mistral_inference_b200/speculative.py).  Same return value and semantics as without it; greedy output
+    stays the model's own argmax choices and sampled output keeps the model's nucleus distribution."""
+    if draft is not None:
+        from .speculative import generate_speculative
+
+        return generate_speculative(encoded_prompts, model, draft, images, max_tokens=max_tokens, temperature=temperature,
+                                    chunk_size=chunk_size, eos_id=eos_id, draft_tokens=draft_tokens)
     # images[b]: the images of prompt b; the model sees all of them, in prompt order (generate.py:54-60,89)
     images_torch: List[List[torch.Tensor]] = []
     if images:

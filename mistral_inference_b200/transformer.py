@@ -530,6 +530,81 @@ class Transformer(nn.Module):
         self._last_static_logits = st["logits"].data_ptr()
         return st["logits"]
 
+    # ------------------------------------------------------------------ speculative decoding: the verify step
+    @torch.inference_mode()
+    def verify_static(self, tokens: torch.Tensor, cache: BufferCache) -> Tuple[torch.Tensor, torch.Tensor]:
+        """One forward of S = tokens.shape[1] tokens for every sequence of `cache` (the verify step of speculative decoding:
+        [last, d_1 .. d_k]), on the chunked-prefill kernels at T = B * S.  Like decode_static, the step state lives on the
+        device: `mb200_spec_meta` builds the metadata block from a device-side position vector, so from the second call per
+        (cache, B, S) on the step is ONE CUDA-graph replay with no host write (the first call runs eagerly, the second captures).
+        Unlike decode_static the positions are not advanced here: the acceptance kernel advances them by what the round keeps,
+        and the caller reports that with `verify_accepted`.  Returns (the static fp32 logits [B * S, V], overwritten by the next
+        step; the device positions [B] int32 the step read)."""
+        B, S = tokens.shape
+        self._check_runnable()
+        self._check_cache(cache)
+        assert self.num_pipeline_ranks == 1, "the verify step runs on a single pipeline stage"
+        seqlens = [S] * B
+        self.workspace(B * S)
+        st = self._decode_state(cache, ("verify", B, S))
+        host = cache._kv_seqlens_host
+        assert host is not None and len(host) == B and min(host) > 0, "verify_static needs a prefilled cache of this batch size"
+        if max(host) + S > ROPE_TABLE_LEN:
+            raise IndexError(f"position {max(host) + S - 1} is out of bounds for the rope table of {ROPE_TABLE_LEN} positions")
+        distinct = sorted(set(cache.cache_sizes))
+        if "meta" not in st:
+            st.update({"graph": None, "warmed": False, "expected": None,
+                       "seqpos": torch.zeros(B, dtype=torch.int32, device=self.device),
+                       "tokens": torch.zeros(B * S, dtype=torch.long, device=self.device),
+                       "meta": torch.zeros(_abi.spec_meta_words(B, S, len(distinct)), dtype=torch.int32, device=self.device),
+                       "logits": torch.empty(B * S, self.vocab_size, dtype=torch.float32, device=self.device)})
+        if st["expected"] != host:  # the cache moved other than by the accepted lengths (or this is the first step)
+            st["seqpos"].copy_(torch.tensor(host, dtype=torch.int32))
+        st["tokens"].copy_(tokens.reshape(-1), non_blocking=True)
+        layout = {"T": B * S, "B": B, "prefill": True, "first_prefill": False, "max_seqlen": S, "windows": distinct}
+        md = cache.metadata_from_block(st["meta"], layout, seqlens)
+
+        def run() -> None:
+            _abi.spec_meta(st["seqpos"], st["meta"], S, distinct)
+            h = self._hidden_no_norm(st["tokens"], seqlens, cache, md)
+            _abi.lm_head(h, self.norm.weight, self.output_weight, st["logits"], self.args.norm_eps, self.workspace(B * S))
+
+        if st["graph"] is None and not st["warmed"]:
+            run()
+            st["warmed"] = True
+        elif st["graph"] is None:
+            g = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(g):
+                run()
+            st["graph"] = g
+            g.replay()
+        else:
+            st["graph"].replay()
+        st["expected"] = None  # valid again once verify_accepted reports what the device positions became
+        self._last_static_logits = 0
+        return st["logits"], st["seqpos"]
+
+    def verify_accepted(self, cache: BufferCache, S: int, device_lens: List[int]) -> None:
+        """After a verify step of S tokens per sequence: the acceptance kernel left `device_lens` in the step's device positions.
+        The next step uploads the host lengths only where they differ (a rewound or frozen sequence)."""
+        st = self._decode_state(cache, ("verify", len(device_lens), S))
+        st["expected"] = list(device_lens)
+
+    @torch.inference_mode()
+    def last_token_logits(self, input_ids: torch.Tensor, seqlens: List[int], cache: BufferCache) -> torch.Tensor:
+        """fp32 logits [B, V] of each sequence's last token of a ragged forward that extends `cache` (the lm head runs on those
+        rows only)."""
+        self._check_runnable()
+        self._check_cache(cache)
+        self._last_static_logits = 0
+        h = self._hidden_no_norm(input_ids, seqlens, cache)
+        cache.update_seqlens(seqlens)
+        last_idx = torch.tensor(seqlens, device=input_ids.device).cumsum(0) - 1
+        logits = torch.empty(len(seqlens), self.vocab_size, dtype=torch.float32, device=h.device)
+        _abi.lm_head(h.index_select(0, last_idx), self.norm.weight, self.output_weight, logits, self.args.norm_eps,
+                     self.workspace(h.shape[0]))
+        return logits
+
     # ------------------------------------------------------------------ generate() support (SURVEY.md N1 / N2)
     def last_argmax_valid_for(self, logits: torch.Tensor) -> bool:
         """True when `last_argmax` is the decode kernel's own argmax of exactly this logits buffer."""
