@@ -108,6 +108,20 @@ __device__ __forceinline__ float warp_max(float v) {
   return v;
 }
 
+// Argmax key of logit v at index idx: the maximum over a row's keys is torch.argmax's answer on every fp32 input
+// (generate.py:156).  High word: an order-preserving map of the value, with -0.0 equal to +0.0 and every NaN one key above +inf
+// (torch treats NaN as the maximum); low word: ~index, so among equal values the smallest index wins.  Shared by the sampling
+// kernels and the megakernel's fused lm-head argmax, which must agree.
+__device__ __forceinline__ unsigned long long argmax_key(float v, int idx) {
+  unsigned u = __float_as_uint(v);
+  if (v != v)
+    u = 0x7f800001u;
+  else if (v == 0.f)
+    u = 0u;
+  u = (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+  return ((unsigned long long)u << 32) | (unsigned)(0x7fffffff - idx);
+}
+
 // Reference numerics helpers ---------------------------------------------------------------------
 // rsqrt as torch's CPU kernel does it: 1 / sqrt(x), both IEEE-rounded (not the 2-ulp rsqrt.approx)
 __device__ __forceinline__ float ref_rsqrt(float x) { return __fdiv_rn(1.0f, __fsqrt_rn(x)); }

@@ -1201,19 +1201,13 @@ __global__ void __launch_bounds__(MK_THREADS, 1) decode_megakernel(const MkParam
 
   // ---- final RMSNorm + lm head (fp32 logits, each a bf16-rounded value) + greedy argmax ----
   stage_x(xs, p.xbuf + (size_t)(p.n_layers & 1) * p.dim, p.final_norm, p.dim, p.eps, red, tid);
-  // argmax key: order-preserving map of the fp32 logit in the high word, ~index in the low word, so that the maximum key is
-  // the largest logit and, among equal logits, the SMALLEST index (what torch.argmax returns; generate.py:156)
+  // the maximum argmax_key (common.cuh) over the row is torch.argmax's answer: among equal logits the SMALLEST index
   unsigned long long best = 0ull;
-  auto key_of = [](float v, int idx) {
-    unsigned u = __float_as_uint(v);
-    u = (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-    return ((unsigned long long)u << 32) | (unsigned)(0x7fffffff - idx);
-  };
   consume_matrix(p.vocab, p.dim, ring, full, empty, p.n_stages, rs, xs, tid, [&](int) { return make_uint2(0u, 0u); },
                  [&](int n, float a0, float a1, uint2) {
                    const float y0 = round_bf16(a0), y1 = round_bf16(a1);
                    *reinterpret_cast<float2*>(p.logits + n) = make_float2(y0, y1);
-                   const unsigned long long k0 = key_of(y0, n), k1 = key_of(y1, n + 1);
+                   const unsigned long long k0 = argmax_key(y0, n), k1 = argmax_key(y1, n + 1);
                    best = max(best, max(k0, k1));
                  });
   if (p.next_token != nullptr) {

@@ -16,14 +16,6 @@ namespace mb200 {
 constexpr int SP_THREADS = 1024;
 constexpr int SP_WARPS = SP_THREADS / 32;
 
-__device__ __forceinline__ unsigned long long argmax_key(float v, int idx) {
-  // order-preserving map of the fp32 value in the high word, ~index in the low word: the maximum key is the largest value
-  // and, among equal values, the smallest index (what torch.argmax returns)
-  unsigned u = __float_as_uint(v);
-  u = (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-  return ((unsigned long long)u << 32) | (unsigned)(0x7fffffff - idx);
-}
-
 // block-wide reductions over SP_THREADS threads; `scratch` holds SP_WARPS values; result broadcast to every thread
 __device__ __forceinline__ float block_sum(float v, float* scratch) {
   v = warp_sum(v);
@@ -163,9 +155,11 @@ __device__ __forceinline__ int block_draw(const Weight& weight, int V, float u) 
     if (w < (int)(threadIdx.x >> 5)) before += wm;
     total += wm;
   }
-  // thread t owns the targets in [upper(t-1), upper(t)); the bounds come from the SAME numbers on both sides of every edge,
-  // and a claim is resolved to the lowest thread, so there is exactly one winner even where rounding makes the prefix
-  // non-monotone by an ulp
+  // the winner is the LOWEST weighted thread with target < upper(t).  Each lane's scan associates its fp32 additions
+  // differently, so a zero-mass thread's upper(t) can exceed its weighted predecessor's by an ulp; a rule that also required
+  // target >= upper(t-1) would leave that interval to nobody.  With this rule every target below the last weighted upper(t) has
+  // exactly one claimant, and the claimant's walk starts at upper(t-1): a target below it takes the thread's first weighted
+  // token, the inverse CDF's neighbour across the ulp.  Only a target past every weighted upper(t) falls through below.
   __shared__ float upper_sm[SP_THREADS];
   __shared__ int winner_tid, winner;
   const float upper = before + incl;
@@ -178,7 +172,7 @@ __device__ __forceinline__ int block_draw(const Weight& weight, int V, float u) 
   const float lower = threadIdx.x ? upper_sm[threadIdx.x - 1] : 0.f;
   total = upper_sm[SP_THREADS - 1];
   const float target = u * total;
-  if (mine > 0.f && target >= lower && target < upper) atomicMin(&winner_tid, (int)threadIdx.x);
+  if (mine > 0.f && target < upper) atomicMin(&winner_tid, (int)threadIdx.x);
   __syncthreads();
   if ((int)threadIdx.x == winner_tid) {
     float run = lower;

@@ -130,7 +130,9 @@ __global__ void __launch_bounds__(SP_THREADS) spec_accept_sample_kernel(const fl
       continue;
     }
     n = j;
-    last = block_draw([&](int i) { return fmaxf(p.at(i) - q.at(i), 0.f); }, V, u[k]);
+    // __fsub_rn: the difference of the two ROUNDED probabilities the acceptance test compared.  A contracted
+    // fma(kept_p, inv_kept_p, -q) leaves the product's rounding error where P == Q, a residual of pure noise.
+    last = block_draw([&](int i) { return fmaxf(__fsub_rn(p.at(i), q.at(i)), 0.f); }, V, u[k]);
     if (last < 0) last = block_draw([&](int i) { return p.kept(i); }, V, u[k]);
     break;
   }
