@@ -359,6 +359,32 @@ int mb200_moe_grouped_ffn_fp8(const void* xs, const void* const* w13_host, const
                               const void* residual, void* g, void* yw, void* out, int64_t T, int64_t dim, int64_t hidden, int64_t n_experts,
                               int64_t top_k, const mb200_moe_comm* comm, void* workspace, size_t workspace_bytes, void* stream);
 
+/* Un-merged LoRA on FP8 experts (LoRALinear on every expert's w1 / w2 / w3, lora.py:71-74).  Each expert Linear [N, K] computes,
+ * on the dequantised W' of the FP8 format above and the rows of the MoE row plan:
+ *   a = bf16(x A_e^T)    L = bf16(a B_e^T)    y = bf16( bf16(x W'_e^T) + bf16(L * scaling) )
+ * for w1 / w3 before SiLU * mul, and for w2 before the routing weight: yw = bf16(w * y).  The combine is unchanged.
+ * mb200_moe_lora: one adapter per expert Linear group, in the packed layout of mb200_lora, whose w13 B rows interleave like w13:
+ *   a_host / b_host  HOST arrays of E device pointers to A [rank_cols, K] and B [N, rank_cols] (bf16); NULL for experts of other
+ *                    ranks, and non-NULL wherever the expert's weights are
+ *   a_buf            [rows_cap, rank_cols] bf16 scratch; l_buf [rows_cap, N] bf16 scratch, 16-byte aligned (it doubles as the fp32
+ *                    split-K partials of the down projection); rows_cap from mb200_moe_sizes.  The two adapters of a call may share
+ *                    their scratch: the w13 stages are done before the w2 stages start.
+ * The down projection a is one launch over the plan's tiles (read on the device: no host sync, graph-replayable), its K split into a
+ * fixed number of slices summed in a fixed order, so every run gives the same bits; L is the bf16 grouped GEMM with K = rank_cols. */
+typedef struct mb200_moe_lora {
+  const void* const* a_host;
+  const void* const* b_host;
+  int64_t rank_cols; /* multiple of 64 */
+  float scaling;     /* args.lora.scaling */
+  void* a_buf;
+  void* l_buf;
+} mb200_moe_lora;
+int mb200_moe_grouped_ffn_fp8_lora(const void* xs, const void* const* w13_host, const float* const* w13_scale_host, const void* const* w2_host,
+                                   const float* const* w2_scale_host, const int32_t* plan, const void* row_w, const int32_t* slot,
+                                   const void* residual, void* g, void* yw, void* out, int64_t T, int64_t dim, int64_t hidden,
+                                   int64_t n_experts, int64_t top_k, const mb200_moe_comm* comm, void* workspace, size_t workspace_bytes,
+                                   void* stream, const mb200_moe_lora* lora13, const mb200_moe_lora* lora2);
+
 /* INT4 expert weights: the INT4 format of the dense Linears (see mb200_quantize_int4_groups below) applied to every expert matrix;
  * each expert's w1 / w3 fill the interleaved w13 rows (row 2i = w1[i], row 2i + 1 = w3[i]) through the quantiser's row strides.
  * mb200_moe_grouped_ffn_int4: mb200_moe_grouped_ffn with INT4 experts: w13_host / w2_host are HOST arrays of E device pointers to

@@ -68,6 +68,9 @@ _SIGNATURES = {
     "mb200_quantize_e4m3_rows": (c_int, [c_void_p, c_int64, c_int64, c_void_p, c_int64, c_void_p, c_int64, c_void_p]),
     "mb200_moe_grouped_ffn_fp8": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                           c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int64, c_int64, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "mb200_moe_grouped_ffn_fp8_lora": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                               c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int64, c_int64, c_void_p, c_void_p,
+                                               c_size_t, c_void_p, c_void_p, c_void_p]),
     "mb200_moe_grouped_ffn_int4": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                            c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int64, c_int64, c_void_p, c_void_p, c_size_t, c_void_p]),
     "mb200_comm_alloc": (c_int, [c_size_t, ctypes.POINTER(c_void_p)]),
@@ -162,16 +165,16 @@ class Workspace:
         self._moe: dict = {}
         self._comm = None
 
-    def moe_buffers(self, T: int, dim: int, hidden: int, E: int, k: int, dtype: torch.dtype, comm=None, parity: int = 0):
+    def moe_buffers(self, T: int, dim: int, hidden: int, E: int, k: int, dtype: torch.dtype, comm=None, parity: int = 0, lora_cols: int = 0):
         from .moe import MoeBuffers
 
-        key = (T, dim, hidden, E, k, parity if comm is not None else 0, id(comm))
+        key = (T, dim, hidden, E, k, parity if comm is not None else 0, id(comm), lora_cols)
         b = self._moe.get(key)
         if b is None:
             if len(self._moe) >= 8:  # prompt chunks of many different lengths: keep the pool small
                 self._moe.clear()
             yw_ptr = comm.yw_ptr(parity) if comm is not None else None
-            b = self._moe[key] = MoeBuffers(T, dim, hidden, E, k, self.buf.device, dtype, yw_ptr=yw_ptr)
+            b = self._moe[key] = MoeBuffers(T, dim, hidden, E, k, self.buf.device, dtype, yw_ptr=yw_ptr, lora_cols=lora_cols)
         return b
 
     def expert_comm(self, layer, T: int, dim: int):
@@ -532,6 +535,30 @@ def moe_grouped_ffn_fp8(b, w13_host, s13_host, w2_host, s2_host, residual: Optio
                                            _ptr(b.slot), _ptr(residual), _ptr(b.g), b.yw_ptr, _ptr(out), T, dim, hidden, E, k,
                                            ctypes.cast(ctypes.pointer(comm), c_void_p) if comm is not None else None, ws.ptr, ws.nbytes,
                                            _stream()), "mb200_moe_grouped_ffn_fp8")
+
+
+class MoeLoraStruct(ctypes.Structure):
+    """mb200_moe_lora (include/mistral_b200.h)."""
+    _fields_ = [("a_host", c_void_p), ("b_host", c_void_p), ("rank_cols", c_int64), ("scaling", c_float), ("a_buf", c_void_p), ("l_buf", c_void_p)]
+
+
+def moe_lora_struct(a_host, b_host, rank_cols: int, scaling: float, a_buf: torch.Tensor, l_buf: torch.Tensor) -> MoeLoraStruct:
+    """The adapters of one grouped expert Linear: host arrays of E device pointers to A [R, K] and B [N, R], and the MoE scratch
+    a_buf [>= rows_cap, R], l_buf [>= rows_cap, N] (bf16)."""
+    assert a_buf.shape[-1] == rank_cols and rank_cols % 64 == 0
+    return MoeLoraStruct(ctypes.cast(a_host, c_void_p), ctypes.cast(b_host, c_void_p), rank_cols, scaling, _ptr(a_buf), _ptr(l_buf))
+
+
+def moe_grouped_ffn_fp8_lora(b, w13_host, s13_host, w2_host, s2_host, residual: Optional[torch.Tensor], out: torch.Tensor, T: int, dim: int,
+                             hidden: int, E: int, k: int, comm: Optional[MoeCommStruct], ws: "Workspace", lora13: MoeLoraStruct,
+                             lora2: MoeLoraStruct) -> None:
+    """moe_grouped_ffn_fp8 with the un-merged adapters of every expert's w1 / w3 (`lora13`) and w2 (`lora2`)."""
+    _check(lib().mb200_moe_grouped_ffn_fp8_lora(_ptr(b.xs), ctypes.cast(w13_host, c_void_p), ctypes.cast(s13_host, c_void_p),
+                                                ctypes.cast(w2_host, c_void_p), ctypes.cast(s2_host, c_void_p), _ptr(b.plan), _ptr(b.row_w),
+                                                _ptr(b.slot), _ptr(residual), _ptr(b.g), b.yw_ptr, _ptr(out), T, dim, hidden, E, k,
+                                                ctypes.cast(ctypes.pointer(comm), c_void_p) if comm is not None else None, ws.ptr, ws.nbytes,
+                                                _stream(), ctypes.cast(ctypes.pointer(lora13), c_void_p),
+                                                ctypes.cast(ctypes.pointer(lora2), c_void_p)), "mb200_moe_grouped_ffn_fp8_lora")
 
 
 def moe_grouped_ffn_int4(b, w13_host, s13_host, w2_host, s2_host, residual: Optional[torch.Tensor], out: torch.Tensor, T: int, dim: int,

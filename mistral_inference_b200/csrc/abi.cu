@@ -854,13 +854,40 @@ int mb200_moe_route(const void* hn, const void* gate_w, int64_t T, int64_t dim, 
   return MB200_OK;
 }
 
+// The un-merged LoRA stages of one grouped expert Linear [N, K] (include/mistral_b200.h): a = bf16(x A_e^T) over the plan's rows
+// (l_buf doubles as the split partials), then L = bf16(a B_e^T) with the bf16 grouped GEMM (K = rank_cols).  The base GEMM's
+// EPI_LORA epilogue adds bf16(L * scaling): `epi` gets those fields.
+static int moe_lora_stages(const void* x, const mb200_moe_lora* l, const void* const* w_host, int E, int64_t rows_cap, int64_t K, int64_t N,
+                           int est, int tile_rows, const int32_t* plan, EpiParams* epi, void* workspace, size_t workspace_bytes, cudaStream_t st) {
+  MB_CHECK_ARG(l->a_host && l->b_host && l->a_buf && l->l_buf, "moe lora: null pointer");
+  MB_CHECK_ARG(l->rank_cols >= 64 && l->rank_cols % 64 == 0, "moe lora: rank_cols=%lld must be a multiple of 64", (long long)l->rank_cols);
+  MB_CHECK_ARG(((uintptr_t)l->a_buf & 15) == 0 && ((uintptr_t)l->l_buf & 15) == 0,
+               "moe lora: a_buf and l_buf must be 16-byte aligned (l_buf doubles as fp32 split-K scratch)");
+  for (int e = 0; e < E; ++e)
+    MB_CHECK_ARG(w_host[e] == nullptr || (l->a_host[e] != nullptr && l->b_host[e] != nullptr), "moe lora: expert %d has weights but no adapter", e);
+  int rc = launch_lora_down_grouped(x, l->a_host, E, plan, tile_rows, est, l->a_buf, rows_cap, l->rank_cols, K, l->l_buf, (size_t)rows_cap * N * 2, st);
+  if (rc) return rc;
+  EpiParams up;
+  up.out = l->l_buf;
+  up.ld_out = N;
+  rc = launch_grouped<EPI_STORE>(l->a_buf, rows_cap, l->rank_cols, N, l->b_host, E, est, tile_rows, plan, up, workspace, workspace_bytes, st,
+                                 MoeFmt::BF16, nullptr);
+  if (rc) return rc;
+  epi->lora_l = l->l_buf;
+  epi->ld_lora = N;
+  epi->lora_scaling = l->scaling;
+  return MB200_OK;
+}
+
 // s13 / s2: NULL for bf16 experts; the host arrays of per-row fp32 scale pointers next to e4m3 weights (FP8), or of bf16 group-scale
-// pointers next to INT4 codes
+// pointers next to INT4 codes.  l13 / l2: the un-merged adapters of FP8 experts, or NULL.
 static int moe_grouped_ffn(const void* xs, const void* const* w13_host, const void* const* w2_host, MoeFmt fmt, const void* const* s13_host,
                            const void* const* s2_host, const int32_t* plan, const void* row_w, const int32_t* slot, const void* residual, void* g,
                            void* yw, void* out, int64_t T, int64_t dim, int64_t hidden, int64_t n_experts, int64_t top_k, const mb200_moe_comm* comm,
-                           void* workspace, size_t workspace_bytes, void* stream) {
+                           void* workspace, size_t workspace_bytes, void* stream, const mb200_moe_lora* l13 = nullptr,
+                           const mb200_moe_lora* l2 = nullptr) {
   MB_CHECK_ARG(xs && w13_host && w2_host && plan && row_w && slot && g && yw && out, "moe_grouped_ffn: null pointer");
+  MB_CHECK_ARG((l13 == nullptr) == (l2 == nullptr) && (l13 == nullptr || fmt == MoeFmt::FP8), "moe_grouped_ffn: adapters need FP8 experts, both of them");
   MB_CHECK_ARG(T >= 1 && top_k >= 1 && top_k <= MOE_MAX_TOPK && n_experts <= MOE_MAX_EXPERTS && dim % 64 == 0 && hidden % 64 == 0,
                "moe_grouped_ffn: T=%lld k=%lld E=%lld dim=%lld hidden=%lld", (long long)T, (long long)top_k, (long long)n_experts, (long long)dim,
                (long long)hidden);
@@ -882,8 +909,16 @@ static int moe_grouped_ffn(const void* xs, const void* const* w13_host, const vo
   EpiParams e1;
   e1.out = g;
   e1.ld_out = hidden;
-  int rc = launch_grouped<EPI_SWIGLU>(xs, rows_cap, dim, 2 * hidden, w13_host, (int)n_experts, est, tile_rows, plan, e1, workspace, workspace_bytes, st,
-                                      fmt, s13_host);
+  int rc;
+  if (l13) {
+    rc = moe_lora_stages(xs, l13, w13_host, (int)n_experts, rows_cap, dim, 2 * hidden, est, tile_rows, plan, &e1, workspace, workspace_bytes, st);
+    if (rc) return rc;
+    rc = launch_grouped<EPI_SWIGLU | EPI_LORA>(xs, rows_cap, dim, 2 * hidden, w13_host, (int)n_experts, est, tile_rows, plan, e1, workspace,
+                                               workspace_bytes, st, fmt, s13_host);
+  } else {
+    rc = launch_grouped<EPI_SWIGLU>(xs, rows_cap, dim, 2 * hidden, w13_host, (int)n_experts, est, tile_rows, plan, e1, workspace, workspace_bytes, st,
+                                    fmt, s13_host);
+  }
   if (rc) return rc;
   EpiParams e2;
   e2.out = yw;
@@ -894,8 +929,15 @@ static int moe_grouped_ffn(const void* xs, const void* const* w13_host, const vo
     MB_CHECK_ARG(comm->peer_yw[r] != nullptr, "moe_grouped_ffn: peer buffer %d missing", r);
     e2.peer_out[r] = comm->peer_yw[r];
   }
-  rc = launch_grouped<EPI_MOE_SCALE>(g, rows_cap, hidden, dim, w2_host, (int)n_experts, est, tile_rows, plan, e2, workspace, workspace_bytes, st,
-                                     fmt, s2_host);
+  if (l2) {
+    rc = moe_lora_stages(g, l2, w2_host, (int)n_experts, rows_cap, hidden, dim, est, tile_rows, plan, &e2, workspace, workspace_bytes, st);
+    if (rc) return rc;
+    rc = launch_grouped<EPI_MOE_SCALE | EPI_LORA>(g, rows_cap, hidden, dim, w2_host, (int)n_experts, est, tile_rows, plan, e2, workspace,
+                                                  workspace_bytes, st, fmt, s2_host);
+  } else {
+    rc = launch_grouped<EPI_MOE_SCALE>(g, rows_cap, hidden, dim, w2_host, (int)n_experts, est, tile_rows, plan, e2, workspace, workspace_bytes, st,
+                                       fmt, s2_host);
+  }
   if (rc) return rc;
   MoeCombineParams c;
   c.yw = (const uint4*)yw;
@@ -942,6 +984,18 @@ int mb200_moe_grouped_ffn_fp8(const void* xs, const void* const* w13_host, const
   return moe_grouped_ffn(xs, w13_host, w2_host, MoeFmt::FP8, reinterpret_cast<const void* const*>(w13_scale_host),
                          reinterpret_cast<const void* const*>(w2_scale_host), plan, row_w, slot, residual, g, yw, out, T, dim, hidden, n_experts,
                          top_k, comm, workspace, workspace_bytes, stream);
+}
+
+int mb200_moe_grouped_ffn_fp8_lora(const void* xs, const void* const* w13_host, const float* const* w13_scale_host, const void* const* w2_host,
+                                   const float* const* w2_scale_host, const int32_t* plan, const void* row_w, const int32_t* slot, const void* residual,
+                                   void* g, void* yw, void* out, int64_t T, int64_t dim, int64_t hidden, int64_t n_experts, int64_t top_k,
+                                   const mb200_moe_comm* comm, void* workspace, size_t workspace_bytes, void* stream, const mb200_moe_lora* lora13,
+                                   const mb200_moe_lora* lora2) {
+  MB_CHECK_ARG(w13_scale_host && w2_scale_host, "moe_grouped_ffn_fp8_lora: null scale table");
+  MB_CHECK_ARG(lora13 && lora2, "moe_grouped_ffn_fp8_lora: null adapter");
+  return moe_grouped_ffn(xs, w13_host, w2_host, MoeFmt::FP8, reinterpret_cast<const void* const*>(w13_scale_host),
+                         reinterpret_cast<const void* const*>(w2_scale_host), plan, row_w, slot, residual, g, yw, out, T, dim, hidden, n_experts,
+                         top_k, comm, workspace, workspace_bytes, stream, lora13, lora2);
 }
 
 int mb200_moe_grouped_ffn_int4(const void* xs, const void* const* w13_host, const void* const* w13_gscale_host, const void* const* w2_host,

@@ -18,9 +18,10 @@ enum EpiMode : int {
   EPI_BIAS = 6,      // out[t, n] = bf16(acc + bias[n]) (bias may be null: bf16(acc))  nn.Linear(bias=True) (vision_encoder.py:108,114)
   EPI_BIAS_GELU = 7, // out[t, n] = bf16( gelu_erf( bf16(acc + bias[n]) ) )           nn.GELU() after w_in (vision_encoder.py:117)
 };
-// Flag OR-ed into EPI_STORE / EPI_RESIDUAL / EPI_SWIGLU / EPI_QKV_ROPE: the un-merged LoRA combine (LoRALinear.forward,
-// lora.py:71-74) runs on the Linear's bf16 output before the mode's own work:
+// Flag OR-ed into EPI_STORE / EPI_RESIDUAL / EPI_SWIGLU / EPI_QKV_ROPE / EPI_MOE_SCALE: the un-merged LoRA combine
+// (LoRALinear.forward, lora.py:71-74) runs on the Linear's bf16 output before the mode's own work:
 //   y = bf16(y + bf16(L[t, n] * scaling))     L = the adapter's up-projection output, bf16 [T, ld_lora]
+// (EPI_MOE_SCALE: t is the expert row, so the routing weight and the expert-parallel peer stores take the combined value.)
 // Instantiations without the flag compile to the same code as before.
 constexpr int EPI_LORA = 16;
 // Flag OR-ed into EPI_STORE / EPI_RESIDUAL / EPI_SWIGLU / EPI_QKV_ROPE: FP8 dense weights (include/mistral_b200.h).  The
@@ -74,7 +75,8 @@ __device__ __forceinline__ void epi_pair(const EpiParams& p, int t, int n, float
   // the Linear's own output rounding (bf16 result of nn.Linear)
   float y0 = round_bf16(acc0), y1 = round_bf16(acc1);
   if constexpr ((FLAGS & EPI_LORA) != 0) {
-    static_assert(MODE == EPI_STORE || MODE == EPI_RESIDUAL || MODE == EPI_SWIGLU || MODE == EPI_QKV_ROPE, "LoRA combine: unsupported mode");
+    static_assert(MODE == EPI_STORE || MODE == EPI_RESIDUAL || MODE == EPI_SWIGLU || MODE == EPI_QKV_ROPE || MODE == EPI_MOE_SCALE,
+                  "LoRA combine: unsupported mode");
     const uint32_t l = *reinterpret_cast<const uint32_t*>(reinterpret_cast<const uint16_t*>(p.lora_l) + (int64_t)t * p.ld_lora + n);
     y0 = round_bf16(y0 + round_bf16(bf16lo(l) * p.lora_scaling));
     y1 = round_bf16(y1 + round_bf16(bf16hi(l) * p.lora_scaling));

@@ -9,8 +9,15 @@
 // 8 warps as 4 (rows) x 2 (columns), warp tile 32 x 32.
 // The up-projection  L = bf16(a * B^T)  is an ordinary GEMM (run_linear<EPI_STORE>, K = R) and the combine is the EPI_LORA
 // stage of epilogue.cuh.
+// GROUPED (the experts of a MoE layer, moe.cuh): the rows are the expert-sorted rows of the MoE row plan, and m tile y is the
+// plan's tile y -- expert tile_expert[y], rows [tile_row0[y], tile_row0[y] + tile_rows), read on the device, so the launch needs no
+// host sync and replays in a graph.  The grid covers the plan's tile capacity; CTAs past plan[0] exit.  A 32- or 64-row plan
+// tile leaves the rest of the 128-row CTA tile zero-filled and unstored.
 #pragma once
+#include <type_traits>
+
 #include "gemm_mma.cuh"
+#include "gemm_wgmma.cuh"
 
 namespace mb200 {
 
@@ -26,18 +33,38 @@ struct LoraDownParams {
   float* partial;   // [S, T, R] fp32 (splits > 1)
   int T, R, K, splits;
 };
+// GROUPED: T is the plan's row capacity; a_e[e] is expert e's A [R, K] (null for experts of other ranks, never in the plan).  A
+// separate type, so that the dense kernel's parameters (and code) stay as they are.
+struct LoraDownGroupedParams : LoraDownParams {
+  const int32_t* plan;
+  int tile_rows;
+  const bf16* a_e[MOE_MAX_EXPERTS];
+};
+template <bool GROUPED>
+using LoraDownArgs = std::conditional_t<GROUPED, LoraDownGroupedParams, LoraDownParams>;
 
-__global__ void __launch_bounds__(LD_THREADS, 2) lora_down_kernel(const LoraDownParams p) {
+template <bool GROUPED>
+__global__ void __launch_bounds__(LD_THREADS, 2) lora_down_kernel(const LoraDownArgs<GROUPED> p) {
   extern __shared__ __align__(128) uint8_t smem[];
   const uint32_t smem_base = (uint32_t)__cvta_generic_to_shared(smem);
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int wm = warp >> 1, wn = warp & 1;
-  const int m0 = blockIdx.y * LD_BM, n0 = blockIdx.x * LD_BN, split = blockIdx.z;
+  int m0 = blockIdx.y * LD_BM;
+  const int n0 = blockIdx.x * LD_BN, split = blockIdx.z;
   const int nk_all = p.K / LD_BK;
   const int kb0 = (int)((int64_t)split * nk_all / p.splits), kb1 = (int)((int64_t)(split + 1) * nk_all / p.splits);
   const int nk = kb1 - kb0;
   pdl_trigger();
-  pdl_wait();  // x is the preceding kernel's output, and the partials may reuse memory it read
+  pdl_wait();  // x (and the plan) are the preceding kernels' output, and the partials may reuse memory they read
+  int m_end = p.T;
+  const bf16* a_w = p.a_w;
+  if constexpr (GROUPED) {
+    if ((int)blockIdx.y >= p.plan[0]) return;
+    const int cap = p.plan[2];
+    a_w = p.a_e[p.plan[MOE_PLAN_HEADER + blockIdx.y]];
+    m0 = p.plan[MOE_PLAN_HEADER + cap + blockIdx.y];
+    m_end = min(m0 + p.tile_rows, p.T);
+  }
 
   auto load_stage = [&](int stage, int kt) {
     const uint32_t sa = smem_base + stage * LD_STAGE_BYTES;
@@ -48,14 +75,14 @@ __global__ void __launch_bounds__(LD_THREADS, 2) lora_down_kernel(const LoraDown
       const int idx = tid + i * LD_THREADS;
       const int row = idx >> 3, chunk = idx & 7;
       const int gm = m0 + row;
-      const bool ok = gm < p.T;
+      const bool ok = gm < m_end;
       cp_async16(sa + swz(row, chunk), p.x + (int64_t)(ok ? gm : 0) * p.K + k0 + chunk * 8, ok);
     }
 #pragma unroll
     for (int i = 0; i < (LD_BN * 8) / LD_THREADS; ++i) {
       const int idx = tid + i * LD_THREADS;
       const int row = idx >> 3, chunk = idx & 7;
-      cp_async16(sb + swz(row, chunk), p.a_w + (int64_t)(n0 + row) * p.K + k0 + chunk * 8, true);
+      cp_async16(sb + swz(row, chunk), a_w + (int64_t)(n0 + row) * p.K + k0 + chunk * 8, true);
     }
   };
 
@@ -113,7 +140,7 @@ __global__ void __launch_bounds__(LD_THREADS, 2) lora_down_kernel(const LoraDown
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         const int r = r0 + 8 * h;
-        if (r >= p.T) continue;
+        if (r >= m_end) continue;
         if (p.splits == 1) {
           *reinterpret_cast<uint32_t*>(p.out + (int64_t)r * p.R + n) = pack_bf16x2(acc[i][j][2 * h], acc[i][j][2 * h + 1]);
         } else {
@@ -140,9 +167,9 @@ __global__ void __launch_bounds__(256) lora_down_reduce_kernel(const float4* __r
   out[i] = make_uint2(pack_bf16x2(s.x, s.y), pack_bf16x2(s.z, s.w));
 }
 
-// K splits: enough CTAs for two per SM, at least 4 k-blocks per split, and partials that fit the caller's scratch.
-inline int lora_down_splits(int64_t T, int64_t R, int64_t K, size_t scratch_bytes, int sms) {
-  const int64_t tiles = (R / LD_BN) * ceil_div(T, LD_BM);
+// K splits: enough CTAs for two per SM over `tiles` output tiles, at least 4 k-blocks per split, and partials [S, T, R] that fit
+// the caller's scratch.
+inline int lora_down_splits(int64_t tiles, int64_t T, int64_t R, int64_t K, size_t scratch_bytes, int sms) {
   int64_t s = (2 * sms + tiles - 1) / tiles;
   const int64_t by_k = (K / LD_BK) / 4, by_scratch = (int64_t)(scratch_bytes / ((size_t)T * R * sizeof(float)));
   if (s > by_k) s = by_k;
@@ -151,14 +178,31 @@ inline int lora_down_splits(int64_t T, int64_t R, int64_t K, size_t scratch_byte
   return s < 1 ? 1 : (int)s;
 }
 
+// The split partials [S, T, R] -> out [T, R]: the fixed-order sum of lora_down_reduce_kernel (T = the plan's row capacity when grouped:
+// rows no plan tile covers sum stale partials into rows nothing reads).
+inline int launch_lora_down_reduce(const void* scratch, void* out, int64_t T, int64_t R, int splits, cudaStream_t stream) {
+  const int64_t n4 = T * R / 4;
+  MB_CHECK_CUDA(launch_pdl(lora_down_reduce_kernel, dim3((unsigned)ceil_div(n4, 256)), dim3(256), 0, stream, (const float4*)scratch, (uint2*)out,
+                           n4, splits));
+  note_launch("lora_down_reduce_kernel");
+  MB_CHECK_LAUNCH("lora_down_reduce_kernel");
+  return MB200_OK;
+}
+
+inline int lora_down_sms(int* sms) {
+  int dev = 0;
+  MB_CHECK_CUDA(cudaGetDevice(&dev));
+  MB_CHECK_CUDA(cudaDeviceGetAttribute(sms, cudaDevAttrMultiProcessorCount, dev));
+  return MB200_OK;
+}
+
 // x [T, K] (already normed), a_w [R, K] -> out [T, R]; `scratch` (scratch_bytes, 16-byte aligned) holds the split partials.
 // Both kernels go through launch_pdl: their launch overlaps the predecessor's tail and they wait for it before touching memory.
 inline int launch_lora_down(const void* x, const void* a_w, void* out, int64_t T, int64_t R, int64_t K, void* scratch, size_t scratch_bytes,
                             cudaStream_t stream) {
   MB_CHECK_ARG(K % LD_BK == 0 && R % LD_BN == 0, "lora down: K=%lld and R=%lld must be multiples of 64", (long long)K, (long long)R);
-  int dev = 0, sms = 0;
-  MB_CHECK_CUDA(cudaGetDevice(&dev));
-  MB_CHECK_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  int sms = 0;
+  if (const int rc = lora_down_sms(&sms)) return rc;
   LoraDownParams p;
   p.x = (const bf16*)x;
   p.a_w = (const bf16*)a_w;
@@ -167,20 +211,42 @@ inline int launch_lora_down(const void* x, const void* a_w, void* out, int64_t T
   p.T = (int)T;
   p.R = (int)R;
   p.K = (int)K;
-  p.splits = lora_down_splits(T, R, K, scratch_bytes, sms);
-  MB_CHECK_CUDA(cudaFuncSetAttribute(lora_down_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, LD_SMEM));
-  MB_CHECK_CUDA(launch_pdl(lora_down_kernel, dim3((unsigned)(R / LD_BN), (unsigned)ceil_div(T, LD_BM), (unsigned)p.splits), dim3(LD_THREADS),
+  p.splits = lora_down_splits((R / LD_BN) * ceil_div(T, LD_BM), T, R, K, scratch_bytes, sms);
+  MB_CHECK_CUDA(cudaFuncSetAttribute(lora_down_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, LD_SMEM));
+  MB_CHECK_CUDA(launch_pdl(lora_down_kernel<false>, dim3((unsigned)(R / LD_BN), (unsigned)ceil_div(T, LD_BM), (unsigned)p.splits), dim3(LD_THREADS),
                            (size_t)LD_SMEM, stream, p));
   note_launch("lora_down_kernel<%d>", p.splits);
   MB_CHECK_LAUNCH("lora_down_kernel");
-  if (p.splits > 1) {
-    const int64_t n4 = T * R / 4;
-    MB_CHECK_CUDA(launch_pdl(lora_down_reduce_kernel, dim3((unsigned)ceil_div(n4, 256)), dim3(256), 0, stream, (const float4*)scratch,
-                             (uint2*)out, n4, p.splits));
-    note_launch("lora_down_reduce_kernel");
-    MB_CHECK_LAUNCH("lora_down_reduce_kernel");
-  }
-  return MB200_OK;
+  return p.splits > 1 ? launch_lora_down_reduce(scratch, out, T, R, p.splits, stream) : MB200_OK;
+}
+
+// Grouped (MoE experts): xs [rows_cap, K] in the plan's row order, a_host[e] expert e's A [R, K] -> out [rows_cap, R].  The split
+// count is sized for `est_mtiles` busy plan tiles (the grouped GEMMs' estimate), so a decode-sized call with one short tile per
+// touched expert still puts two CTAs on every SM; it depends on the shape only, so the bits do too.
+inline int launch_lora_down_grouped(const void* xs, const void* const* a_host, int E, const int32_t* plan, int tile_rows, int est_mtiles, void* out,
+                                    int64_t rows_cap, int64_t R, int64_t K, void* scratch, size_t scratch_bytes, cudaStream_t stream) {
+  MB_CHECK_ARG(K % LD_BK == 0 && R % LD_BN == 0, "lora down (grouped): K=%lld and R=%lld must be multiples of 64", (long long)K, (long long)R);
+  MB_CHECK_ARG(E >= 1 && E <= MOE_MAX_EXPERTS && rows_cap % tile_rows == 0 && tile_rows <= LD_BM, "lora down (grouped): E=%d rows_cap=%lld tile_rows=%d",
+               E, (long long)rows_cap, tile_rows);
+  int sms = 0;
+  if (const int rc = lora_down_sms(&sms)) return rc;
+  LoraDownGroupedParams p = {};
+  p.x = (const bf16*)xs;
+  p.out = (bf16*)out;
+  p.partial = (float*)scratch;
+  p.T = (int)rows_cap;
+  p.R = (int)R;
+  p.K = (int)K;
+  p.plan = plan;
+  p.tile_rows = tile_rows;
+  for (int e = 0; e < E; ++e) p.a_e[e] = (const bf16*)a_host[e];
+  p.splits = lora_down_splits((R / LD_BN) * (est_mtiles < 1 ? 1 : est_mtiles), rows_cap, R, K, scratch_bytes, sms);
+  MB_CHECK_CUDA(cudaFuncSetAttribute(lora_down_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, LD_SMEM));
+  MB_CHECK_CUDA(launch_pdl(lora_down_kernel<true>, dim3((unsigned)(R / LD_BN), (unsigned)(rows_cap / tile_rows), (unsigned)p.splits),
+                           dim3(LD_THREADS), (size_t)LD_SMEM, stream, p));
+  note_launch("lora_down_grouped_kernel<%d>", p.splits);
+  MB_CHECK_LAUNCH("lora_down_grouped_kernel");
+  return p.splits > 1 ? launch_lora_down_reduce(scratch, out, rows_cap, R, p.splits, stream) : MB200_OK;
 }
 
 }  // namespace mb200

@@ -392,6 +392,13 @@ inline int64_t moe_row_cap(int64_t pairs, int64_t E, int tile_rows) { return moe
 // Weight format of a grouped call's experts.  FP8: `scales` holds E per-row fp32 scale arrays; INT4: E bf16 group-scale arrays.
 enum class MoeFmt { BF16, FP8, INT4 };
 
+// The weight formats a grouped MODE is built for.  The un-merged LoRA stages of FP8 experts add two: the up-projection (EPI_STORE)
+// reads bf16 B tables, and the LoRA-combining base GEMMs (EPI_LORA) read e4m3 experts.  Every other mode is built for all three.
+template <int MODE>
+constexpr bool grouped_fmt_built(MoeFmt f) {
+  return MODE == EPI_STORE ? f == MoeFmt::BF16 : ((MODE & EPI_LORA) != 0 ? f == MoeFmt::FP8 : true);
+}
+
 // Tensor maps of the experts' weights (bf16, e4m3, or INT4 codes with boxes of int4_box_bytes) and their scale tables; an expert
 // of another rank (NULL) gets a placeholder that this rank's tiles never reference.
 inline int moe_weight_maps(MoeWeightMaps* maps, MoeWeightScales* sc, MoeWeightGroupScales* gsc, const CUtensorMap& placeholder,
@@ -438,45 +445,53 @@ int launch_grouped_bn(const void* a, int64_t rows_cap, int64_t K, int64_t N, con
   p.N = (int)N;
   p.K = (int)K;
   p.epi = epi;
-  if (fmt == MoeFmt::FP8) {
-    using Cfg8 = TgCfg<BN, TA, true>;
-    MB_CHECK_CUDA(cudaFuncSetAttribute(gemm_wgmma_grouped_fp8_kernel<MODE, BN, TA>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg8::kSmem));
-    gemm_wgmma_grouped_fp8_kernel<MODE, BN, TA><<<sms, Cfg8::kThreads, Cfg8::kSmem, stream>>>(map_a, maps, sc, p, plan);
-    MB_CHECK_LAUNCH("gemm_wgmma_grouped_fp8_kernel");
-    note_launch("gemm_wgmma_grouped_fp8_kernel<%d, 1, %d, %d>", MODE, BN, TA);
-    return MB200_OK;
+  if constexpr (grouped_fmt_built<MODE>(MoeFmt::FP8)) {
+    if (fmt == MoeFmt::FP8) {
+      using Cfg8 = TgCfg<BN, TA, true>;
+      MB_CHECK_CUDA(cudaFuncSetAttribute(gemm_wgmma_grouped_fp8_kernel<MODE, BN, TA>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg8::kSmem));
+      gemm_wgmma_grouped_fp8_kernel<MODE, BN, TA><<<sms, Cfg8::kThreads, Cfg8::kSmem, stream>>>(map_a, maps, sc, p, plan);
+      MB_CHECK_LAUNCH("gemm_wgmma_grouped_fp8_kernel");
+      note_launch("gemm_wgmma_grouped_fp8_kernel<%d, 1, %d, %d>", MODE, BN, TA);
+      return MB200_OK;
+    }
   }
-  if (fmt == MoeFmt::INT4) {
-    using Cfg4 = TgCfg<BN, TA, false, true>;
-    MB_CHECK_CUDA(cudaFuncSetAttribute(gemm_wgmma_grouped_int4_kernel<MODE, BN, TA>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg4::kSmem));
-    gemm_wgmma_grouped_int4_kernel<MODE, BN, TA><<<sms, Cfg4::kThreads, Cfg4::kSmem, stream>>>(map_a, maps, gsc, p, plan);
-    MB_CHECK_LAUNCH("gemm_wgmma_grouped_int4_kernel");
-    note_launch("gemm_wgmma_grouped_int4_kernel<%d, %d, %d>", MODE, BN, TA);
-    return MB200_OK;
+  if constexpr (grouped_fmt_built<MODE>(MoeFmt::INT4)) {
+    if (fmt == MoeFmt::INT4) {
+      using Cfg4 = TgCfg<BN, TA, false, true>;
+      MB_CHECK_CUDA(cudaFuncSetAttribute(gemm_wgmma_grouped_int4_kernel<MODE, BN, TA>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg4::kSmem));
+      gemm_wgmma_grouped_int4_kernel<MODE, BN, TA><<<sms, Cfg4::kThreads, Cfg4::kSmem, stream>>>(map_a, maps, gsc, p, plan);
+      MB_CHECK_LAUNCH("gemm_wgmma_grouped_int4_kernel");
+      note_launch("gemm_wgmma_grouped_int4_kernel<%d, %d, %d>", MODE, BN, TA);
+      return MB200_OK;
+    }
   }
-  MB_CHECK_CUDA(cudaFuncSetAttribute(gemm_wgmma_grouped_kernel<MODE, CL, BN, TA>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmem));
-  if (CL == 1) {
-    gemm_wgmma_grouped_kernel<MODE, CL, BN, TA><<<sms, Cfg::kThreads, Cfg::kSmem, stream>>>(map_a, maps, p, plan);
-    MB_CHECK_LAUNCH("gemm_wgmma_grouped_kernel");
+  if constexpr (!grouped_fmt_built<MODE>(MoeFmt::BF16)) {
+    return fail(MB200_E_INVALID, "grouped gemm: epilogue mode %d has no variant for these weights", MODE);
+  } else {
+    MB_CHECK_CUDA(cudaFuncSetAttribute(gemm_wgmma_grouped_kernel<MODE, CL, BN, TA>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmem));
+    if (CL == 1) {
+      gemm_wgmma_grouped_kernel<MODE, CL, BN, TA><<<sms, Cfg::kThreads, Cfg::kSmem, stream>>>(map_a, maps, p, plan);
+      MB_CHECK_LAUNCH("gemm_wgmma_grouped_kernel");
+      note_launch("gemm_wgmma_grouped_kernel<%d, %d, %d, %d>", MODE, CL, BN, TA);
+      return MB200_OK;
+    }
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(2u * (unsigned)(sms / 2));
+    cfg.blockDim = dim3(Cfg::kThreads);
+    cfg.dynamicSmemBytes = Cfg::kSmem;
+    cfg.stream = stream;
+    cudaLaunchAttribute at[1];
+    at[0].id = cudaLaunchAttributeClusterDimension;
+    at[0].val.clusterDim.x = 2;
+    at[0].val.clusterDim.y = 1;
+    at[0].val.clusterDim.z = 1;
+    cfg.attrs = at;
+    cfg.numAttrs = 1;
+    MB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, gemm_wgmma_grouped_kernel<MODE, CL, BN, TA>, map_a, maps, p, plan));
+    MB_CHECK_LAUNCH("gemm_wgmma_grouped_kernel<cluster 2>");
     note_launch("gemm_wgmma_grouped_kernel<%d, %d, %d, %d>", MODE, CL, BN, TA);
     return MB200_OK;
   }
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(2u * (unsigned)(sms / 2));
-  cfg.blockDim = dim3(Cfg::kThreads);
-  cfg.dynamicSmemBytes = Cfg::kSmem;
-  cfg.stream = stream;
-  cudaLaunchAttribute at[1];
-  at[0].id = cudaLaunchAttributeClusterDimension;
-  at[0].val.clusterDim.x = 2;
-  at[0].val.clusterDim.y = 1;
-  at[0].val.clusterDim.z = 1;
-  cfg.attrs = at;
-  cfg.numAttrs = 1;
-  MB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, gemm_wgmma_grouped_kernel<MODE, CL, BN, TA>, map_a, maps, p, plan));
-  MB_CHECK_LAUNCH("gemm_wgmma_grouped_kernel<cluster 2>");
-  note_launch("gemm_wgmma_grouped_kernel<%d, %d, %d, %d>", MODE, CL, BN, TA);
-  return MB200_OK;
 }
 
 // tile width: prefill (128-row tiles) takes the widest tile that divides N; decode-sized calls (32-row tiles, HBM-bound) pick the
@@ -504,26 +519,35 @@ int launch_grouped_streamk(const void* a, int64_t rows_cap, int64_t K, int64_t N
   p.epi = epi;
   p.partials = reinterpret_cast<float*>((uint8_t*)workspace + kWsSkPartials.offset);
   p.flags = reinterpret_cast<unsigned*>((uint8_t*)workspace + kWsSkFlags.offset);
-  if (fmt == MoeFmt::FP8) {
-    using Cfg8 = TgCfg<SK_BN, TA, true>;
-    MB_CHECK_CUDA(cudaFuncSetAttribute(gemm_streamk_grouped_fp8_kernel<MODE, TA>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg8::kSmem));
-    MB_CHECK_CUDA(launch_pdl(gemm_streamk_grouped_fp8_kernel<MODE, TA>, dim3((unsigned)sms), dim3(Cfg8::kThreads), (size_t)Cfg8::kSmem, stream, map_a, maps,
-                             sc, p, plan));
-    note_launch("gemm_streamk_grouped_fp8_kernel<%d, %d>", MODE, TA);
+  if constexpr (grouped_fmt_built<MODE>(MoeFmt::FP8)) {
+    if (fmt == MoeFmt::FP8) {
+      using Cfg8 = TgCfg<SK_BN, TA, true>;
+      MB_CHECK_CUDA(cudaFuncSetAttribute(gemm_streamk_grouped_fp8_kernel<MODE, TA>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg8::kSmem));
+      MB_CHECK_CUDA(launch_pdl(gemm_streamk_grouped_fp8_kernel<MODE, TA>, dim3((unsigned)sms), dim3(Cfg8::kThreads), (size_t)Cfg8::kSmem, stream, map_a,
+                               maps, sc, p, plan));
+      note_launch("gemm_streamk_grouped_fp8_kernel<%d, %d>", MODE, TA);
+      return MB200_OK;
+    }
+  }
+  if constexpr (grouped_fmt_built<MODE>(MoeFmt::INT4)) {
+    if (fmt == MoeFmt::INT4) {  // (the grouped body waits for the plan before it requests any chunk)
+      using Cfg4 = SkW4Cfg<TA>;
+      MB_CHECK_CUDA(cudaFuncSetAttribute(gemm_streamk_grouped_int4_kernel<MODE, TA>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg4::kSmem));
+      MB_CHECK_CUDA(launch_pdl(gemm_streamk_grouped_int4_kernel<MODE, TA>, dim3((unsigned)sms), dim3(Cfg4::kThreads), (size_t)Cfg4::kSmem, stream, map_a,
+                               maps, gsc, p, plan));
+      note_launch("gemm_streamk_grouped_int4_kernel<%d, %d>", MODE, TA);
+      return MB200_OK;
+    }
+  }
+  if constexpr (!grouped_fmt_built<MODE>(MoeFmt::BF16)) {
+    return fail(MB200_E_INVALID, "grouped stream-K gemm: epilogue mode %d has no variant for these weights", MODE);
+  } else {
+    MB_CHECK_CUDA(cudaFuncSetAttribute(gemm_streamk_grouped_kernel<MODE, TA>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmem));
+    MB_CHECK_CUDA(launch_pdl(gemm_streamk_grouped_kernel<MODE, TA>, dim3((unsigned)sms), dim3(Cfg::kThreads), (size_t)Cfg::kSmem, stream, map_a, maps, p,
+                             plan));
+    note_launch("gemm_streamk_grouped_kernel<%d, %d>", MODE, TA);
     return MB200_OK;
   }
-  if (fmt == MoeFmt::INT4) {  // (the grouped body waits for the plan before it requests any chunk)
-    using Cfg4 = SkW4Cfg<TA>;
-    MB_CHECK_CUDA(cudaFuncSetAttribute(gemm_streamk_grouped_int4_kernel<MODE, TA>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg4::kSmem));
-    MB_CHECK_CUDA(launch_pdl(gemm_streamk_grouped_int4_kernel<MODE, TA>, dim3((unsigned)sms), dim3(Cfg4::kThreads), (size_t)Cfg4::kSmem, stream, map_a,
-                             maps, gsc, p, plan));
-    note_launch("gemm_streamk_grouped_int4_kernel<%d, %d>", MODE, TA);
-    return MB200_OK;
-  }
-  MB_CHECK_CUDA(cudaFuncSetAttribute(gemm_streamk_grouped_kernel<MODE, TA>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmem));
-  MB_CHECK_CUDA(launch_pdl(gemm_streamk_grouped_kernel<MODE, TA>, dim3((unsigned)sms), dim3(Cfg::kThreads), (size_t)Cfg::kSmem, stream, map_a, maps, p, plan));
-  note_launch("gemm_streamk_grouped_kernel<%d, %d>", MODE, TA);
-  return MB200_OK;
 }
 
 template <int MODE>
@@ -535,6 +559,7 @@ int launch_grouped(const void* a, int64_t rows_cap, int64_t K, int64_t N, const 
   MB_CHECK_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   MB_CHECK_ARG(K % TG_BK == 0 && N % 32 == 0, "grouped gemm: K=%lld must be a multiple of 64, N=%lld of 32", (long long)K, (long long)N);
   MB_CHECK_ARG(fmt != MoeFmt::INT4 || K % kInt4Group == 0, "grouped gemm (int4): K=%lld must be a multiple of 128", (long long)K);
+  MB_CHECK_ARG(grouped_fmt_built<MODE>(fmt), "grouped gemm: epilogue mode %d has no variant for these weights", MODE);
   if (tile_rows < 128 && streamk_eligible(tile_rows, N, K)) {
     if (tile_rows == 32) return launch_grouped_streamk<MODE, 32>(a, rows_cap, K, N, w_host, E, plan, epi, workspace, workspace_bytes, sms, stream, fmt, scales);
     return launch_grouped_streamk<MODE, 64>(a, rows_cap, K, N, w_host, E, plan, epi, workspace, workspace_bytes, sms, stream, fmt, scales);

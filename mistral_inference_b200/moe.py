@@ -23,7 +23,7 @@ import torch
 from torch import nn
 
 from . import _abi
-from .args import MoeArgs
+from .args import LoraArgs, MoeArgs
 
 MOE_BLOCK_TOKENS = 16384  # prefill goes through the experts in blocks of this many tokens (bounds the row buffers: ~2 GB at 8x22B)
 
@@ -44,9 +44,11 @@ class Fp8Expert(nn.Module):
     """One expert with FP8 (e4m3) weights, the storage format of include/mistral_b200.h: `w13_q` [2*hidden, dim] (row 2i = w1[i],
     row 2i + 1 = w3[i], like FeedForward.w13) and `w2_q` [dim, hidden] hold the e4m3 bit patterns as uint8, with one fp32 scale
     per row.  The scales are stored as their int32 bit patterns (`w13_scale` / `w2_scale` are the fp32 views): `Module.to(dtype)`
-    casts every floating tensor, and these must keep their bits.  Weights arrive as bf16 and are quantised in place on the device."""
+    casts every floating tensor, and these must keep their bits.  Weights arrive as bf16 and are quantised in place on the device.
+    With `lora` set the expert's w1 / w2 / w3 are LoRALinears (lora.py:22-89) on W': `w13_lora` and `w2_lora` hold their bf16
+    adapters, packed like FeedForward's."""
 
-    def __init__(self, dim: int, hidden_dim: int):
+    def __init__(self, dim: int, hidden_dim: int, lora: Optional[LoraArgs] = None):
         super().__init__()
         self.dim = dim
         self.hidden_dim = hidden_dim
@@ -54,6 +56,20 @@ class Fp8Expert(nn.Module):
         self.w2_q = nn.Parameter(torch.empty(dim, hidden_dim, dtype=torch.uint8), requires_grad=False)
         self.w13_scale_bits = nn.Parameter(torch.empty(2 * hidden_dim, dtype=torch.int32), requires_grad=False)
         self.w2_scale_bits = nn.Parameter(torch.empty(dim, dtype=torch.int32), requires_grad=False)
+        self.lora = lora
+        if lora is not None:
+            from .transformer_layers import LoraAdapter  # (transformer_layers imports this module)
+
+            self.w13_lora = LoraAdapter(dim, [hidden_dim, hidden_dim], lora, interleaved=True)
+            self.w2_lora = LoraAdapter(hidden_dim, [dim], lora)
+
+    def adapter(self, name: str):
+        """(packed adapter, segment) of the reference Linear `name` (w1, w2 or w3)."""
+        if name in ("w1", "w3"):
+            return self.w13_lora, 0 if name == "w1" else 1
+        if name == "w2":
+            return self.w2_lora, 0
+        raise ValueError(f"expert Linear {name!r}")
 
     @property
     def w13_scale(self) -> torch.Tensor:
@@ -149,7 +165,8 @@ class Int4Expert(nn.Module, _Int4Rows):
 class MoeBuffers:
     """Row buffers of one MoE call for up to `T` tokens (shared by all layers of a model; sizes from mb200_moe_sizes)."""
 
-    def __init__(self, T: int, dim: int, hidden: int, E: int, k: int, device: torch.device, dtype: torch.dtype, yw_ptr: Optional[int] = None):
+    def __init__(self, T: int, dim: int, hidden: int, E: int, k: int, device: torch.device, dtype: torch.dtype, yw_ptr: Optional[int] = None,
+                 lora_cols: int = 0):
         self.T = T
         self.tile_rows, self.rows_cap, self.plan_words = _abi.moe_sizes(T, E, k)
         i32 = dict(dtype=torch.int32, device=device)
@@ -163,6 +180,10 @@ class MoeBuffers:
         # weighted expert output rows: a local tensor, or (expert parallel) this rank's IPC-exported region that peers write too
         self.yw = torch.zeros(self.rows_cap, dim, dtype=dtype, device=device) if yw_ptr is None else None
         self.yw_ptr = self.yw.data_ptr() if yw_ptr is None else yw_ptr
+        # un-merged expert adapters (lora_cols = the w13 adapter's rank columns, the wider one): the down projection's output and the
+        # up projection's L, shared by w13 and w2 (include/mistral_b200.h); l_buf doubles as the down projection's split partials
+        self.lora_a = torch.empty(self.rows_cap, lora_cols, dtype=dtype, device=device) if lora_cols else None
+        self.lora_l = torch.empty(self.rows_cap, max(2 * hidden, dim), dtype=dtype, device=device) if lora_cols else None
 
 
 class ExpertComm:
@@ -236,7 +257,9 @@ class MoeLayer(nn.Module):
         first = self.experts[str(self.local_expert_ids[0])]
         # the experts' storage format, one of EXPERT_WEIGHTS: which grouped entry point runs and which tensors it reads
         self.expert_weights = "fp8" if isinstance(first, Fp8Expert) else ("int4" if isinstance(first, Int4Expert) else "bf16")
+        self.lora = first.lora if isinstance(first, Fp8Expert) else None  # un-merged adapters: FP8 experts only
         self._ptrs = None
+        self._lora_ptrs = None
 
     @property
     def gate(self) -> _GateView:
@@ -257,21 +280,32 @@ class MoeLayer(nn.Module):
     def _weight_tables(self):
         """HOST arrays of E device pointers (NULL for experts of other ranks), rebuilt when a weight moved: (w13, w2), for FP8
         experts (w13_q, w13 scales, w2_q, w2 scales), for INT4 experts (w13 codes, w13 group scales, w2 codes, w2 group scales)."""
-        E = self.args.num_experts
         if self.expert_weights == "fp8":
             tensors = lambda ex: (ex.w13_q, ex.w13_scale_bits, ex.w2_q, ex.w2_scale_bits)  # noqa: E731
         elif self.expert_weights == "int4":
             tensors = lambda ex: (ex.w13, ex.w13_gscale_bits, ex.w2_weight, ex.w2_gscale_bits)  # noqa: E731
         else:
             tensors = lambda ex: (ex.w13, ex.w2_weight)  # noqa: E731
+        return self._pointer_tables("_ptrs", tensors)
+
+    def _adapter_tables(self):
+        """The same for the FP8 experts' packed adapters: (w13 A, w13 B, w2 A, w2 B)."""
+        return self._pointer_tables("_lora_ptrs", lambda ex: (ex.w13_lora.a, ex.w13_lora.b, ex.w2_lora.a, ex.w2_lora.b))
+
+    def _pointer_tables(self, cache: str, tensors):
+        """One HOST array of E device pointers per tensor that `tensors(expert)` returns, cached in attribute `cache` until a pointer
+        changes."""
+        E = self.args.num_experts
         key = tuple((e, *(t.data_ptr() for t in tensors(self.experts[str(e)]))) for e in self.local_expert_ids)
-        if self._ptrs is None or self._ptrs[0] != key:
+        cached = getattr(self, cache)
+        if cached is None or cached[0] != key:
             tables = [(ctypes.c_void_p * E)() for _ in key[0][1:]]
             for e in self.local_expert_ids:
                 for tab, t in zip(tables, tensors(self.experts[str(e)])):
                     tab[e] = t.data_ptr()
-            self._ptrs = (key, tables)
-        return self._ptrs[1]
+            cached = (key, tables)
+            setattr(self, cache, cached)
+        return cached[1]
 
     def run(self, hn: torch.Tensor, residual: Optional[torch.Tensor], ws: "_abi.Workspace") -> torch.Tensor:
         """`hn` = ffn_norm(h) [T, dim]; returns residual + moe(hn) (or moe(hn) when residual is None)."""
@@ -280,17 +314,25 @@ class MoeLayer(nn.Module):
         E, k = self.args.num_experts, self.args.num_experts_per_tok
         out = torch.empty_like(hn)
         tables = self._weight_tables()
+        lora_tables = self._adapter_tables() if self.lora is not None else None
+        lora_cols = first.w13_lora.rank_cols if self.lora is not None else 0
         g, G = self.expert_shard
         for r0 in range(0, T, MOE_BLOCK_TOKENS):
             r1 = min(T, r0 + MOE_BLOCK_TOKENS)
             n = r1 - r0
             comm = ws.expert_comm(self, n, dim) if self.sharded else None
-            b = ws.moe_buffers(n, dim, first.hidden_dim, E, k, hn.dtype, comm, self.layer_parity)
+            b = ws.moe_buffers(n, dim, first.hidden_dim, E, k, hn.dtype, comm, self.layer_parity, lora_cols)
             assert comm is None or b.rows_cap <= comm.rows_cap
             _abi.moe_route(hn[r0:r1], self.gate_weight, E, k, g, G, b)
             res = residual[r0:r1] if residual is not None else None
             cs = comm.struct(self.layer_parity) if comm is not None else None
-            if self.expert_weights == "fp8":
+            if lora_tables is not None:
+                a13, b13, a2, b2 = lora_tables
+                l13 = _abi.moe_lora_struct(a13, b13, first.w13_lora.rank_cols, first.w13_lora.scaling, b.lora_a, b.lora_l)
+                r2 = first.w2_lora.rank_cols
+                l2 = _abi.moe_lora_struct(a2, b2, r2, first.w2_lora.scaling, b.lora_a.view(-1)[: b.rows_cap * r2].view(b.rows_cap, r2), b.lora_l)
+                _abi.moe_grouped_ffn_fp8_lora(b, *tables, res, out[r0:r1], n, dim, first.hidden_dim, E, k, cs, ws, l13, l2)
+            elif self.expert_weights == "fp8":
                 _abi.moe_grouped_ffn_fp8(b, *tables, res, out[r0:r1], n, dim, first.hidden_dim, E, k, cs, ws)
             elif self.expert_weights == "int4":
                 _abi.moe_grouped_ffn_int4(b, *tables, res, out[r0:r1], n, dim, first.hidden_dim, E, k, cs, ws)

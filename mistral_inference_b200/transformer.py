@@ -8,6 +8,7 @@ import json
 import logging
 import math
 import os
+import re
 from pathlib import Path
 from typing import Any, Dict, List, Mapping, Optional, Tuple, Union
 
@@ -19,7 +20,7 @@ from .args import PATCH_MERGE, TransformerArgs
 from .cache import KV_CACHE_FORMATS, BufferCache, CacheInputMetadata
 from .rope import precompute_freqs_cis
 from .moe import EXPERT_WEIGHTS, Fp8Expert, Int4Expert
-from .transformer_layers import LoraAdapter, RMSNorm, TransformerBlock
+from .transformer_layers import LoraAdapter, RMSNorm, TransformerBlock, check_moe_lora
 from .vision_encoder import PatchMerger, VisionLanguageAdapter, VisionTransformer
 
 ROPE_TABLE_LEN = 128_000  # transformer.py:116
@@ -29,6 +30,7 @@ _LORA_LINEARS = {"attention.wq": ("attention.wqkv_lora", 0), "attention.wk": ("a
                  "feed_forward.w1": ("feed_forward.w13_lora", 0), "feed_forward.w3": ("feed_forward.w13_lora", 1),
                  "feed_forward.w2": ("feed_forward.w2_lora", 0)}
 _LORA_PARTS = (".linear.weight", ".lora_A.weight", ".lora_B.weight")
+_EXPERT_LINEAR = re.compile(r"^feed_forward\.experts\.\d+\.w[123]$")  # the LoRALinears of a MoE block's experts (below `layers.{i}.`)
 _VISION_PREFIXES = ("vision_encoder.", "vision_language_adapter.", "patch_merger.", "pre_mm_projector_norm.")  # transformer.py:279-291
 _NVTX = os.environ.get("MB200_NVTX", "0") == "1"
 
@@ -130,8 +132,7 @@ class Transformer(nn.Module):
                              "of the scale groups")
         self.expert_weights = expert_weights
         if args.lora is not None and args.moe is not None:
-            raise NotImplementedError("un-merged LoRA on mixture-of-experts layers is not built: the grouped expert GEMMs have no "
-                                      "LoRA stage (merge the adapter instead: args.lora = None, then load_lora)")
+            check_moe_lora(expert_weights, dense_weights)
         self.args = args
         self.expert_parallel = expert_parallel or (0, 1)
         assert 0 <= self.expert_parallel[0] < self.expert_parallel[1], self.expert_parallel
@@ -699,9 +700,18 @@ class Transformer(nn.Module):
             for suffix in _LORA_PARTS:
                 if rest.endswith(suffix):
                     name, part = rest[: -len(suffix)], suffix
+            slot = None
             if name in _LORA_LINEARS:
                 path, seg = _LORA_LINEARS[name]
-                adapter = blk.get_submodule(path)
+                slot = blk.get_submodule(path), seg
+            elif _EXPERT_LINEAR.match(name) and (part or rest.endswith(".weight")) and hasattr(blk.feed_forward, "experts"):
+                # the LoRALinears of FP8 experts
+                e, lin = name.split(".")[2:]
+                if e not in blk.feed_forward.experts:
+                    return False  # an expert owned by another expert-parallel rank
+                slot = blk.feed_forward.experts[e].adapter(lin)
+            if slot is not None:
+                adapter, seg = slot
                 if part == ".lora_A.weight":
                     put(adapter.lora_A(seg), adapter.put_A, seg)
                     return True
@@ -851,7 +861,9 @@ class Transformer(nn.Module):
             have = set(loaded) | {k[: -len(".weight")] + sfx for k in loaded
                                   for sfx in (".weight_e4m3", ".weight_scale", ".weight_int4", ".weight_gscale")}
             return set(self.reference_keys()) - have
-        have = set(loaded) | {k[: -len(".weight")] + ".linear.weight" for k in loaded}
+        # an FP8 expert's `X.linear.weight_e4m3` and `X.linear.weight_scale` are set by `X.linear.weight` or a plain `X.weight`
+        bases = {k[: -len(".linear.weight")] if k.endswith(".linear.weight") else k[: -len(".weight")] for k in loaded}
+        have = set(loaded) | {b + sfx for b in bases for sfx in (".linear.weight", ".linear.weight_e4m3", ".linear.weight_scale")}
         return {k for k in self.reference_keys() if k not in have and not k.endswith((".lora_A.weight", ".lora_B.weight"))}
 
     def state_dict(self, *args: Any, **kwargs: Any) -> Dict[str, torch.Tensor]:  # type: ignore[override]
@@ -911,7 +923,13 @@ class Transformer(nn.Module):
             out[p + "feed_forward.gate.weight"] = ff.gate_weight
             for e, ex in ff.experts.items():  # keyed by the global expert id; the local ones only when sharded
                 for n in ("w1", "w2", "w3"):
-                    if isinstance(ex, Fp8Expert):  # the stored format itself: no dequantised copies
+                    if isinstance(ex, Fp8Expert) and ex.lora is not None:  # LoRALinear's keys, the base in its stored format
+                        adapter, seg = ex.adapter(n)
+                        out[p + f"feed_forward.experts.{e}.{n}.lora_A.weight"] = adapter.lora_A(seg)
+                        out[p + f"feed_forward.experts.{e}.{n}.lora_B.weight"] = adapter.lora_B(seg)
+                        out[p + f"feed_forward.experts.{e}.{n}.linear.weight_e4m3"] = ex.weight_e4m3(n)
+                        out[p + f"feed_forward.experts.{e}.{n}.linear.weight_scale"] = ex.weight_scale(n)
+                    elif isinstance(ex, Fp8Expert):  # the stored format itself: no dequantised copies
                         out[p + f"feed_forward.experts.{e}.{n}.weight_e4m3"] = ex.weight_e4m3(n)
                         out[p + f"feed_forward.experts.{e}.{n}.weight_scale"] = ex.weight_scale(n)
                     elif isinstance(ex, Int4Expert):
@@ -959,7 +977,7 @@ class Transformer(nn.Module):
         if self.dense_weights != "bf16" and any(key.startswith("layers.") for key in lora_state_dict):
             raise NotImplementedError(f"merging a LoRA adapter into {self.dense_weights.upper()} dense weights is not built: the layer "
                                       "Linears are stored quantised (load the adapter into a bf16 model)")
-        if self.expert_weights != "bf16" and any(".experts." in key for key in lora_state_dict):
+        if self.args.lora is None and self.expert_weights != "bf16" and any(".experts." in key for key in lora_state_dict):
             raise NotImplementedError(f"merging a LoRA adapter into {self.expert_weights.upper()} expert weights is not built: the experts "
                                       "are stored quantised (load the adapter into a bf16 model, or drop its expert Linears)")
         lora_state_dict = {k: v.to(self.device) for k, v in lora_state_dict.items()}

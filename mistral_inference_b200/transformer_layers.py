@@ -367,6 +367,19 @@ class FeedForward(nn.Module, _Fp8Rows, _Int4Rows):
         return self.run(x, None, 0.0, None, ws)
 
 
+def check_moe_lora(expert_weights: str, dense_weights: str) -> None:
+    """Un-merged LoRA on a mixture-of-experts model is built for FP8 experts with bf16 attention Linears only."""
+    if expert_weights == "int4":
+        raise NotImplementedError("un-merged LoRA on INT4 experts is not built: the INT4 grouped expert GEMMs have no LoRA stage "
+                                  "(expert_weights='fp8' runs the adapters)")
+    if expert_weights != "fp8":
+        raise NotImplementedError("un-merged LoRA on mixture-of-experts layers with bf16 experts is not built: the bf16 grouped expert "
+                                  "GEMMs have no LoRA stage (merge the adapter instead: args.lora = None, then load_lora; or "
+                                  "expert_weights='fp8')")
+    if dense_weights != "bf16":
+        raise NotImplementedError(f"un-merged LoRA on {dense_weights.upper()} dense weights is not built")
+
+
 class TransformerBlock(nn.Module):
     """transformer_layers.py:123-169: pre-norm residual wiring; FeedForward or MoeLayer."""
 
@@ -375,8 +388,7 @@ class TransformerBlock(nn.Module):
                  expert_weights: str = "bf16", dense_weights: str = "bf16"):
         super().__init__()
         if lora is not None and moe is not None:
-            raise NotImplementedError("un-merged LoRA on mixture-of-experts layers is not built: the grouped expert GEMMs have no "
-                                      "LoRA stage (merge the adapter instead: args.lora = None, then load_lora)")
+            check_moe_lora(expert_weights, dense_weights)
         self.n_heads = n_heads
         self.dim = dim
         self.norm_eps = norm_eps
@@ -390,7 +402,7 @@ class TransformerBlock(nn.Module):
         self.feed_forward: nn.Module
         if moe is not None:
             g, G = expert_shard  # this rank allocates only the experts it owns (e % G == g): SURVEY.md 8(e)
-            expert = {"fp8": lambda: Fp8Expert(dim, hidden_dim), "int4": lambda: Int4Expert(dim, hidden_dim)}.get(
+            expert = {"fp8": lambda: Fp8Expert(dim, hidden_dim, lora), "int4": lambda: Int4Expert(dim, hidden_dim)}.get(
                 expert_weights, lambda: FeedForward(dim=dim, hidden_dim=hidden_dim, lora=lora))
             self.feed_forward = MoeLayer(experts={e: expert() for e in range(moe.num_experts) if e % G == g},
                                          gate_weight=nn.Parameter(torch.empty(moe.num_experts, dim), requires_grad=False), moe_args=moe,
