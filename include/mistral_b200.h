@@ -30,7 +30,7 @@
 extern "C" {
 #endif
 
-#define MB200_ABI_VERSION 2
+#define MB200_ABI_VERSION 3
 
 #define MB200_OK 0
 #define MB200_E_INVALID (-1)   /* bad argument / unsupported shape */
@@ -207,14 +207,23 @@ int mb200_ffn_gateup(const void* x, const void* norm_w, const void* w13, void* g
  *        unchanged; MB200_E_INVALID otherwise); the down
  *        projection splits K across CTAs and keeps its fp32 partials in l_buf before the up projection overwrites it.  The split
  *        bounds and the summation order depend on the shape and the device's SM count only, so results are deterministic.
+ * A bank of adapter slots, one slot chosen per token (row_slot non-NULL): a_w and b_w stack n adapters of slot_cols columns each,
+ * each packed as above (slot j: a_w rows and b_w columns j*slot_cols .. j*slot_cols + slot_cols - 1; rank_cols = n*slot_cols), and
+ * the down projection keeps only token t's own slot:
+ *   a[t, c] = bf16(xn[t] . a_w[c])  if c / slot_cols == row_slot[t],  0 otherwise (the whole row when row_slot[t] == -1)
+ * The up projection and the combine are unchanged (the zero columns add exact zeros), so token t's result depends only on its
+ * input, its slot's adapter and the call's shape -- not on the other tokens' slots -- and a token with slot -1 gets the counterpart's
+ * result (up to the sign of a zero).  The call has the same launches as with one adapter.  row_slot NULL: one adapter, as above.
  */
 typedef struct mb200_lora {
-  const void* a_w;   /* [rank_cols, K] bf16 */
-  const void* b_w;   /* [N, rank_cols] bf16 */
-  int64_t rank_cols; /* multiple of 64 */
-  float scaling;     /* args.lora.scaling */
-  void* a_buf;       /* [T, rank_cols] bf16 scratch */
-  void* l_buf;       /* [T, N] bf16 scratch */
+  const void* a_w;          /* [rank_cols, K] bf16 */
+  const void* b_w;          /* [N, rank_cols] bf16 */
+  int64_t rank_cols;        /* multiple of 64 */
+  float scaling;            /* args.lora.scaling */
+  void* a_buf;              /* [T, rank_cols] bf16 scratch */
+  void* l_buf;              /* [T, N] bf16 scratch */
+  const int32_t* row_slot;  /* [T] int32 device: the slot of each token, in [0, rank_cols / slot_cols) or -1; NULL: one adapter */
+  int64_t slot_cols;        /* with row_slot: the columns of one slot, a multiple of 64 that divides rank_cols */
 } mb200_lora;
 int mb200_attn_qkv_lora(const void* x, const void* norm_w, const void* wqkv, const float* rope, const int32_t* positions,
                         void* q_out, void* k_out, void* v_out, void* cache_k, void* cache_v, const int32_t* cache_rows,

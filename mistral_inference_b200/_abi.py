@@ -15,7 +15,7 @@ import torch
 _LIB_PATH = Path(os.environ.get("MB200_LIB_PATH") or Path(__file__).resolve().parent / "libmb200.so")  # override: A/B builds of experiments
 _lib: Optional[ctypes.CDLL] = None
 
-ABI_VERSION = 2
+ABI_VERSION = 3
 SKINNY_MAX_T = 4
 WORKSPACE_HEADER_BYTES = 64 * 1024
 
@@ -393,14 +393,22 @@ def quantize_int4_groups(w: torch.Tensor, q: torch.Tensor, gscale: torch.Tensor)
 
 class LoraStruct(ctypes.Structure):
     """mb200_lora (include/mistral_b200.h)."""
-    _fields_ = [("a_w", c_void_p), ("b_w", c_void_p), ("rank_cols", c_int64), ("scaling", c_float), ("a_buf", c_void_p), ("l_buf", c_void_p)]
+    _fields_ = [("a_w", c_void_p), ("b_w", c_void_p), ("rank_cols", c_int64), ("scaling", c_float), ("a_buf", c_void_p), ("l_buf", c_void_p),
+                ("row_slot", c_void_p), ("slot_cols", c_int64)]
 
 
-def lora_struct(a_w: torch.Tensor, b_w: torch.Tensor, scaling: float, a_buf: torch.Tensor, l_buf: torch.Tensor) -> LoraStruct:
-    """One adapter of a fused Linear: packed a_w [R, K], b_w [N, R], scratch a_buf [>= T, R] and l_buf [>= T, N] (bf16)."""
+def lora_struct(a_w: torch.Tensor, b_w: torch.Tensor, scaling: float, a_buf: torch.Tensor, l_buf: torch.Tensor,
+                row_slot: Optional[torch.Tensor] = None, slot_cols: int = 0) -> LoraStruct:
+    """One adapter of a fused Linear: packed a_w [R, K], b_w [N, R], scratch a_buf [>= T, R] and l_buf [>= T, N] (bf16).  With
+    `row_slot` (int32 [T] on the device) a_w / b_w are a bank of slots of `slot_cols` columns each and token t uses slot
+    row_slot[t] (-1: none)."""
     R = a_w.shape[0]
     assert b_w.shape[1] == R and a_buf.shape[-1] == R and l_buf.shape[-1] == b_w.shape[0]
-    return LoraStruct(_ptr(a_w), _ptr(b_w), R, scaling, _ptr(a_buf), _ptr(l_buf))
+    if row_slot is not None:
+        assert row_slot.dtype == torch.int32 and row_slot.is_cuda and row_slot.is_contiguous() and row_slot.shape[0] >= a_buf.shape[0], \
+            (row_slot.dtype, tuple(row_slot.shape))
+        assert slot_cols > 0 and R % slot_cols == 0, (R, slot_cols)
+    return LoraStruct(_ptr(a_w), _ptr(b_w), R, scaling, _ptr(a_buf), _ptr(l_buf), _ptr(row_slot), slot_cols if row_slot is not None else 0)
 
 
 def _lora_ref(lora: LoraStruct):

@@ -184,7 +184,8 @@ static int run_linear_quant(const void* x, const void* norm_w, const void* w, co
 }
 
 // Un-merged LoRA around one fused Linear (include/mistral_b200.h): down projection -> up projection -> base GEMM whose epilogue
-// adds bf16(l * scaling) before the mode's work.  For T > MB200_SKINNY_MAX_T the input is normed once into the workspace and both
+// adds bf16(l * scaling) before the mode's work.  With row_slot (a bank of adapter slots) the down projection masks each row to its
+// slot's columns; the up projection and the base GEMM are the same kernels, so the call has the same launches.  For T > MB200_SKINNY_MAX_T the input is normed once into the workspace and both
 // the down kernel and the base GEMM read it; for T <= MB200_SKINNY_MAX_T both are weight-streaming GEMVs that norm in-kernel.
 template <int MODE>
 static int run_linear_lora(const void* x, const void* norm_w, const void* w, EpiParams epi, const mb200_lora* lora, int64_t T, int64_t N,
@@ -193,6 +194,9 @@ static int run_linear_lora(const void* x, const void* norm_w, const void* w, Epi
   const int64_t R = lora->rank_cols;
   MB_CHECK_ARG(R >= 64 && R % 64 == 0 && K % 64 == 0, "lora: rank_cols=%lld and K=%lld must be multiples of 64", (long long)R, (long long)K);
   MB_CHECK_ARG(T >= 1, "lora: T=%lld", (long long)T);
+  const int64_t Rc = lora->slot_cols;
+  MB_CHECK_ARG(lora->row_slot == nullptr || (Rc >= 64 && Rc % 64 == 0 && R % Rc == 0),
+               "lora: slot_cols=%lld must be a multiple of 64 that divides rank_cols=%lld", (long long)Rc, (long long)R);
   MB_CHECK_ARG(((uintptr_t)lora->a_buf & 15) == 0 && ((uintptr_t)lora->l_buf & 15) == 0,
                "lora: a_buf and l_buf must be 16-byte aligned (l_buf doubles as fp32 split-K scratch)");
   const void* xn = x;
@@ -207,7 +211,14 @@ static int run_linear_lora(const void* x, const void* norm_w, const void* w, Epi
     p.eps = eps;
     p.epi.out = lora->a_buf;
     p.epi.ld_out = R;
-    rc = norm_w ? launch_skinny<EPI_STORE, true>(p, (int)T, st) : launch_skinny<EPI_STORE, false>(p, (int)T, st);
+    if (lora->row_slot != nullptr) {
+      p.row_slot = lora->row_slot;
+      p.slot_cols = (int)Rc;
+      constexpr int M = EPI_STORE | SKINNY_SLOT_MASK;
+      rc = norm_w ? launch_skinny<M, true>(p, (int)T, st) : launch_skinny<M, false>(p, (int)T, st);
+    } else {
+      rc = norm_w ? launch_skinny<EPI_STORE, true>(p, (int)T, st) : launch_skinny<EPI_STORE, false>(p, (int)T, st);
+    }
   } else {
     if (norm_w) {
       const WsRegion nr = ws_normed(T, K);
@@ -218,7 +229,7 @@ static int run_linear_lora(const void* x, const void* norm_w, const void* w, Epi
       xn = normed;
       norm_w = nullptr;
     }
-    rc = launch_lora_down(xn, lora->a_w, lora->a_buf, T, R, K, lora->l_buf, (size_t)T * N * 2, st);
+    rc = launch_lora_down(xn, lora->a_w, lora->a_buf, T, R, K, lora->l_buf, (size_t)T * N * 2, st, lora->row_slot, Rc);
   }
   if (rc) return rc;
   EpiParams up;

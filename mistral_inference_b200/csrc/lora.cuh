@@ -13,6 +13,10 @@
 // plan's tile y -- expert tile_expert[y], rows [tile_row0[y], tile_row0[y] + tile_rows), read on the device, so the launch needs no
 // host sync and replays in a graph.  The grid covers the plan's tile capacity; CTAs past plan[0] exit.  A 32- or 64-row plan
 // tile leaves the rest of the 128-row CTA tile zero-filled and unstored.
+// MASKED (a bank of adapter slots, one slot per row): A stacks n slots of slot_cols rows each, and row t keeps only the columns of
+// its own slot, a[t, c] = 0 unless c / slot_cols == row_slot[t] (all of row t when row_slot[t] == -1).  The mask is applied where
+// a is written -- the splits == 1 store here, or lora_down_reduce_masked_kernel -- so the split-K partials and the split count
+// are those of the unmasked call.  A 64-column tile lies inside one slot (slot_cols is a multiple of 64).
 #pragma once
 #include <type_traits>
 
@@ -40,11 +44,17 @@ struct LoraDownGroupedParams : LoraDownParams {
   int tile_rows;
   const bf16* a_e[MOE_MAX_EXPERTS];
 };
-template <bool GROUPED>
-using LoraDownArgs = std::conditional_t<GROUPED, LoraDownGroupedParams, LoraDownParams>;
+// MASKED: row_slot [T] int32, the slot of each row (-1: none); slot_cols, the A rows of one slot.  Also a separate type.
+struct LoraDownMaskedParams : LoraDownParams {
+  const int32_t* row_slot;
+  int slot_cols;
+};
+template <bool GROUPED, bool MASKED>
+using LoraDownArgs = std::conditional_t<GROUPED, LoraDownGroupedParams, std::conditional_t<MASKED, LoraDownMaskedParams, LoraDownParams>>;
 
-template <bool GROUPED>
-__global__ void __launch_bounds__(LD_THREADS, 2) lora_down_kernel(const LoraDownArgs<GROUPED> p) {
+template <bool GROUPED, bool MASKED = false>
+__global__ void __launch_bounds__(LD_THREADS, 2) lora_down_kernel(const LoraDownArgs<GROUPED, MASKED> p) {
+  static_assert(!(GROUPED && MASKED), "lora down: the slot mask is a dense-call mode");
   extern __shared__ __align__(128) uint8_t smem[];
   const uint32_t smem_base = (uint32_t)__cvta_generic_to_shared(smem);
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -142,7 +152,11 @@ __global__ void __launch_bounds__(LD_THREADS, 2) lora_down_kernel(const LoraDown
         const int r = r0 + 8 * h;
         if (r >= m_end) continue;
         if (p.splits == 1) {
-          *reinterpret_cast<uint32_t*>(p.out + (int64_t)r * p.R + n) = pack_bf16x2(acc[i][j][2 * h], acc[i][j][2 * h + 1]);
+          uint32_t v = pack_bf16x2(acc[i][j][2 * h], acc[i][j][2 * h + 1]);
+          if constexpr (MASKED) {
+            if (p.row_slot[r] != n0 / p.slot_cols) v = 0u;
+          }
+          *reinterpret_cast<uint32_t*>(p.out + (int64_t)r * p.R + n) = v;
         } else {
           *reinterpret_cast<float2*>(p.partial + ((int64_t)split * p.T + r) * p.R + n) = make_float2(acc[i][j][2 * h], acc[i][j][2 * h + 1]);
         }
@@ -156,6 +170,29 @@ __global__ void __launch_bounds__(256) lora_down_reduce_kernel(const float4* __r
   pdl_trigger();
   pdl_wait();
   if (i >= n4) return;
+  float4 s = partial[i];
+  for (int k = 1; k < splits; ++k) {
+    const float4 v = partial[(int64_t)k * n4 + i];
+    s.x += v.x;
+    s.y += v.y;
+    s.z += v.z;
+    s.w += v.w;
+  }
+  out[i] = make_uint2(pack_bf16x2(s.x, s.y), pack_bf16x2(s.z, s.w));
+}
+
+// The same fixed-order sum for a masked call: r4 = R / 4 float4s per row, slot4 = slot_cols / 4.  A column outside its row's slot
+// is written as zero without reading its partials.
+__global__ void __launch_bounds__(256) lora_down_reduce_masked_kernel(const float4* __restrict__ partial, uint2* __restrict__ out, int64_t n4,
+                                                                      int splits, const int32_t* __restrict__ row_slot, int r4, int slot4) {
+  const int64_t i = (int64_t)blockIdx.x * 256 + threadIdx.x;
+  pdl_trigger();
+  pdl_wait();
+  if (i >= n4) return;
+  if (row_slot[i / r4] != (int)(i % r4) / slot4) {
+    out[i] = make_uint2(0u, 0u);
+    return;
+  }
   float4 s = partial[i];
   for (int k = 1; k < splits; ++k) {
     const float4 v = partial[(int64_t)k * n4 + i];
@@ -189,6 +226,16 @@ inline int launch_lora_down_reduce(const void* scratch, void* out, int64_t T, in
   return MB200_OK;
 }
 
+inline int launch_lora_down_reduce_masked(const void* scratch, void* out, int64_t T, int64_t R, int splits, const int32_t* row_slot,
+                                          int64_t slot_cols, cudaStream_t stream) {
+  const int64_t n4 = T * R / 4;
+  MB_CHECK_CUDA(launch_pdl(lora_down_reduce_masked_kernel, dim3((unsigned)ceil_div(n4, 256)), dim3(256), 0, stream, (const float4*)scratch,
+                           (uint2*)out, n4, splits, row_slot, (int)(R / 4), (int)(slot_cols / 4)));
+  note_launch("lora_down_reduce_masked_kernel");
+  MB_CHECK_LAUNCH("lora_down_reduce_masked_kernel");
+  return MB200_OK;
+}
+
 inline int lora_down_sms(int* sms) {
   int dev = 0;
   MB_CHECK_CUDA(cudaGetDevice(&dev));
@@ -198,8 +245,9 @@ inline int lora_down_sms(int* sms) {
 
 // x [T, K] (already normed), a_w [R, K] -> out [T, R]; `scratch` (scratch_bytes, 16-byte aligned) holds the split partials.
 // Both kernels go through launch_pdl: their launch overlaps the predecessor's tail and they wait for it before touching memory.
+// row_slot non-null: the MASKED kernels (a bank of slots of slot_cols columns each), with the same grid and split count.
 inline int launch_lora_down(const void* x, const void* a_w, void* out, int64_t T, int64_t R, int64_t K, void* scratch, size_t scratch_bytes,
-                            cudaStream_t stream) {
+                            cudaStream_t stream, const int32_t* row_slot = nullptr, int64_t slot_cols = 0) {
   MB_CHECK_ARG(K % LD_BK == 0 && R % LD_BN == 0, "lora down: K=%lld and R=%lld must be multiples of 64", (long long)K, (long long)R);
   int sms = 0;
   if (const int rc = lora_down_sms(&sms)) return rc;
@@ -212,9 +260,20 @@ inline int launch_lora_down(const void* x, const void* a_w, void* out, int64_t T
   p.R = (int)R;
   p.K = (int)K;
   p.splits = lora_down_splits((R / LD_BN) * ceil_div(T, LD_BM), T, R, K, scratch_bytes, sms);
+  const dim3 grid((unsigned)(R / LD_BN), (unsigned)ceil_div(T, LD_BM), (unsigned)p.splits);
+  if (row_slot != nullptr) {
+    LoraDownMaskedParams m;
+    static_cast<LoraDownParams&>(m) = p;
+    m.row_slot = row_slot;
+    m.slot_cols = (int)slot_cols;
+    MB_CHECK_CUDA(cudaFuncSetAttribute(lora_down_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, LD_SMEM));
+    MB_CHECK_CUDA(launch_pdl(lora_down_kernel<false, true>, grid, dim3(LD_THREADS), (size_t)LD_SMEM, stream, m));
+    note_launch("lora_down_masked_kernel<%d>", p.splits);
+    MB_CHECK_LAUNCH("lora_down_masked_kernel");
+    return p.splits > 1 ? launch_lora_down_reduce_masked(scratch, out, T, R, p.splits, row_slot, slot_cols, stream) : MB200_OK;
+  }
   MB_CHECK_CUDA(cudaFuncSetAttribute(lora_down_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, LD_SMEM));
-  MB_CHECK_CUDA(launch_pdl(lora_down_kernel<false>, dim3((unsigned)(R / LD_BN), (unsigned)ceil_div(T, LD_BM), (unsigned)p.splits), dim3(LD_THREADS),
-                           (size_t)LD_SMEM, stream, p));
+  MB_CHECK_CUDA(launch_pdl(lora_down_kernel<false>, grid, dim3(LD_THREADS), (size_t)LD_SMEM, stream, p));
   note_launch("lora_down_kernel<%d>", p.splits);
   MB_CHECK_LAUNCH("lora_down_kernel");
   return p.splits > 1 ? launch_lora_down_reduce(scratch, out, T, R, p.splits, stream) : MB200_OK;

@@ -23,7 +23,13 @@ struct SkinnyParams {
   float eps;
   EpiParams epi;
   const uint16_t* gscale = nullptr;  // W4: bf16 group scales [N, K/128]
+  const int32_t* row_slot = nullptr;  // SKINNY_SLOT_MASK: [T] slot of each token (-1: none)
+  int slot_cols = 0;                  // SKINNY_SLOT_MASK: output columns of one slot (a multiple of 64)
 };
+
+// Flag OR-ed into EPI_STORE of the bf16 GEMV only: the LoRA down projection of a bank of adapter slots (lora.cuh, MASKED).  Output
+// column n of token t is stored as zero unless n / slot_cols == row_slot[t]; the pair n, n + 1 always lies in one slot.
+constexpr int SKINNY_SLOT_MASK = 64;
 
 // W8 (FP8 dense weights, launch_skinny_fp8): p.w is e4m3 [N, K] (K % 16 == 0) and MODE carries EPI_WSCALE (the row
 // scales in p.epi.w_scale).  Same CTA, x staging and row pairs; a 16-byte load is 16 weights (half the bytes of a bf16 load, still
@@ -37,6 +43,7 @@ inline bool skinny_needs_optin(size_t smem, int T) { return smem + (size_t)T * k
 // A 16-byte load is 32 weights of one group; the lane converts them to W' (int4x8_to_bf16x2) and feeds the same fp32 FMAs.
 template <int T, int MODE, bool NORM, bool W8 = false, bool W4 = false>
 __global__ void __launch_bounds__(kSkinnyThreads) skinny_linear_kernel(const SkinnyParams p) {
+  static_assert((MODE & SKINNY_SLOT_MASK) == 0 || (MODE == (EPI_STORE | SKINNY_SLOT_MASK) && !W8 && !W4), "slot mask: bf16 EPI_STORE only");
   extern __shared__ __align__(16) uint8_t smem_raw[];
   uint4* xs = reinterpret_cast<uint4*>(smem_raw);  // [T][K/8] 16-byte chunks
   __shared__ float red[T][kSkinnyWarps];
@@ -271,7 +278,14 @@ __global__ void __launch_bounds__(kSkinnyThreads) skinny_linear_kernel(const Ski
   }
 #pragma unroll
   for (int t = 0; t < T; ++t)
-    if (lane == t) epi_pair<MODE>(p.epi, t, n0, acc[0][t], acc[1][t]);
+    if (lane == t) {
+      if constexpr ((MODE & SKINNY_SLOT_MASK) != 0) {
+        if (p.row_slot[t] != n0 / p.slot_cols) acc[0][t] = acc[1][t] = 0.f;
+        epi_pair<EPI_STORE>(p.epi, t, n0, acc[0][t], acc[1][t]);
+      } else {
+        epi_pair<MODE>(p.epi, t, n0, acc[0][t], acc[1][t]);
+      }
+    }
 }
 
 template <int MODE, bool NORM>

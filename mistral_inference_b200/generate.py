@@ -55,10 +55,18 @@ class _PromptPlan:
 @torch.inference_mode()
 def generate(encoded_prompts: List[List[int]], model: Transformer, images: List[List] = [], *, max_tokens: int,  # noqa: B006
              temperature: float, chunk_size: Optional[int] = None, eos_id: Optional[int] = None,
-             draft: Optional[Transformer] = None, draft_tokens: int = 4) -> Tuple[List[List[int]], List[List[float]]]:
+             draft: Optional[Transformer] = None, draft_tokens: int = 4,
+             lora_ids: Optional[List[int]] = None) -> Tuple[List[List[int]], List[List[float]]]:
     """`draft`: another Transformer with the same vocabulary that proposes `draft_tokens` tokens per round for the model to verify
     (speculative decoding, mistral_inference_b200/speculative.py).  Same return value and semantics as without it; greedy output
-    stays the model's own argmax choices and sampled output keeps the model's nucleus distribution."""
+    stays the model's own argmax choices and sampled output keeps the model's nucleus distribution.
+    `lora_ids`: one entry per prompt, the model's adapter slot that sequence runs through (Transformer `lora_slots`), or -1 for the
+    base model; None is slot 0 for every sequence.  A sequence's result does not depend on the other sequences' ids."""
+    if lora_ids is not None:
+        if draft is not None:
+            raise ValueError("lora_ids with a draft model (speculative decoding) is not built")
+        model.check_lora_ids(lora_ids, len(encoded_prompts))
+    lora_kw = {} if lora_ids is None else {"lora_ids": lora_ids}  # no ids: the model calls take no LoRA keyword
     if draft is not None:
         from .speculative import generate_speculative
 
@@ -88,7 +96,7 @@ def generate(encoded_prompts: List[List[int]], model: Transformer, images: List[
     for flat, seqlens, targets, _ in plan.chunks:
         ids = torch.tensor(flat, dtype=torch.long, device=dev)
         tgt = torch.tensor(targets, dtype=torch.long, device=dev)
-        lp, last_logits = model.forward_logprobs(ids, seqlens, cache, tgt, images=flattened_images)
+        lp, last_logits = model.forward_logprobs(ids, seqlens, cache, tgt, images=flattened_images, **lora_kw)
         prompt_lp.append(lp)
     assert last_logits is not None and last_logits.shape == (B, V)
 
@@ -110,7 +118,7 @@ def generate(encoded_prompts: List[List[int]], model: Transformer, images: List[
                 break
         steps_run = step + 1
         if step + 1 < max_tokens:  # the reference runs one more forward whose result is never used; skip it
-            last_logits = model.next_token_logits(nxt, cache)
+            last_logits = model.next_token_logits(nxt, cache, **lora_kw)
 
     # ---- one trip back to the host ----
     if eos_id is not None and max_tokens > 0:

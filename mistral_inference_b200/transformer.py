@@ -33,6 +33,13 @@ _LORA_PARTS = (".linear.weight", ".lora_A.weight", ".lora_B.weight")
 _EXPERT_LINEAR = re.compile(r"^feed_forward\.experts\.\d+\.w[123]$")  # the LoRALinears of a MoE block's experts (below `layers.{i}.`)
 _VISION_PREFIXES = ("vision_encoder.", "vision_language_adapter.", "patch_merger.", "pre_mm_projector_norm.")  # transformer.py:279-291
 _NVTX = os.environ.get("MB200_NVTX", "0") == "1"
+MAX_LORA_SLOTS = 16  # every decode step reads every resident slot's adapters (DESIGN.md, "Multi-adapter LoRA")
+
+
+def expand_lora_ids(lora_ids: List[int], seqlens: List[int]) -> torch.Tensor:
+    """Per-sequence adapter slots -> the int32 slot of every token of the flattened batch (CPU)."""
+    assert len(lora_ids) == len(seqlens), (len(lora_ids), len(seqlens))
+    return torch.repeat_interleave(torch.tensor(lora_ids, dtype=torch.int32), torch.tensor(seqlens, dtype=torch.long))
 
 
 class _nvtx:
@@ -96,7 +103,7 @@ def _check_dense_weights(args: TransformerArgs, dense_weights: str, expert_weigh
 class Transformer(nn.Module):
     def __init__(self, args: TransformerArgs, pipeline_rank: int = 0, num_pipeline_ranks: int = 1, softmax_fp32: bool = True,
                  expert_parallel: Optional[Tuple[int, int]] = None, expert_group: Any = None, expert_weights: str = "bf16", *,
-                 kv_cache: str = "bf16", dense_weights: str = "bf16"):
+                 kv_cache: str = "bf16", dense_weights: str = "bf16", lora_slots: int = 1):
         """Same signature as the reference (transformer.py:34-40) plus `expert_parallel = (rank, world)`: MoE experts sharded
         `e % world == rank` over the ranks of `expert_group` (default process group), everything else replicated, one
         all-reduce of [T, dim] per MoE layer (SURVEY.md 8e); and `expert_weights`: "bf16", or "fp8" to store every MoE expert
@@ -110,8 +117,18 @@ class Transformer(nn.Module):
         the lm head, the norms and the vision tower stay bf16).  That model is not bit-identical to any bf16 model.  "int4" stores the
         same Linears as symmetric 4-bit codes with one bf16 scale per group of 128 k of a row; that model computes exactly what the
         bf16 model computes with the dequantised weights W' (include/mistral_b200.h).  On a mixture-of-experts model "int4" stores
-        wq, wk, wv and wo only, and needs quantised experts (`expert_weights` "int4" or "fp8")."""
+        wq, wk, wv and wo only, and needs quantised experts (`expert_weights` "int4" or "fp8").  `lora_slots` (with `args.lora`, dense
+        models): every un-merged adapter is a bank of that many slots, loaded with `load_lora(slot=...)`, and each sequence of a batch
+        runs through the slot its `lora_ids` entry names (`generate`, `forward`, ...); at most MAX_LORA_SLOTS."""
+        if not isinstance(lora_slots, int) or not 1 <= lora_slots <= MAX_LORA_SLOTS:
+            raise ValueError(f"lora_slots={lora_slots!r}: expected an int in [1, {MAX_LORA_SLOTS}] (every decode step reads every slot)")
+        if lora_slots > 1 and args.lora is None:
+            raise ValueError(f"lora_slots={lora_slots} needs un-merged adapters: set args.lora (params.json `lora`)")
+        if lora_slots > 1 and args.moe is not None:
+            raise ValueError(f"lora_slots={lora_slots} on a mixture-of-experts model is not built: the grouped expert GEMMs have no "
+                             "per-sequence adapter mask")
         super().__init__()
+        self.lora_slots = lora_slots
         _check_dense_weights(args, dense_weights, expert_weights)
         self.dense_weights = dense_weights
         if kv_cache not in KV_CACHE_FORMATS:
@@ -177,7 +194,7 @@ class Transformer(nn.Module):
             str(i): TransformerBlock(dim=args.dim, hidden_dim=args.hidden_dim, n_heads=args.n_heads, n_kv_heads=args.n_kv_heads,
                                      head_dim=args.head_dim, norm_eps=args.norm_eps, lora=args.lora, moe=args.moe,
                                      expert_shard=self.expert_parallel, expert_group=expert_group, expert_weights=expert_weights,
-                                     dense_weights=dense_weights)
+                                     dense_weights=dense_weights, lora_slots=lora_slots)
             for i in range(offset, end)
         })
         self.n_local_layers = len(self.layers)
@@ -235,6 +252,36 @@ class Transformer(nn.Module):
         assert cache is None or cache.kv_cache == self.kv_cache, (
             f"a {cache.kv_cache} KV cache passed to a model built with kv_cache={self.kv_cache!r}")
 
+    def check_lora_ids(self, lora_ids: List[int], batch: int) -> None:
+        """Raises ValueError unless `lora_ids` names one adapter slot in [0, lora_slots), or -1 for the base model, per sequence."""
+        if self.args.lora is None:
+            raise ValueError("lora_ids needs un-merged adapters: set args.lora (params.json `lora`)")
+        if self.num_pipeline_ranks > 1:
+            raise ValueError("lora_ids with pipeline ranks is not built: the stages would each need the per-token slots")
+        if self.expert_parallel[1] > 1:
+            raise ValueError("lora_ids with expert parallelism is not built: the grouped expert GEMMs have no per-sequence adapter mask")
+        if self.args.moe is not None:
+            raise ValueError("lora_ids on a mixture-of-experts model is not built: the grouped expert GEMMs have no per-sequence adapter mask")
+        if len(lora_ids) != batch:
+            raise ValueError(f"lora_ids has {len(lora_ids)} entries for {batch} sequences")
+        bad = [i for i in lora_ids if not isinstance(i, int) or not -1 <= i < self.lora_slots]
+        if bad:
+            raise ValueError(f"lora_ids {bad}: expected adapter slots in [0, {self.lora_slots}) or -1 (no adapter)")
+
+    def _lora_rows(self, lora_ids: Optional[List[int]], seqlens: List[int]) -> Optional[torch.Tensor]:
+        """The device int32 slot of every token of one forward (uploaded once), or None: the caller's default (`_default_rows`)."""
+        if lora_ids is None:
+            return None
+        self.check_lora_ids(lora_ids, len(seqlens))
+        return expand_lora_ids(lora_ids, seqlens).to(self.device)
+
+    def _default_rows(self, rows: Optional[torch.Tensor], num_toks: int) -> Optional[torch.Tensor]:
+        """No ids: slot 0 for every token of a multi-slot model (the unmasked bank would sum every slot), the unmasked adapter of a
+        single-slot one.  torch.zeros, not an upload, so that it can be captured in a graph."""
+        if rows is None and self.lora_slots > 1:
+            return torch.zeros(num_toks, dtype=torch.int32, device=self.device)
+        return rows
+
     @torch.inference_mode()
     def forward_partial(self, input_ids: torch.Tensor, seqlens: List[int], cache: Optional[BufferCache] = None,
                         images: Optional[List[torch.Tensor]] = None) -> torch.Tensor:
@@ -263,9 +310,10 @@ class Transformer(nn.Module):
             torch.distributed.recv(h, src=self.pipeline_rank - 1)
 
         rope = self.rope_table
+        rows = self._default_rows(None, num_toks)
         for local_layer_id, layer in enumerate(self.layers.values()):
             view = cache.get_view(local_layer_id, input_metadata[local_layer_id]) if cache is not None else None
-            h = layer(h, rope, positions, view, ws)
+            h = layer(h, rope, positions, view, ws, rows)
 
         if cache is not None:
             cache.update_seqlens(seqlens)
@@ -277,17 +325,20 @@ class Transformer(nn.Module):
 
     @torch.inference_mode()
     def forward(self, input_ids: torch.Tensor, seqlens: List[int], cache: Optional[BufferCache] = None,
-                images: Optional[List[torch.Tensor]] = None) -> torch.Tensor:
-        """transformer.py:221-242.  [T, vocab] logits, fp32 when softmax_fp32."""
+                images: Optional[List[torch.Tensor]] = None, *, lora_ids: Optional[List[int]] = None) -> torch.Tensor:
+        """transformer.py:221-242.  [T, vocab] logits, fp32 when softmax_fp32.  `lora_ids`: the adapter slot of each sequence (-1: no
+        adapter); None is slot 0 for every sequence."""
         self._check_runnable()
         self._check_cache(cache)
+        if lora_ids is not None:
+            self.check_lora_ids(lora_ids, len(seqlens))
         last = self.pipeline_rank == self.num_pipeline_ranks - 1
         if last and self.num_pipeline_ranks == 1:
             if not self._uses_images(images) and self._graph_decode_ok(seqlens, cache):
-                outs32 = self.decode_static(input_ids, cache).clone()
+                outs32 = self.decode_static(input_ids, cache, lora_ids=lora_ids).clone()
                 return outs32 if self.softmax_fp32 else outs32.to(self.dtype)
             # single stage: final norm + lm head + .float() are one fused call (no [T, dim] normed round trip)
-            h = self._hidden_no_norm(input_ids, seqlens, cache, images=images)
+            h = self._hidden_no_norm(input_ids, seqlens, cache, images=images, lora_rows=self._lora_rows(lora_ids, seqlens))
             if cache is not None:
                 cache.update_seqlens(seqlens)
             outs32 = torch.empty(h.shape[0], self.vocab_size, device=h.device, dtype=torch.float32)
@@ -307,7 +358,7 @@ class Transformer(nn.Module):
 
     def _hidden_no_norm(self, input_ids: torch.Tensor, seqlens: List[int], cache: Optional[BufferCache],
                         input_metadata: Optional[List[CacheInputMetadata]] = None,
-                        images: Optional[List[torch.Tensor]] = None) -> torch.Tensor:
+                        images: Optional[List[torch.Tensor]] = None, lora_rows: Optional[torch.Tensor] = None) -> torch.Tensor:
         assert len(seqlens) <= self.args.max_batch_size, f"Max batch size is {self.args.max_batch_size}, got batch size of {len(seqlens)}"
         (num_toks,) = input_ids.shape
         assert sum(seqlens) == num_toks, (sum(seqlens), num_toks)
@@ -322,10 +373,11 @@ class Transformer(nn.Module):
         assert self.tok_embeddings is not None
         h = self._embed(input_ids, images)
         rope = self.rope_table
+        lora_rows = self._default_rows(lora_rows, num_toks)
         with _nvtx(f"mb200.layers[T={num_toks}]"):
             for local_layer_id, layer in enumerate(self.layers.values()):
                 view = cache.get_view(local_layer_id, input_metadata[local_layer_id]) if cache is not None else None
-                h = layer(h, rope, positions, view, ws)
+                h = layer(h, rope, positions, view, ws, lora_rows)
         return h
 
     # ------------------------------------------------------------------ images (transformer.py:122-161,188-193)
@@ -476,20 +528,31 @@ class Transformer(nn.Module):
         return st["logits"]
 
     @torch.inference_mode()
-    def decode_static(self, tokens: torch.Tensor, cache: BufferCache) -> torch.Tensor:
+    def decode_static(self, tokens: torch.Tensor, cache: BufferCache, *, lora_ids: Optional[List[int]] = None) -> torch.Tensor:
         """One decode step for every sequence of `cache` (one new token each).  Batch 1: the persistent megakernel.  Batch > 1:
         the per-layer kernels replayed from a CUDA graph.  The step state lives on the DEVICE: `mb200_decode_meta` derives
         positions / ring rows / kv lengths from a device-side position vector and advances it inside the graph, so a replay
         needs no host write at all (a pinned staging buffer rewritten by the host while earlier copies are still queued was the
         round-1 design and a race).  Returns the STATIC fp32 logits buffer [B, V] (overwritten by the next step).  The first call
-        per (cache, batch) runs eagerly (warm-up: loads modules, sets function attributes), the second captures."""
+        per (cache, batch) runs eagerly (warm-up: loads modules, sets function attributes), the second captures.
+        `lora_ids` (see forward) live in a static device vector of the step state, rewritten only when they change."""
         B = tokens.shape[0]
         self._check_cache(cache)
-        if self._megakernel_ok(B):
+        if lora_ids is not None:
+            self.check_lora_ids(lora_ids, B)
+        if self._megakernel_ok(B):  # never with adapters
             return self._decode_megakernel(tokens, cache)
         seqlens = [1] * B
         self.workspace(B)
-        st = self._decode_state(cache, ("graph", B))
+        masked = lora_ids is not None or self.lora_slots > 1
+        st = self._decode_state(cache, ("graph", B, "lora_rows") if masked else ("graph", B))
+        if masked:
+            ids = list(lora_ids) if lora_ids is not None else [0] * B
+            if "lora_rows" not in st:
+                st.update({"lora_rows": torch.empty(B, dtype=torch.int32, device=self.device), "lora_ids": None})
+            if st["lora_ids"] != ids:
+                st["lora_rows"].copy_(torch.tensor(ids, dtype=torch.int32))  # pageable source: staged by the runtime, like seqpos
+                st["lora_ids"] = ids
         host = cache._kv_seqlens_host
         assert host is not None and len(host) == B, "decode_static needs a prefilled cache of this batch size"
         if max(host) >= ROPE_TABLE_LEN:
@@ -510,7 +573,7 @@ class Transformer(nn.Module):
 
         def run() -> None:
             _abi.decode_meta(st["seqpos"], st["meta"], distinct)
-            h = self._hidden_no_norm(st["tokens"], seqlens, cache, md)
+            h = self._hidden_no_norm(st["tokens"], seqlens, cache, md, lora_rows=st.get("lora_rows"))
             _abi.lm_head(h, self.norm.weight, self.output_weight, st["logits"], self.args.norm_eps, self.workspace(B))
             _abi.argmax_rows(st["logits"], st["next"])  # greedy pick on the device (generate.py:156): feeds the next step
 
@@ -592,13 +655,14 @@ class Transformer(nn.Module):
         st["expected"] = list(device_lens)
 
     @torch.inference_mode()
-    def last_token_logits(self, input_ids: torch.Tensor, seqlens: List[int], cache: BufferCache) -> torch.Tensor:
+    def last_token_logits(self, input_ids: torch.Tensor, seqlens: List[int], cache: BufferCache, *,
+                          lora_ids: Optional[List[int]] = None) -> torch.Tensor:
         """fp32 logits [B, V] of each sequence's last token of a ragged forward that extends `cache` (the lm head runs on those
-        rows only)."""
+        rows only).  `lora_ids`: see forward."""
         self._check_runnable()
         self._check_cache(cache)
         self._last_static_logits = 0
-        h = self._hidden_no_norm(input_ids, seqlens, cache)
+        h = self._hidden_no_norm(input_ids, seqlens, cache, lora_rows=self._lora_rows(lora_ids, seqlens))
         cache.update_seqlens(seqlens)
         last_idx = torch.tensor(seqlens, device=input_ids.device).cumsum(0) - 1
         logits = torch.empty(len(seqlens), self.vocab_size, dtype=torch.float32, device=h.device)
@@ -612,26 +676,29 @@ class Transformer(nn.Module):
         return self.last_argmax is not None and logits.data_ptr() == self._last_static_logits
 
     @torch.inference_mode()
-    def next_token_logits(self, tokens: torch.Tensor, cache: BufferCache) -> torch.Tensor:
+    def next_token_logits(self, tokens: torch.Tensor, cache: BufferCache, *, lora_ids: Optional[List[int]] = None) -> torch.Tensor:
         """fp32 logits [B, V] of one decode step for every sequence.  On the single-stage CUDA path this is the step's static
-        buffer (no clone; valid until the next step), otherwise `forward`."""
+        buffer (no clone; valid until the next step), otherwise `forward`.  `lora_ids`: see forward."""
         B = tokens.shape[0]
         if self.pipeline_rank == self.num_pipeline_ranks - 1 == 0 and self._graph_decode_ok([1] * B, cache):
             self._check_runnable()
-            return self.decode_static(tokens, cache)
+            return self.decode_static(tokens, cache, lora_ids=lora_ids)
         self._last_static_logits = 0
-        out = self.forward(tokens, [1] * B, cache)
+        out = self.forward(tokens, [1] * B, cache, lora_ids=lora_ids)
         return out if out.dtype == torch.float32 else out.float()
 
     @torch.inference_mode()
     def forward_logprobs(self, input_ids: torch.Tensor, seqlens: List[int], cache: Optional[BufferCache],
-                         targets: torch.Tensor, images: Optional[List[torch.Tensor]] = None) -> Tuple[torch.Tensor, torch.Tensor]:
+                         targets: torch.Tensor, images: Optional[List[torch.Tensor]] = None, *,
+                         lora_ids: Optional[List[int]] = None) -> Tuple[torch.Tensor, torch.Tensor]:
         """One prompt chunk for generate(): returns (lp [T] fp32 with lp[t] = log_softmax(logits[t])[targets[t]] where
         targets[t] >= 0, logits [B, V] fp32 of each sequence's last token).  Replaces forward + log_softmax over [T, V] +
         per-token gathers (generate.py:97-118): the lm head runs over blocks of rows, each followed by the fused
-        log-softmax + gather kernel, so the full [T, V] logits never exist."""
+        log-softmax + gather kernel, so the full [T, V] logits never exist.  `lora_ids`: see forward."""
         self._last_static_logits = 0
         self._check_cache(cache)
+        if lora_ids is not None:
+            self.check_lora_ids(lora_ids, len(seqlens))
         T, V = input_ids.shape[0], self.vocab_size
         last_idx = torch.tensor(seqlens, device=input_ids.device).cumsum(0) - 1
         lp = torch.zeros(T, dtype=torch.float32, device=input_ids.device)
@@ -640,7 +707,7 @@ class Transformer(nn.Module):
             _abi.logprob_gather(logits, targets, out=lp)
             return lp, logits.index_select(0, last_idx)
         self._check_runnable()
-        h = self._hidden_no_norm(input_ids, seqlens, cache, images=images)
+        h = self._hidden_no_norm(input_ids, seqlens, cache, images=images, lora_rows=self._lora_rows(lora_ids, seqlens))
         if cache is not None:
             cache.update_seqlens(seqlens)
         assert self.norm is not None and self.output_weight is not None
@@ -656,9 +723,9 @@ class Transformer(nn.Module):
         return lp, last_logits
 
     # ------------------------------------------------------------------ weights
-    def _assign(self, k: str, v: torch.Tensor) -> bool:
-        """Copies reference-keyed tensor `v` into the packed parameters.  Returns False when the key belongs to
-        another pipeline rank."""
+    def _assign(self, k: str, v: torch.Tensor, lora_slot: int = 0) -> bool:
+        """Copies reference-keyed tensor `v` into the packed parameters (LoRA keys: into adapter slot `lora_slot`).  Returns False
+        when the key belongs to another pipeline rank."""
         def put(dst: torch.Tensor, setter=None, seg: int = 0) -> None:
             assert dst.shape == v.shape, f"{k}: shape {tuple(v.shape)} != expected {tuple(dst.shape)}"
             if setter is None:
@@ -686,13 +753,13 @@ class Transformer(nn.Module):
             _, lid, rest = k.split(".", 2)
             if lid not in self.layers:
                 return False
-            return self._assign_block(self.layers[lid], k, rest, put)
+            return self._assign_block(self.layers[lid], k, rest, put, lora_slot)
         else:
             raise ValueError(f"Unexpected key {k}")
         return True
 
     @staticmethod
-    def _assign_block(blk: TransformerBlock, k: str, rest: str, put) -> bool:
+    def _assign_block(blk: TransformerBlock, k: str, rest: str, put, lora_slot: int = 0) -> bool:
         """`rest` = the key below `layers.{i}.` of one TransformerBlock (text or vision)."""
         att = blk.attention
         if att.lora is not None:
@@ -713,13 +780,13 @@ class Transformer(nn.Module):
             if slot is not None:
                 adapter, seg = slot
                 if part == ".lora_A.weight":
-                    put(adapter.lora_A(seg), adapter.put_A, seg)
+                    put(adapter.lora_A(seg, lora_slot), lambda s, w: adapter.put_A(s, w, lora_slot), seg)
                     return True
                 if part == ".lora_B.weight":
-                    put(adapter.lora_B(seg), adapter.put_B, seg)
+                    put(adapter.lora_B(seg, lora_slot), lambda s, w: adapter.put_B(s, w, lora_slot), seg)
                     return True
                 if part == "":  # a full checkpoint's plain weight: zero adapter (lora.py:76-89)
-                    adapter.zero(seg)
+                    adapter.zero(seg, lora_slot)
                 rest = name + ".weight"
         ff = blk.feed_forward
         if getattr(att, "fp8", False):  # FP8 dense weights: the reference's bf16 weight, quantised into place
@@ -954,21 +1021,24 @@ class Transformer(nn.Module):
         out[p + name + ".linear.weight"] = weight
 
     # ------------------------------------------------------------------ LoRA (lora.py:92-155)
-    def load_lora(self, lora_path: Union[Path, str], scaling: float = 2.0) -> None:
+    def load_lora(self, lora_path: Union[Path, str], scaling: float = 2.0, *, slot: int = 0) -> None:
         """Loads a LoRA checkpoint.  args.lora None: MERGES it into the packed weights (lora.py:120-139).  args.lora set: copies
-        it into the un-merged adapters (lora.py:140-155), replacing the previous adapter of every Linear it names."""
+        it into the un-merged adapters (lora.py:140-155) of adapter slot `slot` (in [0, lora_slots)), replacing that slot's
+        previous adapter of every Linear it names."""
         import safetensors.torch
 
         lora_path = Path(lora_path)
         assert lora_path.is_file(), f"{lora_path} does not exist or is not a file"
-        self._load_lora_state_dict(safetensors.torch.load_file(str(lora_path)), scaling=scaling)
+        self._load_lora_state_dict(safetensors.torch.load_file(str(lora_path)), scaling=scaling, slot=slot)
 
-    def _load_lora_state_dict(self, lora_state_dict: Dict[str, torch.Tensor], scaling: float = 2.0) -> None:
+    def _load_lora_state_dict(self, lora_state_dict: Dict[str, torch.Tensor], scaling: float = 2.0, slot: int = 0) -> None:
         """args.lora None: weight <- weight + (lora_B @ lora_A) * scaling for every Linear of this rank except the output layer,
         with the same torch ops and dtype as the reference (lora.py:129-137).
         args.lora set: each `X.lora_A/B.weight` is copied in place into this rank's adapter slots (captured decode graphs keep
         their pointers).  `scaling` is ignored, as in the reference: every adapter keeps args.lora.scaling.  Keys of layers that
         other pipeline ranks own are skipped (the reference's strict load_state_dict would raise on them)."""
+        if not isinstance(slot, int) or not 0 <= slot < self.lora_slots:
+            raise ValueError(f"adapter slot {slot!r} outside [0, {self.lora_slots})")
         lora_dtypes = set(p.dtype for p in lora_state_dict.values())
         assert len(lora_dtypes) == 1, f"LoRA weights have multiple different dtypes {lora_dtypes}. All weights need to have the same dtype"
         lora_dtype = lora_dtypes.pop()
@@ -986,7 +1056,7 @@ class Transformer(nn.Module):
                 for k, v in lora_state_dict.items():
                     if not k.endswith((".lora_A.weight", ".lora_B.weight")) or not k.startswith("layers."):
                         raise ValueError(f"Unexpected key {k}")
-                    if not self._assign(k, v):
+                    if not self._assign(k, v, slot):
                         logging.debug("Skipping parameter %s at pipeline rank %d", k, self.pipeline_rank)
             return
         with torch.no_grad():
@@ -1020,12 +1090,14 @@ class Transformer(nn.Module):
     def from_folder(folder: Union[Path, str], max_batch_size: int = 1, num_pipeline_ranks: int = 1,
                     device: Union[torch.device, str] = "cuda", dtype: Optional[torch.dtype] = None,
                     softmax_fp32: bool = True, expert_parallel: Optional[Tuple[int, int]] = None, expert_group: Any = None,
-                    expert_weights: str = "bf16", *, kv_cache: str = "bf16", dense_weights: str = "bf16") -> "Transformer":
+                    expert_weights: str = "bf16", *, kv_cache: str = "bf16", dense_weights: str = "bf16",
+                    lora_slots: int = 1) -> "Transformer":
         """transformer.py:297-338.  Tensors stream from disk straight into the packed device buffers; with `expert_parallel`
         the experts of other ranks are skipped (never read into device memory).  With expert_weights="fp8" or "int4" each bf16
         expert tensor is copied to the device and quantised into place: the peak is the quantised model plus about one bf16 tensor.
         `kv_cache` ("bf16" | "fp8") is the format of the KV cache that generate() builds (see Transformer).  With
-        dense_weights="fp8" or "int4" every bf16 layer Linear is quantised into place the same way."""
+        dense_weights="fp8" or "int4" every bf16 layer Linear is quantised into place the same way.  `lora_slots`: see Transformer;
+        the checkpoint's adapter, if any, fills slot 0."""
         with open(Path(folder) / "params.json", "r") as f:
             model_args = TransformerArgs.from_dict(json.load(f))
         model_args.max_batch_size = max_batch_size
@@ -1045,7 +1117,7 @@ class Transformer(nn.Module):
             # on meta and assigns, transformer.py:321-331; a fp32 build followed by .to(bf16) would need 3x the model's bytes)
             return Transformer.empty(model_args, dev, dtype or ck_dtype, pipeline_rank=pipeline_rank, num_pipeline_ranks=num_pipeline_ranks,
                                      softmax_fp32=softmax_fp32, expert_parallel=expert_parallel, expert_group=expert_group,
-                                     expert_weights=expert_weights, kv_cache=kv_cache, dense_weights=dense_weights)
+                                     expert_weights=expert_weights, kv_cache=kv_cache, dense_weights=dense_weights, lora_slots=lora_slots)
 
         if pt_model_file.exists():
             loaded = torch.load(str(pt_model_file), mmap=True)

@@ -38,53 +38,63 @@ class LoraAdapter(nn.Module):
       a [R, in]  rows s*r .. s*r + r - 1 = lora_A of segment s, R = S*r rounded up to 64, padding rows zero
       b [N, R]   row n = lora_B of n's segment in that segment's r columns, zeros elsewhere; `interleaved` (w13): segment s owns
                  rows 2i + s, like FeedForward.w13
-    `lora_A(s)` / `lora_B(s)` are zero-copy views under the reference's names.  Loads copy in place (captured decode graphs hold
-    the pointers) and keep the zeros: every entry outside a segment's views stays zero."""
+    With `slots` > 1 the adapter is a bank of that many such adapters: slot j owns rows j*Rc .. of `a` and columns j*Rc .. of `b`,
+    Rc = `rank_cols` (one slot's R), each laid out as above; a call given per-token slot ids runs each token through its own slot.
+    `lora_A(s, slot)` / `lora_B(s, slot)` are zero-copy views under the reference's names.  Loads copy in place (captured decode
+    graphs hold the pointers) and keep the zeros: every entry outside a segment's views stays zero."""
 
-    def __init__(self, in_features: int, segments: List[int], lora: LoraArgs, interleaved: bool = False):
+    def __init__(self, in_features: int, segments: List[int], lora: LoraArgs, interleaved: bool = False, slots: int = 1):
         super().__init__()
         assert not interleaved or (len(segments) == 2 and segments[0] == segments[1])
+        assert slots >= 1, slots
         self.rank = lora.rank
         self.scaling = float(lora.scaling)  # fixed at construction, like LoRALinear.scaling
         self.segments = list(segments)
         self.interleaved = interleaved
+        self.slots = slots
         self.rank_cols = -(-len(segments) * lora.rank // 64) * 64
-        self.a = nn.Parameter(torch.zeros(self.rank_cols, in_features), requires_grad=False)
-        self.b = nn.Parameter(torch.zeros(sum(segments), self.rank_cols), requires_grad=False)
+        self.a = nn.Parameter(torch.zeros(slots * self.rank_cols, in_features), requires_grad=False)
+        self.b = nn.Parameter(torch.zeros(sum(segments), slots * self.rank_cols), requires_grad=False)
 
-    def _cols(self, s: int) -> slice:
-        return slice(s * self.rank, (s + 1) * self.rank)
+    def _cols(self, s: int, slot: int) -> slice:
+        assert 0 <= slot < self.slots, f"adapter slot {slot} outside [0, {self.slots})"
+        o = slot * self.rank_cols
+        return slice(o + s * self.rank, o + (s + 1) * self.rank)
 
     def _rows(self, s: int) -> torch.Tensor:
         if self.interleaved:
-            return self.b.view(self.segments[0], 2, self.rank_cols)[:, s]
+            return self.b.view(self.segments[0], 2, self.b.shape[1])[:, s]
         o = sum(self.segments[:s])
         return self.b[o: o + self.segments[s]]
 
-    def lora_A(self, s: int) -> torch.Tensor:
-        return self.a[self._cols(s)]
+    def lora_A(self, s: int, slot: int = 0) -> torch.Tensor:
+        return self.a[self._cols(s, slot)]
 
-    def lora_B(self, s: int) -> torch.Tensor:
-        return self._rows(s)[:, self._cols(s)]
+    def lora_B(self, s: int, slot: int = 0) -> torch.Tensor:
+        return self._rows(s)[:, self._cols(s, slot)]
 
-    def put_A(self, s: int, v: torch.Tensor) -> None:
-        assert v.shape == self.lora_A(s).shape, f"lora_A: shape {tuple(v.shape)} != {tuple(self.lora_A(s).shape)} (rank {self.rank})"
-        self.lora_A(s).copy_(v)
+    def put_A(self, s: int, v: torch.Tensor, slot: int = 0) -> None:
+        want = self.lora_A(s, slot).shape
+        assert v.shape == want, f"lora_A: shape {tuple(v.shape)} != {tuple(want)} (rank {self.rank})"
+        self.lora_A(s, slot).copy_(v)
 
-    def put_B(self, s: int, v: torch.Tensor) -> None:
-        assert v.shape == self.lora_B(s).shape, f"lora_B: shape {tuple(v.shape)} != {tuple(self.lora_B(s).shape)} (rank {self.rank})"
-        self.lora_B(s).copy_(v)
+    def put_B(self, s: int, v: torch.Tensor, slot: int = 0) -> None:
+        want = self.lora_B(s, slot).shape
+        assert v.shape == want, f"lora_B: shape {tuple(v.shape)} != {tuple(want)} (rank {self.rank})"
+        self.lora_B(s, slot).copy_(v)
 
-    def zero(self, s: int) -> None:
+    def zero(self, s: int, slot: int = 0) -> None:
         """A plain `X.weight` checkpoint entry: segment s gets a zero adapter (lora.py:76-89)."""
-        self.lora_A(s).zero_()
-        self.lora_B(s).zero_()
+        self.lora_A(s, slot).zero_()
+        self.lora_B(s, slot).zero_()
 
-    def call(self, T: int) -> "_abi.LoraStruct":
-        """The adapter argument of one `_lora` call over T tokens, with its own scratch."""
-        a_buf = torch.empty(T, self.rank_cols, dtype=self.a.dtype, device=self.a.device)
+    def call(self, T: int, lora_rows: Optional[torch.Tensor] = None) -> "_abi.LoraStruct":
+        """The adapter argument of one `_lora` call over T tokens, with its own scratch.  `lora_rows` (int32 [T] on the device): the
+        slot of each token, -1 for none; None runs the whole packed adapter unmasked (one slot's adapter when `slots` is 1)."""
+        R = self.a.shape[0]
+        a_buf = torch.empty(T, R, dtype=self.a.dtype, device=self.a.device)
         l_buf = torch.empty(T, self.b.shape[0], dtype=self.a.dtype, device=self.a.device)
-        st = _abi.lora_struct(self.a, self.b, self.scaling, a_buf, l_buf)
+        st = _abi.lora_struct(self.a, self.b, self.scaling, a_buf, l_buf, lora_rows, self.rank_cols)
         st.keep = (a_buf, l_buf)  # alive until the call has been enqueued
         return st
 
@@ -128,7 +138,7 @@ class Attention(nn.Module, _Fp8Rows, _Int4Rows):
     """transformer_layers.py:31-93."""
 
     def __init__(self, dim: int, n_heads: int, head_dim: int, n_kv_heads: int, lora: Optional[LoraArgs] = None, fp8: bool = False,
-                 int4: bool = False):
+                 int4: bool = False, lora_slots: int = 1):
         super().__init__()
         self.dim = dim
         self.n_heads = n_heads
@@ -152,8 +162,8 @@ class Attention(nn.Module, _Fp8Rows, _Int4Rows):
             self.wo_weight = nn.Parameter(torch.empty(dim, self.q_dim), requires_grad=False)
         self.lora = lora
         if lora is not None:
-            self.wqkv_lora = LoraAdapter(dim, [self.q_dim, self.kv_dim, self.kv_dim], lora)
-            self.wo_lora = LoraAdapter(self.q_dim, [dim], lora)
+            self.wqkv_lora = LoraAdapter(dim, [self.q_dim, self.kv_dim, self.kv_dim], lora, slots=lora_slots)
+            self.wo_lora = LoraAdapter(self.q_dim, [dim], lora, slots=lora_slots)
 
     # state-dict compatible views
     @property
@@ -198,8 +208,9 @@ class Attention(nn.Module, _Fp8Rows, _Int4Rows):
         raise ValueError(f"attention Linear {name!r}")
 
     def attend(self, x: torch.Tensor, norm_w: torch.Tensor, eps: float, rope: torch.Tensor, positions: torch.Tensor,
-               cache: Optional[CacheView], ws: "_abi.Workspace") -> torch.Tensor:
-        """RMSNorm + QKV + RoPE + cache phase + attention core.  Returns the pre-`wo` output [T, H*hd]."""
+               cache: Optional[CacheView], ws: "_abi.Workspace", lora_rows: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """RMSNorm + QKV + RoPE + cache phase + attention core.  Returns the pre-`wo` output [T, H*hd].  `lora_rows`: the adapter
+        slot of each token (LoraAdapter.call)."""
         T = x.shape[0]
         q = torch.empty(T, self.q_dim, dtype=x.dtype, device=x.device)
         k = torch.empty(T, self.kv_dim, dtype=x.dtype, device=x.device)
@@ -208,31 +219,31 @@ class Attention(nn.Module, _Fp8Rows, _Int4Rows):
         H, KV, hd = self.n_heads, self.n_kv_heads, self.head_dim
         if cache is None:
             # cache-less forward: unmasked over the whole flattened batch (SURVEY.md Appendix E-2)
-            self._qkv(x, norm_w, rope, positions, q, k, v, None, None, None, eps, ws)
+            self._qkv(x, norm_w, rope, positions, q, k, v, None, None, None, eps, ws, lora_rows)
             _abi.attn_prefill(q, k, v, None, None, None, None, out, 1, T, 0, H, KV, hd, causal=False)
             return out
         md = cache.metadata
         if cache.fp8:
-            return self._attend_fp8(x, norm_w, eps, rope, positions, cache, ws, q, k, v, out)
+            return self._attend_fp8(x, norm_w, eps, rope, positions, cache, ws, q, k, v, out, lora_rows)
         if md.prefill:
             # read the old ring, THEN write (transformer_layers.py:75-76)
-            self._qkv(x, norm_w, rope, positions, q, k, v, None, None, None, eps, ws)
+            self._qkv(x, norm_w, rope, positions, q, k, v, None, None, None, eps, ws, lora_rows)
             _abi.attn_prefill(q, k, v, cache.cache_k, cache.cache_v, md.q_start, md.seqpos, out, len(md.seqlens), md.max_seqlen,
                               md.window, H, KV, hd, causal=True, first_prefill=md.first_prefill)
             _abi.kv_ring_write(k, v, cache.cache_k, cache.cache_v, md.cache_rows, KV, hd)
         else:
             # write, THEN read the ring (transformer_layers.py:78-81); the scatter is the QKV kernel's epilogue
-            self._qkv(x, norm_w, rope, positions, q, k, v, cache.cache_k, cache.cache_v, md.cache_rows, eps, ws)
+            self._qkv(x, norm_w, rope, positions, q, k, v, cache.cache_k, cache.cache_v, md.cache_rows, eps, ws, lora_rows)
             B = len(md.seqlens)
             _abi.attn_decode(q, cache.cache_k, cache.cache_v, md.kv_len, out, H, KV, hd, decode_splits(B, KV, md.window), ws)
         return out
 
-    def _attend_fp8(self, x, norm_w, eps, rope, positions, cache: CacheView, ws, q, k, v, out) -> torch.Tensor:
+    def _attend_fp8(self, x, norm_w, eps, rope, positions, cache: CacheView, ws, q, k, v, out, lora_rows=None) -> torch.Tensor:
         """The FP8-cache model: k, v become k', v' (include/mistral_b200.h) right after RoPE, and attention sees only those."""
         H, KV, hd = self.n_heads, self.n_kv_heads, self.head_dim
         md = cache.metadata
         ring = (cache.cache_k, cache.cache_v, cache.cache_k_exp, cache.cache_v_exp)
-        self._qkv(x, norm_w, rope, positions, q, k, v, None, None, None, eps, ws)
+        self._qkv(x, norm_w, rope, positions, q, k, v, None, None, None, eps, ws, lora_rows)
         if md.prefill:
             # k', v' in place; read the old ring, THEN write it from k', v' (transformer_layers.py:75-76)
             _abi.kv_quantize(k, v, True)
@@ -246,7 +257,7 @@ class Attention(nn.Module, _Fp8Rows, _Int4Rows):
             _abi.attn_decode_fp8(q, *ring, md.kv_len, out, H, KV, hd, decode_splits(B, KV, md.window), ws)
         return out
 
-    def _qkv(self, x, norm_w, rope, positions, q, k, v, cache_k, cache_v, cache_rows, eps, ws) -> None:
+    def _qkv(self, x, norm_w, rope, positions, q, k, v, cache_k, cache_v, cache_rows, eps, ws, lora_rows=None) -> None:
         H, KV, hd = self.n_heads, self.n_kv_heads, self.head_dim
         if self.fp8:
             _abi.attn_qkv_fp8(x, norm_w, self.wqkv, self.wqkv_scale, rope, positions, q, k, v, cache_k, cache_v, cache_rows, H, KV, hd, eps, ws)
@@ -257,9 +268,10 @@ class Attention(nn.Module, _Fp8Rows, _Int4Rows):
             _abi.attn_qkv(x, norm_w, self.wqkv, rope, positions, q, k, v, cache_k, cache_v, cache_rows, H, KV, hd, eps, ws)
         else:
             _abi.attn_qkv_lora(x, norm_w, self.wqkv, rope, positions, q, k, v, cache_k, cache_v, cache_rows, H, KV, hd, eps, ws,
-                               self.wqkv_lora.call(x.shape[0]))
+                               self.wqkv_lora.call(x.shape[0], lora_rows))
 
-    def project_out(self, a: torch.Tensor, residual: torch.Tensor, out: torch.Tensor, ws: "_abi.Workspace") -> None:
+    def project_out(self, a: torch.Tensor, residual: torch.Tensor, out: torch.Tensor, ws: "_abi.Workspace",
+                    lora_rows: Optional[torch.Tensor] = None) -> None:
         """out = residual + wo(a)."""
         if self.fp8:
             _abi.linear_residual_fp8(a, self.wo_weight, self.wo_scale, residual, out, ws)
@@ -268,7 +280,7 @@ class Attention(nn.Module, _Fp8Rows, _Int4Rows):
         elif self.lora is None:
             _abi.linear_residual(a, self.wo_weight, residual, out, ws)
         else:
-            _abi.linear_residual_lora(a, self.wo_weight, residual, out, ws, self.wo_lora.call(a.shape[0]))
+            _abi.linear_residual_lora(a, self.wo_weight, residual, out, ws, self.wo_lora.call(a.shape[0], lora_rows))
 
 
 def decode_splits(B: int, KV: int, W: int, n_sm: int = 132) -> int:
@@ -282,7 +294,8 @@ def decode_splits(B: int, KV: int, W: int, n_sm: int = 132) -> int:
 class FeedForward(nn.Module, _Fp8Rows, _Int4Rows):
     """transformer_layers.py:96-106."""
 
-    def __init__(self, dim: int, hidden_dim: int, lora: Optional[LoraArgs] = None, fp8: bool = False, int4: bool = False):
+    def __init__(self, dim: int, hidden_dim: int, lora: Optional[LoraArgs] = None, fp8: bool = False, int4: bool = False,
+                 lora_slots: int = 1):
         super().__init__()
         self.dim = dim
         self.hidden_dim = hidden_dim
@@ -300,8 +313,8 @@ class FeedForward(nn.Module, _Fp8Rows, _Int4Rows):
             self.w2_weight = nn.Parameter(torch.empty(dim, hidden_dim), requires_grad=False)
         self.lora = lora
         if lora is not None:
-            self.w13_lora = LoraAdapter(dim, [hidden_dim, hidden_dim], lora, interleaved=True)
-            self.w2_lora = LoraAdapter(hidden_dim, [dim], lora)
+            self.w13_lora = LoraAdapter(dim, [hidden_dim, hidden_dim], lora, interleaved=True, slots=lora_slots)
+            self.w2_lora = LoraAdapter(hidden_dim, [dim], lora, slots=lora_slots)
 
     @property
     def w1(self) -> _WeightView:
@@ -343,8 +356,8 @@ class FeedForward(nn.Module, _Fp8Rows, _Int4Rows):
         raise ValueError(f"feed-forward Linear {name!r}")
 
     def run(self, x: torch.Tensor, norm_w: Optional[torch.Tensor], eps: float, residual: Optional[torch.Tensor],
-            ws: "_abi.Workspace") -> torch.Tensor:
-        """[norm] -> gate/up -> silu*mul -> down [+ residual]."""
+            ws: "_abi.Workspace", lora_rows: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """[norm] -> gate/up -> silu*mul -> down [+ residual].  `lora_rows`: the adapter slot of each token (LoraAdapter.call)."""
         T = x.shape[0]
         g = torch.empty(T, self.hidden_dim, dtype=x.dtype, device=x.device)
         out = torch.empty(T, self.dim, dtype=x.dtype, device=x.device)
@@ -358,8 +371,8 @@ class FeedForward(nn.Module, _Fp8Rows, _Int4Rows):
             _abi.ffn_gateup(x, norm_w, self.w13, g, eps, ws)
             _abi.linear_residual(g, self.w2_weight, residual, out, ws)
         else:
-            _abi.ffn_gateup_lora(x, norm_w, self.w13, g, eps, ws, self.w13_lora.call(T))
-            _abi.linear_residual_lora(g, self.w2_weight, residual, out, ws, self.w2_lora.call(T))
+            _abi.ffn_gateup_lora(x, norm_w, self.w13, g, eps, ws, self.w13_lora.call(T, lora_rows))
+            _abi.linear_residual_lora(g, self.w2_weight, residual, out, ws, self.w2_lora.call(T, lora_rows))
         return out
 
     def forward(self, x: torch.Tensor, ws: Optional["_abi.Workspace"] = None) -> torch.Tensor:
@@ -385,8 +398,9 @@ class TransformerBlock(nn.Module):
 
     def __init__(self, dim: int, hidden_dim: int, n_heads: int, n_kv_heads: int, head_dim: int, norm_eps: float,
                  lora: Optional[LoraArgs] = None, moe: Optional[MoeArgs] = None, expert_shard: Tuple[int, int] = (0, 1), expert_group=None,
-                 expert_weights: str = "bf16", dense_weights: str = "bf16"):
+                 expert_weights: str = "bf16", dense_weights: str = "bf16", lora_slots: int = 1):
         super().__init__()
+        assert lora_slots == 1 or (lora is not None and moe is None), "a bank of adapter slots: dense layers with un-merged LoRA only"
         if lora is not None and moe is not None:
             check_moe_lora(expert_weights, dense_weights)
         self.n_heads = n_heads
@@ -396,7 +410,8 @@ class TransformerBlock(nn.Module):
         assert not (fp8 or int4) or lora is None, "quantised dense weights: layers without un-merged LoRA only"
         assert not fp8 or moe is None, "FP8 dense weights: dense layers only"
         # on a MoE block INT4 dense weights are the attention Linears only; the experts follow expert_weights
-        self.attention = Attention(dim=dim, n_heads=n_heads, head_dim=head_dim, n_kv_heads=n_kv_heads, lora=lora, fp8=fp8, int4=int4)
+        self.attention = Attention(dim=dim, n_heads=n_heads, head_dim=head_dim, n_kv_heads=n_kv_heads, lora=lora, fp8=fp8, int4=int4,
+                                   lora_slots=lora_slots)
         self.attention_norm = RMSNorm(dim, eps=norm_eps)
         self.ffn_norm = RMSNorm(dim, eps=norm_eps)
         self.feed_forward: nn.Module
@@ -408,16 +423,17 @@ class TransformerBlock(nn.Module):
                                          gate_weight=nn.Parameter(torch.empty(moe.num_experts, dim), requires_grad=False), moe_args=moe,
                                          expert_shard=expert_shard, expert_group=expert_group)
         else:
-            self.feed_forward = FeedForward(dim=dim, hidden_dim=hidden_dim, lora=lora, fp8=fp8, int4=int4)
+            self.feed_forward = FeedForward(dim=dim, hidden_dim=hidden_dim, lora=lora, fp8=fp8, int4=int4, lora_slots=lora_slots)
 
     def forward(self, x: torch.Tensor, rope: torch.Tensor, positions: torch.Tensor, cache: Optional[CacheView],
-                ws: "_abi.Workspace") -> torch.Tensor:
+                ws: "_abi.Workspace", lora_rows: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """`lora_rows`: int32 [T] on the device, the adapter slot of each token (-1: none), or None for the unmasked adapter."""
         # r = attention(attention_norm(x)); h = x + r        (transformer_layers.py:165-166)
-        a = self.attention.attend(x, self.attention_norm.weight, self.norm_eps, rope, positions, cache, ws)
+        a = self.attention.attend(x, self.attention_norm.weight, self.norm_eps, rope, positions, cache, ws, lora_rows)
         h = torch.empty_like(x)
-        self.attention.project_out(a, x, h, ws)
+        self.attention.project_out(a, x, h, ws, lora_rows)
         # r = feed_forward(ffn_norm(h)); out = h + r          (transformer_layers.py:167-168)
         if isinstance(self.feed_forward, MoeLayer):
             hn = _abi.rmsnorm(h, self.ffn_norm.weight, self.norm_eps)
             return self.feed_forward.run(hn, h, ws)  # router + grouped experts + ordered combine + residual, no host sync
-        return self.feed_forward.run(h, self.ffn_norm.weight, self.norm_eps, h, ws)
+        return self.feed_forward.run(h, self.ffn_norm.weight, self.norm_eps, h, ws, lora_rows)
