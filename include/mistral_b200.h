@@ -30,7 +30,7 @@
 extern "C" {
 #endif
 
-#define MB200_ABI_VERSION 3
+#define MB200_ABI_VERSION 4
 
 #define MB200_OK 0
 #define MB200_E_INVALID (-1)   /* bad argument / unsupported shape */
@@ -548,6 +548,45 @@ int mb200_decode_step_fp8(const mb200_layer_desc_fp8* layers_dev, const int32_t*
                           int64_t n_kv_heads, int64_t head_dim, int64_t vocab, float eps, void* workspace, size_t workspace_bytes, void* stream);
 int mb200_decode_step_fp8_supported(int64_t dim, int64_t hidden, int64_t n_heads, int64_t n_kv_heads, int64_t head_dim, int64_t vocab,
                                     int64_t smem_optin);
+
+/* ---------------------------------------------------------------------------------------------
+ * FP8 activations for FP8 dense weights (Python: Transformer(..., dense_weights="fp8", prefill_compute="fp8")).  Opt-in numeric
+ * mode of the prefill-sized Linears: both GEMM operands are e4m3 and the product runs on the FP8 tensor cores.
+ *
+ * Which calls.  Every call of the three _fp8a8 entry points that the _fp8 dispatch above would give to the prefill wgmma kernel
+ * (T >= 128 and not stream-K; stream-K takes T <= 128 when N % 128 == 0, so T >= 129 for every Linear of the real shapes).  Every
+ * other call (GEMV, stream-K, small-batch wgmma) is the _fp8 entry point's call, kernel and bits.  The rule depends on the call's
+ * token count only: chunks of <= 128 tokens compute exactly what the FP8 model computes.
+ *
+ * Activations.  Row t of the Linear's bf16 input v (wqkv, w13: the RMSNorm output, the same bf16 values mb200_rmsnorm gives; wo, w2:
+ * x itself), in fp32:
+ *     a[t]      = max_k |v[t, k]|
+ *     e[t]      = 0 if a[t] == 0, else the smallest integer with a[t] <= 448 * 2^e[t]     (int32, in [-141, 120] for bf16 inputs)
+ *     xq[t, k]  = e4m3fn_rn(v[t, k] * 2^-e[t])       (the power of two scales exactly: the e4m3 rounding is the only one)
+ *     A row holding an inf or a NaN gets e[t] = 0 and every xq[t, k] = NaN (0x7f): every output of that token is NaN.
+ * Product.  The tensor cores sum each k-block of 128 products float(xq[t, k]) * float(q[n, k]) (k = 128 j .. 128 j + 127) from
+ *     zero, and each block sum is added into an IEEE fp32 accumulator on the CUDA cores, blocks in ascending order (promotion
+ *     interval: one k-block of 128).  Inside a k-block the sum is the tensor core's, about 14 significant bits wide: on an H100
+ *     (tests/test_gpu_fp8_prefill.py) the block sum of 2^16 + 2^j keeps 2^j for j >= 3 and drops it for j <= 2.  It is exact
+ *     whenever every product and partial sum of the block is a multiple of a power of two p and below 2^13 * p.
+ *         acc[t, n] = fp32 sum over j of block_j[t, n]
+ * Output.  y[t, n] = bf16(fp32(fp32(s[n] * acc[t, n]) * 2^e[t])), then the mode's own epilogue exactly as in the _fp8 entry
+ *     points (residual add, SiLU * mul, RoPE + ring scatter).
+ *
+ * mb200_attn_qkv_fp8a8, mb200_ffn_gateup_fp8a8, mb200_linear_residual_fp8a8: the _fp8 signatures.  A call in the FP8-activation
+ *     regime needs K % 128 == 0 and N % 64 == 0 (MB200_E_INVALID otherwise) and writes xq and e into the normed-activation scratch
+ *     of the workspace (mb200_workspace_bytes is unchanged).
+ * mb200_quantize_act_e4m3: xq (e4m3 [T, dim], 8-byte aligned) and e (int32 [T]) of x (bf16 [T, dim], dim % 8 == 0), or of its RMSNorm
+ *     output with weight norm_w when norm_w is not NULL.  The quantiser the entry points above run.
+ */
+int mb200_attn_qkv_fp8a8(const void* x, const void* norm_w, const void* w_q, const float* w_scale, const float* rope, const int32_t* positions,
+                         void* q_out, void* k_out, void* v_out, void* cache_k, void* cache_v, const int32_t* cache_rows, int64_t T, int64_t dim,
+                         int64_t n_heads, int64_t n_kv_heads, int64_t head_dim, float eps, void* workspace, size_t workspace_bytes, void* stream);
+int mb200_ffn_gateup_fp8a8(const void* x, const void* norm_w, const void* w_q, const float* w_scale, void* g_out, int64_t T, int64_t dim,
+                           int64_t hidden, float eps, void* workspace, size_t workspace_bytes, void* stream);
+int mb200_linear_residual_fp8a8(const void* x, const void* w_q, const float* w_scale, const void* residual, void* out, int64_t T, int64_t N,
+                                int64_t K, void* workspace, size_t workspace_bytes, void* stream);
+int mb200_quantize_act_e4m3(const void* x, const void* norm_w, void* q, int32_t* exps, int64_t T, int64_t dim, float eps, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * INT4 dense weights (Python: Transformer(..., dense_weights="int4")).  Each layer Linear's weight W [N, K] (K % 128 == 0) is

@@ -15,7 +15,7 @@ import torch
 _LIB_PATH = Path(os.environ.get("MB200_LIB_PATH") or Path(__file__).resolve().parent / "libmb200.so")  # override: A/B builds of experiments
 _lib: Optional[ctypes.CDLL] = None
 
-ABI_VERSION = 3
+ABI_VERSION = 4
 SKINNY_MAX_T = 4
 WORKSPACE_HEADER_BYTES = 64 * 1024
 
@@ -94,6 +94,13 @@ _SIGNATURES = {
                                      c_size_t, c_void_p]),
     "mb200_linear_residual_fp8": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_void_p,
                                           c_size_t, c_void_p]),
+    "mb200_attn_qkv_fp8a8": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                     c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int64, c_int64, c_float, c_void_p, c_size_t, c_void_p]),
+    "mb200_ffn_gateup_fp8a8": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_float, c_void_p,
+                                       c_size_t, c_void_p]),
+    "mb200_linear_residual_fp8a8": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_void_p,
+                                            c_size_t, c_void_p]),
+    "mb200_quantize_act_e4m3": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_float, c_void_p]),
     "mb200_decode_step_fp8": (c_int, [c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64,
                                       c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int64, c_int64, c_int64, c_float, c_void_p, c_size_t,
                                       c_void_p]),
@@ -316,28 +323,40 @@ def _check_fp8(w_q: torch.Tensor, w_scale: torch.Tensor) -> None:
 
 
 def attn_qkv_fp8(x, norm_w, w_q, w_scale, rope, positions, q_out, k_out, v_out, cache_k, cache_v, cache_rows, n_heads, n_kv_heads, head_dim,
-                 eps, ws: Workspace) -> None:
+                 eps, ws: Workspace, *, a8: bool = False) -> None:
+    """a8: the prefill-sized calls take FP8 activations (mb200_attn_qkv_fp8a8); every other call is the same as without."""
     _check_fp8(w_q, w_scale)
     T, dim = x.shape
-    _check(lib().mb200_attn_qkv_fp8(_ptr(x), _ptr(norm_w), _ptr(w_q), _ptr(w_scale), _ptr(rope), _ptr(positions), _ptr(q_out), _ptr(k_out),
-                                    _ptr(v_out), _ptr(cache_k), _ptr(cache_v), _ptr(cache_rows), T, dim, n_heads, n_kv_heads, head_dim, eps,
-                                    ws.ptr, ws.nbytes, _stream()), "mb200_attn_qkv_fp8")
+    fn, name = (lib().mb200_attn_qkv_fp8a8, "mb200_attn_qkv_fp8a8") if a8 else (lib().mb200_attn_qkv_fp8, "mb200_attn_qkv_fp8")
+    _check(fn(_ptr(x), _ptr(norm_w), _ptr(w_q), _ptr(w_scale), _ptr(rope), _ptr(positions), _ptr(q_out), _ptr(k_out), _ptr(v_out), _ptr(cache_k),
+              _ptr(cache_v), _ptr(cache_rows), T, dim, n_heads, n_kv_heads, head_dim, eps, ws.ptr, ws.nbytes, _stream()), name)
 
 
-def ffn_gateup_fp8(x, norm_w, w_q, w_scale, g_out, eps, ws: Workspace) -> None:
+def ffn_gateup_fp8(x, norm_w, w_q, w_scale, g_out, eps, ws: Workspace, *, a8: bool = False) -> None:
     _check_fp8(w_q, w_scale)
     T, dim = x.shape
     hidden = w_q.shape[0] // 2
-    _check(lib().mb200_ffn_gateup_fp8(_ptr(x), _ptr(norm_w), _ptr(w_q), _ptr(w_scale), _ptr(g_out), T, dim, hidden, eps, ws.ptr, ws.nbytes,
-                                      _stream()), "mb200_ffn_gateup_fp8")
+    fn, name = (lib().mb200_ffn_gateup_fp8a8, "mb200_ffn_gateup_fp8a8") if a8 else (lib().mb200_ffn_gateup_fp8, "mb200_ffn_gateup_fp8")
+    _check(fn(_ptr(x), _ptr(norm_w), _ptr(w_q), _ptr(w_scale), _ptr(g_out), T, dim, hidden, eps, ws.ptr, ws.nbytes, _stream()), name)
 
 
-def linear_residual_fp8(x, w_q, w_scale, residual, out, ws: Workspace) -> None:
+def linear_residual_fp8(x, w_q, w_scale, residual, out, ws: Workspace, *, a8: bool = False) -> None:
     _check_fp8(w_q, w_scale)
     T, K = x.shape
     N = w_q.shape[0]
-    _check(lib().mb200_linear_residual_fp8(_ptr(x), _ptr(w_q), _ptr(w_scale), _ptr(residual), _ptr(out), T, N, K, ws.ptr, ws.nbytes,
-                                           _stream()), "mb200_linear_residual_fp8")
+    fn, name = ((lib().mb200_linear_residual_fp8a8, "mb200_linear_residual_fp8a8") if a8
+                else (lib().mb200_linear_residual_fp8, "mb200_linear_residual_fp8"))
+    _check(fn(_ptr(x), _ptr(w_q), _ptr(w_scale), _ptr(residual), _ptr(out), T, N, K, ws.ptr, ws.nbytes, _stream()), name)
+
+
+def quantize_act_e4m3(x: torch.Tensor, norm_w: Optional[torch.Tensor] = None, eps: float = 0.0):
+    """(xq uint8 [T, dim], e int32 [T]): the per-token e4m3 activations of x, or of its RMSNorm output with norm_w (include/mistral_b200.h)."""
+    assert x.dtype == torch.bfloat16 and x.dim() == 2 and x.is_contiguous(), (x.dtype, x.shape)
+    T, dim = x.shape
+    q = torch.empty(T, dim, dtype=torch.uint8, device=x.device)
+    e = torch.empty(T, dtype=torch.int32, device=x.device)
+    _check(lib().mb200_quantize_act_e4m3(_ptr(x), _ptr(norm_w), _ptr(q), _ptr(e), T, dim, eps, _stream()), "mb200_quantize_act_e4m3")
+    return q, e
 
 
 # ---- INT4 dense weights (include/mistral_b200.h): w_q the packed codes uint8 [N, K/2], w_gscale the bf16 group scales [N, K/128] ----

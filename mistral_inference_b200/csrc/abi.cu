@@ -12,6 +12,7 @@
 #include "gemm_mma.cuh"
 #include "gemm_streamk.cuh"
 #include "gemm_wgmma.cuh"
+#include "gemm_wgmma_a8.cuh"
 #include "int4.cuh"
 #include "kv_fp8.cuh"
 #include "lora.cuh"
@@ -125,9 +126,12 @@ static int run_linear(const void* x, const void* norm_w, const void* w, const Ep
 // gemm_mma_kernel is refused (that kernel has no quantised variant).  One function for both formats, so the regime choice lives here
 // once.  FP8 (INT4 = false): w is e4m3 [N, K], epi.w_scale its fp32 row scales, applied by the epilogue (EPI_WSCALE).  INT4: w is
 // the packed code matrix [N, K/2], gscale its bf16 group scales [N, K/128]; the kernels convert to W' and keep the bf16 epilogue.
-template <int MODE, bool INT4>
+// A8 (FP8 only): the calls that would run the prefill wgmma kernel (T >= 128, not stream-K) quantise their input per token into the
+// workspace and run the e4m3 x e4m3 kernel instead; every other call is the FP8 call unchanged.
+template <int MODE, bool INT4, bool A8 = false>
 static int run_linear_quant(const void* x, const void* norm_w, const void* w, const uint16_t* gscale, const EpiParams& epi, int64_t T,
                             int64_t N, int64_t K, float eps, void* workspace, size_t workspace_bytes, cudaStream_t st) {
+  static_assert(!(A8 && INT4), "FP8 activations: FP8 weights only");
   const char* fmt = INT4 ? "int4" : "fp8";
   constexpr int KMODE = INT4 ? MODE : (MODE | EPI_WSCALE);  // the kernels' epilogue mode
   MB_CHECK_ARG(T >= 1, "linear (%s): T=%lld", fmt, (long long)T);
@@ -158,6 +162,27 @@ static int run_linear_quant(const void* x, const void* norm_w, const void* w, co
   const bool sk = streamk_eligible(T, N, K);
   MB_CHECK_ARG(sk || wgmma_gemm_eligible(T, N, K), "linear (%s): T=%lld N=%lld K=%lld needs the mma.sync GEMM, which has no %s variant", fmt,
                (long long)T, (long long)N, (long long)K, INT4 ? "int4" : "e4m3");
+  if constexpr (A8) {
+    if (!sk && T >= A8_BM) {
+      MB_CHECK_ARG(a8_gemm_eligible(T, N, K), "linear (fp8 activations): N=%lld K=%lld (K must be a multiple of 128 and N of 64)", (long long)N,
+                   (long long)K);
+      const WsActE4m3 r = ws_act_e4m3(T, K);
+      if (workspace == nullptr || workspace_bytes < r.exps.end())
+        return fail(MB200_E_WORKSPACE, "linear: workspace %zu < %zu", workspace_bytes, r.exps.end());
+      uint8_t* xq = (uint8_t*)workspace + r.q.offset;
+      int32_t* exps = (int32_t*)((uint8_t*)workspace + r.exps.offset);
+      int rc = launch_quantize_act(x, norm_w, xq, exps, T, K, eps, st);
+      if (rc) return rc;
+      GemmParams g;
+      g.a = xq;
+      g.w = w;
+      g.T = (int)T;
+      g.N = (int)N;
+      g.K = (int)K;
+      g.epi = epi;
+      return launch_gemm_wgmma_a8<KMODE | EPI_ASCALE>(g, exps, st);
+    }
+  }
   const void* a = x;
   if (norm_w) {
     const WsRegion nr = ws_normed(T, K);
@@ -280,7 +305,8 @@ int mb200_rmsnorm(const void* x, const void* w, void* out, int64_t T, int64_t di
 static int attn_qkv_impl(const void* x, const void* norm_w, const void* wqkv, const float* rope, const int32_t* positions, void* q_out,
                          void* k_out, void* v_out, void* cache_k, void* cache_v, const int32_t* cache_rows, int64_t T, int64_t dim,
                          int64_t n_heads, int64_t n_kv_heads, int64_t head_dim, float eps, void* workspace, size_t workspace_bytes,
-                         void* stream, const mb200_lora* lora, const float* w_scale = nullptr, const uint16_t* w_gscale = nullptr) {
+                         void* stream, const mb200_lora* lora, const float* w_scale = nullptr, const uint16_t* w_gscale = nullptr,
+                         bool a8 = false) {
   MB_CHECK_ARG(x && norm_w && wqkv && rope && positions && q_out && k_out && v_out, "attn_qkv: null pointer");
   MB_CHECK_ARG(head_dim == kHeadDim || head_dim == 64, "attn_qkv: head_dim=%lld unsupported (64 or 128)", (long long)head_dim);
   MB_CHECK_ARG(cache_rows == nullptr || (cache_k && cache_v), "attn_qkv: cache_rows without cache pointers");
@@ -299,6 +325,8 @@ static int attn_qkv_impl(const void* x, const void* norm_w, const void* wqkv, co
   const int64_t N = (n_heads + 2 * n_kv_heads) * head_dim;
   if (w_scale) {
     e.w_scale = w_scale;
+    if (a8)
+      return run_linear_quant<EPI_QKV_ROPE, false, true>(x, norm_w, wqkv, nullptr, e, T, N, dim, eps, workspace, workspace_bytes, (cudaStream_t)stream);
     return run_linear_quant<EPI_QKV_ROPE, false>(x, norm_w, wqkv, nullptr, e, T, N, dim, eps, workspace, workspace_bytes, (cudaStream_t)stream);
   }
   if (w_gscale) return run_linear_quant<EPI_QKV_ROPE, true>(x, norm_w, wqkv, w_gscale, e, T, N, dim, eps, workspace, workspace_bytes,
@@ -644,6 +672,45 @@ int mb200_ffn_gateup_fp8(const void* x, const void* norm_w, const void* w_q, con
   e.ld_out = hidden;
   e.w_scale = w_scale;
   return run_linear_quant<EPI_SWIGLU, false>(x, norm_w, w_q, nullptr, e, T, 2 * hidden, dim, eps, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+int mb200_attn_qkv_fp8a8(const void* x, const void* norm_w, const void* w_q, const float* w_scale, const float* rope, const int32_t* positions,
+                         void* q_out, void* k_out, void* v_out, void* cache_k, void* cache_v, const int32_t* cache_rows, int64_t T, int64_t dim,
+                         int64_t n_heads, int64_t n_kv_heads, int64_t head_dim, float eps, void* workspace, size_t workspace_bytes, void* stream) {
+  MB_CHECK_ARG(w_scale, "attn_qkv_fp8a8: null scale");
+  return attn_qkv_impl(x, norm_w, w_q, rope, positions, q_out, k_out, v_out, cache_k, cache_v, cache_rows, T, dim, n_heads, n_kv_heads,
+                       head_dim, eps, workspace, workspace_bytes, stream, nullptr, w_scale, nullptr, true);
+}
+
+int mb200_linear_residual_fp8a8(const void* x, const void* w_q, const float* w_scale, const void* residual, void* out, int64_t T, int64_t N,
+                                int64_t K, void* workspace, size_t workspace_bytes, void* stream) {
+  MB_CHECK_ARG(x && w_q && w_scale && out, "linear_residual_fp8a8: null pointer");
+  EpiParams e;
+  e.out = out;
+  e.residual = residual;
+  e.ld_out = N;
+  e.w_scale = w_scale;
+  if (residual)
+    return run_linear_quant<EPI_RESIDUAL, false, true>(x, nullptr, w_q, nullptr, e, T, N, K, 0.f, workspace, workspace_bytes, (cudaStream_t)stream);
+  return run_linear_quant<EPI_STORE, false, true>(x, nullptr, w_q, nullptr, e, T, N, K, 0.f, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+int mb200_ffn_gateup_fp8a8(const void* x, const void* norm_w, const void* w_q, const float* w_scale, void* g_out, int64_t T, int64_t dim,
+                           int64_t hidden, float eps, void* workspace, size_t workspace_bytes, void* stream) {
+  MB_CHECK_ARG(x && w_q && w_scale && g_out, "ffn_gateup_fp8a8: null pointer");
+  EpiParams e;
+  e.out = g_out;
+  e.ld_out = hidden;
+  e.w_scale = w_scale;
+  return run_linear_quant<EPI_SWIGLU, false, true>(x, norm_w, w_q, nullptr, e, T, 2 * hidden, dim, eps, workspace, workspace_bytes,
+                                                   (cudaStream_t)stream);
+}
+
+int mb200_quantize_act_e4m3(const void* x, const void* norm_w, void* q, int32_t* exps, int64_t T, int64_t dim, float eps, void* stream) {
+  MB_CHECK_ARG(x && q && exps, "quantize_act_e4m3: null pointer");
+  MB_CHECK_ARG(((uintptr_t)x & 15) == 0 && ((uintptr_t)norm_w & 15) == 0 && ((uintptr_t)q & 7) == 0 && ((uintptr_t)exps & 3) == 0,
+               "quantize_act_e4m3: misaligned pointer");
+  return launch_quantize_act(x, norm_w, (uint8_t*)q, exps, T, dim, eps, (cudaStream_t)stream);
 }
 
 int mb200_attn_qkv_int4(const void* x, const void* norm_w, const void* w_q, const void* w_gscale, const float* rope, const int32_t* positions,

@@ -29,6 +29,13 @@ constexpr int EPI_LORA = 16;
 //   y = bf16(fp32(w_scale[n] * acc))
 // Instantiations without the flag compile to the same code as before.
 constexpr int EPI_WSCALE = 32;
+// Flag OR-ed with EPI_WSCALE: FP8 activations (prefill_compute="fp8", include/mistral_b200.h).  The accumulator is
+// sum_k float(xq[t, k]) * float(q[n, k]) over the per-token e4m3 activations xq = e4m3(x * 2^-e[t]); the token's power of two
+// (the `ascale` argument of epi_pair, 2^e[t]) comes back after the row scale as one fp32 product:
+//   y = bf16(fp32(fp32(w_scale[n] * acc) * 2^e[t]))
+// The exponents travel as a kernel argument of their own, so EpiParams and the code of instantiations without the flag are
+// unchanged.
+constexpr int EPI_ASCALE = 128;  // 64 is SKINNY_SLOT_MASK
 
 constexpr int kMaxPeers = 8;
 
@@ -63,14 +70,22 @@ struct EpiParams {
   const float* w_scale = nullptr;  // fp32 [N]
 };
 
+// 2^e as an fp32 number for e in [-149, 127] (subnormal below -126): exact, so a product with it rounds once
+__device__ __forceinline__ float exp2_exact(int e) { return __int_as_float(e >= -126 ? (e + 127) << 23 : 1 << (e + 149)); }
+
 template <int FLAGS>
-__device__ __forceinline__ void epi_pair(const EpiParams& p, int t, int n, float acc0, float acc1) {
-  constexpr int MODE = FLAGS & ~(EPI_LORA | EPI_WSCALE);
+__device__ __forceinline__ void epi_pair(const EpiParams& p, int t, int n, float acc0, float acc1, float ascale = 1.f) {
+  constexpr int MODE = FLAGS & ~(EPI_LORA | EPI_WSCALE | EPI_ASCALE);
   if constexpr ((FLAGS & EPI_WSCALE) != 0) {
     static_assert(MODE == EPI_STORE || MODE == EPI_RESIDUAL || MODE == EPI_SWIGLU || MODE == EPI_QKV_ROPE, "FP8 row scale: unsupported mode");
     const float2 s = *reinterpret_cast<const float2*>(p.w_scale + n);
     acc0 = __fmul_rn(s.x, acc0);
     acc1 = __fmul_rn(s.y, acc1);
+  }
+  if constexpr ((FLAGS & EPI_ASCALE) != 0) {
+    static_assert((FLAGS & (EPI_WSCALE | EPI_LORA)) == EPI_WSCALE, "FP8 activations: FP8 dense weights without LoRA only");
+    acc0 = __fmul_rn(acc0, ascale);
+    acc1 = __fmul_rn(acc1, ascale);
   }
   // the Linear's own output rounding (bf16 result of nn.Linear)
   float y0 = round_bf16(acc0), y1 = round_bf16(acc1);

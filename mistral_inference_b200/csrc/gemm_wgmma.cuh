@@ -182,6 +182,44 @@ __device__ __forceinline__ void epi_fragment(const EpiParams& epi, const float (
   }
 }
 
+// Tile order of the persistent GEMMs.  The persistent CTAs take tiles t = cta, cta + n_cta, ...: at any moment ~n_cta consecutive
+// tile ids are in flight, in lock step through K.  With few m units the walk is m-fastest: the CTAs that share a W tile run together.
+// With many (a 32 x 1024-token prefill: A = 335 MB; a Mixtral prefill: hundreds of MB of gathered rows, far beyond the 50 MB L2)
+// m-fastest makes every CTA stream its own A tile from DRAM once per n tile.  There the in-flight set is shaped as a GM x GN block
+// instead (GM m units share each W tile, GN n tiles share each A tile): DRAM traffic per tile drops ~4x.
+template <int kGM, int kGN>
+__device__ __forceinline__ void tile_walk_mn(int tile, int num_m, int num_n, int& mu, int& nt) {
+  if (num_m <= 16) {
+    mu = tile % num_m;
+    nt = tile / num_m;
+    return;
+  }
+  const int per_row = kGN * num_m, rows_full = num_n / kGN;  // an "n-block row": all m units x kGN n tiles
+  int nb, r, gn;
+  if (tile < rows_full * per_row) {
+    nb = tile / per_row;
+    r = tile % per_row;
+    gn = kGN;
+  } else {
+    nb = rows_full;
+    r = tile - rows_full * per_row;
+    gn = num_n - rows_full * kGN;
+  }
+  const int blk = kGM * gn, mb_full = num_m / kGM;
+  int mblk, q, gm;
+  if (r < mb_full * blk) {
+    mblk = r / blk;
+    q = r % blk;
+    gm = kGM;
+  } else {
+    mblk = mb_full;
+    q = r - mb_full * blk;
+    gm = num_m - mb_full * kGM;
+  }
+  mu = mblk * kGM + q % gm;
+  nt = nb * kGN + q / gm;
+}
+
 // CL = 2: thread-block clusters of two CTAs that work on vertically adjacent tiles (same W columns, consecutive 128-row blocks).
 // Each CTA fetches HALF of the shared [256 x 64] W tile and TMA-multicasts it into both shared memories, so the L2 -> SM traffic
 // per CTA and k-block drops from 48 KB to 32 KB.  A stage may be refilled only when BOTH CTAs' consumers have read it: the empty
@@ -236,43 +274,8 @@ __device__ __forceinline__ void tc_gemm_body(const CUtensorMap& map_a, const CUt
   const int num_n = p.N / BN, num_tiles = num_m * num_n, num_k = p.K / TG_BK;
   const int32_t* tile_expert = GROUPED ? plan + MOE_PLAN_HEADER + (CL > 1 ? 2 * plan[2] : 0) : nullptr;
   const int32_t* tile_row0 = GROUPED ? tile_expert + plan[2] : nullptr;
-  // Tile order.  The persistent CTAs take tiles t = cta, cta + n_cta, ...: at any moment ~n_cta consecutive tile ids are in flight,
-  // in lock step through K.  With few m units the walk is m-fastest: the CTAs that share a W tile run together.  With many (a
-  // 32 x 1024-token prefill: A = 335 MB; a Mixtral prefill: hundreds of MB of gathered rows, far beyond the 50 MB L2) m-fastest
-  // makes every CTA stream its own A tile from DRAM once per n tile.  There the in-flight set is shaped as a GM x GN block instead
-  // (GM m units share each W tile, GN n tiles share each A tile): DRAM traffic per tile drops ~4x.
   constexpr int kGM = CL > 1 ? 8 : 12, kGN = CL > 1 ? 9 : 12;
-  auto tile_mn = [&](int tile, int& mu, int& nt) {
-    if (num_m <= 16) {
-      mu = tile % num_m;
-      nt = tile / num_m;
-      return;
-    }
-    const int per_row = kGN * num_m, rows_full = num_n / kGN;  // an "n-block row": all m units x kGN n tiles
-    int nb, r, gn;
-    if (tile < rows_full * per_row) {
-      nb = tile / per_row;
-      r = tile % per_row;
-      gn = kGN;
-    } else {
-      nb = rows_full;
-      r = tile - rows_full * per_row;
-      gn = num_n - rows_full * kGN;
-    }
-    const int blk = kGM * gn, mb_full = num_m / kGM;
-    int mblk, q, gm;
-    if (r < mb_full * blk) {
-      mblk = r / blk;
-      q = r % blk;
-      gm = kGM;
-    } else {
-      mblk = mb_full;
-      q = r - mb_full * blk;
-      gm = num_m - mb_full * kGM;
-    }
-    mu = mblk * kGM + q % gm;
-    nt = nb * kGN + q / gm;
-  };
+  auto tile_mn = [&](int tile, int& mu, int& nt) { tile_walk_mn<kGM, kGN>(tile, num_m, num_n, mu, nt); };
   // first row of this CTA's m tile of unit `u` (cluster rank 1 takes the pair's second tile; a missing second tile is recomputed
   // from the first one's rows and not stored)
   auto grouped_m0 = [&](int u, bool& store) {

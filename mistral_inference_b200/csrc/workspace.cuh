@@ -45,6 +45,16 @@ static_assert(ws_header_regions_disjoint(), "workspace header regions overlap or
 constexpr WsRegion kWsSkPartials = {kWsHeader, SK_PARTIAL_BYTES};
 // Activations normed once for a tensor-core GEMM ([T, K] bf16): after the stream-K slots, which that GEMM may use.
 inline WsRegion ws_normed(int64_t T, int64_t K) { return {kWsSkPartials.end(), align256((size_t)T * K * 2)}; }
+// FP8 activations (prefill_compute="fp8") in the same region: e4m3 codes [T, K], then the int32 exponents [T] on a 256-byte
+// boundary.  T*K rounded up to 256 plus 4T bytes fit in the 2*T*K bytes of ws_normed for every K >= 128.
+struct WsActE4m3 {
+  WsRegion q, exps;
+};
+inline WsActE4m3 ws_act_e4m3(int64_t T, int64_t K) {
+  const WsRegion nr = ws_normed(T, K);
+  const WsRegion q = {nr.offset, align256((size_t)T * K)};
+  return {q, {q.end(), (size_t)T * sizeof(int32_t)}};
+}
 // Split-KV decode attention partials: [B, KV, S, rep, hd + 2] fp32 (m, l, acc).
 inline WsRegion ws_splitkv_partials(int64_t B, int64_t KV, int64_t S, int64_t rep) {
   return {kWsHeader, (size_t)B * KV * S * rep * (kHeadDim + 2) * sizeof(float)};

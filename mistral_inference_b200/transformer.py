@@ -67,6 +67,25 @@ class _OutputView:
 
 
 DENSE_WEIGHTS = ("bf16", "fp8", "int4")
+PREFILL_COMPUTE = ("bf16", "fp8")
+
+
+def _check_prefill_compute(args: TransformerArgs, prefill_compute: str, dense_weights: str) -> None:
+    """The refusals of prefill_compute="fp8", before anything is allocated (after _check_dense_weights)."""
+    if prefill_compute not in PREFILL_COMPUTE:
+        raise ValueError(f"prefill_compute={prefill_compute!r}: expected one of {PREFILL_COMPUTE}")
+    if prefill_compute == "bf16":
+        return
+    if dense_weights != "fp8":
+        raise ValueError(f"prefill_compute='fp8' needs dense_weights='fp8' (got {dense_weights!r}): the FP8 tensor-core GEMM multiplies "
+                         "e4m3 activations by e4m3 weights")
+    # the e4m3 x e4m3 kernel reads 128-element k-blocks and 64- or 128-wide tiles (include/mistral_b200.h)
+    q_dim, kv_dim = args.n_heads * args.head_dim, args.n_kv_heads * args.head_dim
+    for name, N, K in [("wqkv", q_dim + 2 * kv_dim, args.dim), ("wo", args.dim, q_dim), ("w13", 2 * args.hidden_dim, args.dim),
+                       ("w2", args.dim, args.hidden_dim)]:
+        if K % 128 != 0 or N % 64 != 0:
+            raise ValueError(f"prefill_compute='fp8': {name} [{N}, {K}] does not fit the FP8 tensor-core GEMM (K must be a multiple of "
+                             "128 and N of 64)")
 
 
 def _check_dense_weights(args: TransformerArgs, dense_weights: str, expert_weights: str) -> None:
@@ -103,7 +122,7 @@ def _check_dense_weights(args: TransformerArgs, dense_weights: str, expert_weigh
 class Transformer(nn.Module):
     def __init__(self, args: TransformerArgs, pipeline_rank: int = 0, num_pipeline_ranks: int = 1, softmax_fp32: bool = True,
                  expert_parallel: Optional[Tuple[int, int]] = None, expert_group: Any = None, expert_weights: str = "bf16", *,
-                 kv_cache: str = "bf16", dense_weights: str = "bf16", lora_slots: int = 1):
+                 kv_cache: str = "bf16", dense_weights: str = "bf16", lora_slots: int = 1, prefill_compute: str = "bf16"):
         """Same signature as the reference (transformer.py:34-40) plus `expert_parallel = (rank, world)`: MoE experts sharded
         `e % world == rank` over the ranks of `expert_group` (default process group), everything else replicated, one
         all-reduce of [T, dim] per MoE layer (SURVEY.md 8e); and `expert_weights`: "bf16", or "fp8" to store every MoE expert
@@ -119,7 +138,11 @@ class Transformer(nn.Module):
         bf16 model computes with the dequantised weights W' (include/mistral_b200.h).  On a mixture-of-experts model "int4" stores
         wq, wk, wv and wo only, and needs quantised experts (`expert_weights` "int4" or "fp8").  `lora_slots` (with `args.lora`, dense
         models): every un-merged adapter is a bank of that many slots, loaded with `load_lora(slot=...)`, and each sequence of a batch
-        runs through the slot its `lora_ids` entry names (`generate`, `forward`, ...); at most MAX_LORA_SLOTS."""
+        runs through the slot its `lora_ids` entry names (`generate`, `forward`, ...); at most MAX_LORA_SLOTS.  `prefill_compute`
+        (with dense_weights="fp8"): "bf16", or "fp8" to quantise the input of every layer Linear call of at least 128 tokens that does
+        not take stream-K per token to e4m3 with a power-of-two scale and multiply it by the e4m3 weights on the FP8 tensor cores
+        (include/mistral_b200.h); smaller calls, and so every decode step and chunks of at most 128 tokens, are unchanged.  The
+        weights and the state dict are those of dense_weights="fp8"."""
         if not isinstance(lora_slots, int) or not 1 <= lora_slots <= MAX_LORA_SLOTS:
             raise ValueError(f"lora_slots={lora_slots!r}: expected an int in [1, {MAX_LORA_SLOTS}] (every decode step reads every slot)")
         if lora_slots > 1 and args.lora is None:
@@ -130,7 +153,9 @@ class Transformer(nn.Module):
         super().__init__()
         self.lora_slots = lora_slots
         _check_dense_weights(args, dense_weights, expert_weights)
+        _check_prefill_compute(args, prefill_compute, dense_weights)
         self.dense_weights = dense_weights
+        self.prefill_compute = prefill_compute
         if kv_cache not in KV_CACHE_FORMATS:
             raise ValueError(f"kv_cache={kv_cache!r}: expected one of {KV_CACHE_FORMATS}")
         if kv_cache == "fp8" and args.head_dim != 128:
@@ -194,7 +219,7 @@ class Transformer(nn.Module):
             str(i): TransformerBlock(dim=args.dim, hidden_dim=args.hidden_dim, n_heads=args.n_heads, n_kv_heads=args.n_kv_heads,
                                      head_dim=args.head_dim, norm_eps=args.norm_eps, lora=args.lora, moe=args.moe,
                                      expert_shard=self.expert_parallel, expert_group=expert_group, expert_weights=expert_weights,
-                                     dense_weights=dense_weights, lora_slots=lora_slots)
+                                     dense_weights=dense_weights, lora_slots=lora_slots, prefill_compute=prefill_compute)
             for i in range(offset, end)
         })
         self.n_local_layers = len(self.layers)
@@ -1091,13 +1116,13 @@ class Transformer(nn.Module):
                     device: Union[torch.device, str] = "cuda", dtype: Optional[torch.dtype] = None,
                     softmax_fp32: bool = True, expert_parallel: Optional[Tuple[int, int]] = None, expert_group: Any = None,
                     expert_weights: str = "bf16", *, kv_cache: str = "bf16", dense_weights: str = "bf16",
-                    lora_slots: int = 1) -> "Transformer":
+                    lora_slots: int = 1, prefill_compute: str = "bf16") -> "Transformer":
         """transformer.py:297-338.  Tensors stream from disk straight into the packed device buffers; with `expert_parallel`
         the experts of other ranks are skipped (never read into device memory).  With expert_weights="fp8" or "int4" each bf16
         expert tensor is copied to the device and quantised into place: the peak is the quantised model plus about one bf16 tensor.
         `kv_cache` ("bf16" | "fp8") is the format of the KV cache that generate() builds (see Transformer).  With
-        dense_weights="fp8" or "int4" every bf16 layer Linear is quantised into place the same way.  `lora_slots`: see Transformer;
-        the checkpoint's adapter, if any, fills slot 0."""
+        dense_weights="fp8" or "int4" every bf16 layer Linear is quantised into place the same way.  `lora_slots` and
+        `prefill_compute`: see Transformer; the checkpoint's adapter, if any, fills slot 0."""
         with open(Path(folder) / "params.json", "r") as f:
             model_args = TransformerArgs.from_dict(json.load(f))
         model_args.max_batch_size = max_batch_size
@@ -1117,7 +1142,8 @@ class Transformer(nn.Module):
             # on meta and assigns, transformer.py:321-331; a fp32 build followed by .to(bf16) would need 3x the model's bytes)
             return Transformer.empty(model_args, dev, dtype or ck_dtype, pipeline_rank=pipeline_rank, num_pipeline_ranks=num_pipeline_ranks,
                                      softmax_fp32=softmax_fp32, expert_parallel=expert_parallel, expert_group=expert_group,
-                                     expert_weights=expert_weights, kv_cache=kv_cache, dense_weights=dense_weights, lora_slots=lora_slots)
+                                     expert_weights=expert_weights, kv_cache=kv_cache, dense_weights=dense_weights, lora_slots=lora_slots,
+                                     prefill_compute=prefill_compute)
 
         if pt_model_file.exists():
             loaded = torch.load(str(pt_model_file), mmap=True)

@@ -7,7 +7,8 @@ include/mistral_b200.h); weights are stored pre-packed for the fused kernels:
 `wq/wk/wv/w1/w3` are exposed as zero-copy views for state-dict compatibility.
 With `lora` set (un-merged adapters) each fused call also owns a packed LoraAdapter and runs the `_lora` entry points.
 With `fp8` (FP8 dense weights, include/mistral_b200.h) the packed matrices hold e4m3 bytes (uint8, same packing) next to one fp32
-scale per row, and every call runs the `_fp8` entry points.
+scale per row, and every call runs the `_fp8` entry points; with `a8` as well (prefill_compute="fp8") the `_fp8a8` ones, whose
+prefill-sized calls quantise the activations per token to e4m3 and run the FP8 tensor cores.
 With `int4` (INT4 dense weights, include/mistral_b200.h) they hold packed 4-bit codes (uint8 [N, K/2], same row packing) next to one
 bf16 scale per group of 128 k of a row, and every call runs the `_int4` entry points.
 """
@@ -138,7 +139,7 @@ class Attention(nn.Module, _Fp8Rows, _Int4Rows):
     """transformer_layers.py:31-93."""
 
     def __init__(self, dim: int, n_heads: int, head_dim: int, n_kv_heads: int, lora: Optional[LoraArgs] = None, fp8: bool = False,
-                 int4: bool = False, lora_slots: int = 1):
+                 int4: bool = False, lora_slots: int = 1, a8: bool = False):
         super().__init__()
         self.dim = dim
         self.n_heads = n_heads
@@ -150,7 +151,8 @@ class Attention(nn.Module, _Fp8Rows, _Int4Rows):
         self.kv_dim = n_kv_heads * head_dim
         self.fp8 = fp8
         self.int4 = int4
-        assert not (fp8 and int4)
+        self.a8 = a8
+        assert not (fp8 and int4) and (fp8 or not a8)
         if fp8:
             self.wqkv = self._fp8_params("wqkv", self.q_dim + 2 * self.kv_dim, dim)
             self.wo_weight = self._fp8_params("wo", dim, self.q_dim)
@@ -260,7 +262,8 @@ class Attention(nn.Module, _Fp8Rows, _Int4Rows):
     def _qkv(self, x, norm_w, rope, positions, q, k, v, cache_k, cache_v, cache_rows, eps, ws, lora_rows=None) -> None:
         H, KV, hd = self.n_heads, self.n_kv_heads, self.head_dim
         if self.fp8:
-            _abi.attn_qkv_fp8(x, norm_w, self.wqkv, self.wqkv_scale, rope, positions, q, k, v, cache_k, cache_v, cache_rows, H, KV, hd, eps, ws)
+            _abi.attn_qkv_fp8(x, norm_w, self.wqkv, self.wqkv_scale, rope, positions, q, k, v, cache_k, cache_v, cache_rows, H, KV, hd, eps, ws,
+                              a8=self.a8)
         elif self.int4:
             _abi.attn_qkv_int4(x, norm_w, self.wqkv, self.wqkv_gscale, rope, positions, q, k, v, cache_k, cache_v, cache_rows, H, KV, hd, eps,
                                ws)
@@ -274,7 +277,7 @@ class Attention(nn.Module, _Fp8Rows, _Int4Rows):
                     lora_rows: Optional[torch.Tensor] = None) -> None:
         """out = residual + wo(a)."""
         if self.fp8:
-            _abi.linear_residual_fp8(a, self.wo_weight, self.wo_scale, residual, out, ws)
+            _abi.linear_residual_fp8(a, self.wo_weight, self.wo_scale, residual, out, ws, a8=self.a8)
         elif self.int4:
             _abi.linear_residual_int4(a, self.wo_weight, self.wo_gscale, residual, out, ws)
         elif self.lora is None:
@@ -295,13 +298,14 @@ class FeedForward(nn.Module, _Fp8Rows, _Int4Rows):
     """transformer_layers.py:96-106."""
 
     def __init__(self, dim: int, hidden_dim: int, lora: Optional[LoraArgs] = None, fp8: bool = False, int4: bool = False,
-                 lora_slots: int = 1):
+                 lora_slots: int = 1, a8: bool = False):
         super().__init__()
         self.dim = dim
         self.hidden_dim = hidden_dim
         self.fp8 = fp8
         self.int4 = int4
-        assert not (fp8 and int4)
+        self.a8 = a8
+        assert not (fp8 and int4) and (fp8 or not a8)
         if fp8:
             self.w13 = self._fp8_params("w13", 2 * hidden_dim, dim)
             self.w2_weight = self._fp8_params("w2", dim, hidden_dim)
@@ -362,8 +366,8 @@ class FeedForward(nn.Module, _Fp8Rows, _Int4Rows):
         g = torch.empty(T, self.hidden_dim, dtype=x.dtype, device=x.device)
         out = torch.empty(T, self.dim, dtype=x.dtype, device=x.device)
         if self.fp8:
-            _abi.ffn_gateup_fp8(x, norm_w, self.w13, self.w13_scale, g, eps, ws)
-            _abi.linear_residual_fp8(g, self.w2_weight, self.w2_scale, residual, out, ws)
+            _abi.ffn_gateup_fp8(x, norm_w, self.w13, self.w13_scale, g, eps, ws, a8=self.a8)
+            _abi.linear_residual_fp8(g, self.w2_weight, self.w2_scale, residual, out, ws, a8=self.a8)
         elif self.int4:
             _abi.ffn_gateup_int4(x, norm_w, self.w13, self.w13_gscale, g, eps, ws)
             _abi.linear_residual_int4(g, self.w2_weight, self.w2_gscale, residual, out, ws)
@@ -398,7 +402,7 @@ class TransformerBlock(nn.Module):
 
     def __init__(self, dim: int, hidden_dim: int, n_heads: int, n_kv_heads: int, head_dim: int, norm_eps: float,
                  lora: Optional[LoraArgs] = None, moe: Optional[MoeArgs] = None, expert_shard: Tuple[int, int] = (0, 1), expert_group=None,
-                 expert_weights: str = "bf16", dense_weights: str = "bf16", lora_slots: int = 1):
+                 expert_weights: str = "bf16", dense_weights: str = "bf16", lora_slots: int = 1, prefill_compute: str = "bf16"):
         super().__init__()
         assert lora_slots == 1 or (lora is not None and moe is None), "a bank of adapter slots: dense layers with un-merged LoRA only"
         if lora is not None and moe is not None:
@@ -409,9 +413,11 @@ class TransformerBlock(nn.Module):
         fp8, int4 = dense_weights == "fp8", dense_weights == "int4"
         assert not (fp8 or int4) or lora is None, "quantised dense weights: layers without un-merged LoRA only"
         assert not fp8 or moe is None, "FP8 dense weights: dense layers only"
+        a8 = prefill_compute == "fp8"
+        assert not a8 or fp8, "FP8 activations: FP8 dense weights only"
         # on a MoE block INT4 dense weights are the attention Linears only; the experts follow expert_weights
         self.attention = Attention(dim=dim, n_heads=n_heads, head_dim=head_dim, n_kv_heads=n_kv_heads, lora=lora, fp8=fp8, int4=int4,
-                                   lora_slots=lora_slots)
+                                   lora_slots=lora_slots, a8=a8)
         self.attention_norm = RMSNorm(dim, eps=norm_eps)
         self.ffn_norm = RMSNorm(dim, eps=norm_eps)
         self.feed_forward: nn.Module
@@ -423,7 +429,7 @@ class TransformerBlock(nn.Module):
                                          gate_weight=nn.Parameter(torch.empty(moe.num_experts, dim), requires_grad=False), moe_args=moe,
                                          expert_shard=expert_shard, expert_group=expert_group)
         else:
-            self.feed_forward = FeedForward(dim=dim, hidden_dim=hidden_dim, lora=lora, fp8=fp8, int4=int4, lora_slots=lora_slots)
+            self.feed_forward = FeedForward(dim=dim, hidden_dim=hidden_dim, lora=lora, fp8=fp8, int4=int4, lora_slots=lora_slots, a8=a8)
 
     def forward(self, x: torch.Tensor, rope: torch.Tensor, positions: torch.Tensor, cache: Optional[CacheView],
                 ws: "_abi.Workspace", lora_rows: Optional[torch.Tensor] = None) -> torch.Tensor:
