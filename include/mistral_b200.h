@@ -30,7 +30,7 @@
 extern "C" {
 #endif
 
-#define MB200_ABI_VERSION 4
+#define MB200_ABI_VERSION 5
 
 #define MB200_OK 0
 #define MB200_E_INVALID (-1)   /* bad argument / unsupported shape */
@@ -271,6 +271,28 @@ int mb200_argmax_rows(const float* logits, int64_t* out_dev, int64_t T, int64_t 
 int mb200_logprob_gather(const float* logits, const int64_t* target_dev, float* out_dev, int64_t T, int64_t vocab, void* stream);
 int mb200_sample_top_p(const float* logits, const float* uniform_dev, int64_t* out_dev, int64_t T, int64_t vocab,
                        float temperature, float top_p, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * mb200_select_tokens: one token per row b < B of logits [B, vocab] fp32 with per-row sampling controls (generate()'s
+ * temperature / top_p / random_seed / presence_penalty / frequency_penalty).  One CTA per row; nothing of size [B, vocab] is written.
+ *   temperature_dev, top_p_dev, presence_dev, frequency_dev [B] fp32: the row's controls.  The caller keeps them in range
+ *                  (temperature >= 0 and finite, top_p in [0, 1], penalties finite); the kernel does not check device values.
+ *   counts_dev     [B, vocab] int32 or NULL: c[b, v], how often row b's sequence selected v so far.
+ *   step_dev       [B] int32: t, the row's step.
+ *   seeds_dev [B] uint64 or uniform_dev [B] fp32 in [0, 1): exactly one is non-NULL.
+ * Per row b:
+ *   1. l'[v] = fp32(l[v] - pen[v]), pen[v] = fp32(fp32(c[v]) * frequency) then + presence (one fp32 add) where c[v] > 0, all
+ *      round-to-nearest without FMA.  With counts_dev NULL, or both penalties of the row 0, l' is l bit for bit.
+ *   2. temperature == 0: argmax of l' as mb200_argmax_rows (-0 == +0, NaN above +inf, the first index on ties).
+ *   3. otherwise the draw of mb200_sample_top_p on l' at (temperature, top_p) with the uniform u:
+ *      seeded: u = (x0 >> 8) * 2^-24 with x0 word 0 of Philox4x32-10, key (seed mod 2^32, seed >> 32), counter (t, 0, 0, 0);
+ *      else u = uniform_dev[b].
+ *   4. out_dev[b] (int64) = the token; then counts_dev[b, token] += 1 (when given) and step_dev[b] += 1, on the device.
+ * No argument changes from step to step, so a stream capture of the call replays as a decode loop's selection.
+ */
+int mb200_select_tokens(const float* logits, const float* temperature_dev, const float* top_p_dev, const float* presence_dev,
+                        const float* frequency_dev, const uint64_t* seeds_dev, const float* uniform_dev, int32_t* step_dev,
+                        int32_t* counts_dev, int64_t* out_dev, int64_t B, int64_t vocab, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Speculative decoding: a draft model proposes k tokens per sequence, the target scores the S = k + 1 tokens

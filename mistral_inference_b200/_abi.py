@@ -15,7 +15,7 @@ import torch
 _LIB_PATH = Path(os.environ.get("MB200_LIB_PATH") or Path(__file__).resolve().parent / "libmb200.so")  # override: A/B builds of experiments
 _lib: Optional[ctypes.CDLL] = None
 
-ABI_VERSION = 4
+ABI_VERSION = 5
 SKINNY_MAX_T = 4
 WORKSPACE_HEADER_BYTES = 64 * 1024
 
@@ -56,6 +56,7 @@ _SIGNATURES = {
     "mb200_argmax_rows": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_void_p]),
     "mb200_logprob_gather": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_void_p]),
     "mb200_sample_top_p": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_float, c_float, c_void_p]),
+    "mb200_select_tokens": (c_int, [c_void_p] * 10 + [c_int64, c_int64, c_void_p]),
     "mb200_spec_meta": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_void_p, c_int64, c_void_p]),
     "mb200_spec_accept_greedy": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_void_p]),
     "mb200_spec_accept_sample": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64,
@@ -484,6 +485,24 @@ def sample_top_p(logits: torch.Tensor, uniform: torch.Tensor, temperature: float
     assert logits.dtype == torch.float32 and uniform.dtype == torch.float32 and uniform.shape == (T,)
     out = torch.empty(T, dtype=torch.long, device=logits.device) if out is None else out
     _check(lib().mb200_sample_top_p(_ptr(logits), _ptr(uniform), _ptr(out), T, V, temperature, top_p, _stream()), "mb200_sample_top_p")
+    return out
+
+
+def select_tokens(logits: torch.Tensor, temperature: torch.Tensor, top_p: torch.Tensor, presence: torch.Tensor, frequency: torch.Tensor,
+                  step: torch.Tensor, out: torch.Tensor, *, seeds: Optional[torch.Tensor] = None, uniform: Optional[torch.Tensor] = None,
+                  counts: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """One token per row with per-row controls (mb200_select_tokens): the four controls [B] fp32, `step` [B] int32 and `counts`
+    [B, V] int32 (or None) are advanced in place; `seeds` [B] int64 holding the uint64 bit patterns, or `uniform` [B] fp32."""
+    T, V = logits.shape
+    assert logits.dtype == torch.float32 and (seeds is None) != (uniform is None)
+    for t in (temperature, top_p, presence, frequency):
+        assert t.dtype == torch.float32 and t.shape == (T,)
+    assert step.dtype == torch.int32 and step.shape == (T,) and out.dtype == torch.long and out.shape == (T,)
+    assert seeds is None or (seeds.dtype in (torch.int64, torch.uint64) and seeds.shape == (T,))
+    assert uniform is None or (uniform.dtype == torch.float32 and uniform.shape == (T,))
+    assert counts is None or (counts.dtype == torch.int32 and counts.shape == (T, V))
+    _check(lib().mb200_select_tokens(_ptr(logits), _ptr(temperature), _ptr(top_p), _ptr(presence), _ptr(frequency), _ptr(seeds), _ptr(uniform),
+                                     _ptr(step), _ptr(counts), _ptr(out), T, V, _stream()), "mb200_select_tokens")
     return out
 
 

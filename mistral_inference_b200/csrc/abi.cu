@@ -879,6 +879,22 @@ int mb200_sample_top_p(const float* logits, const float* uniform_dev, int64_t* o
   return MB200_OK;
 }
 
+int mb200_select_tokens(const float* logits, const float* temperature_dev, const float* top_p_dev, const float* presence_dev,
+                        const float* frequency_dev, const uint64_t* seeds_dev, const float* uniform_dev, int32_t* step_dev, int32_t* counts_dev,
+                        int64_t* out_dev, int64_t B, int64_t vocab, void* stream) {
+  MB_CHECK_ARG(logits && temperature_dev && top_p_dev && presence_dev && frequency_dev && step_dev && out_dev && B >= 0 && vocab >= 1 &&
+                   vocab <= INT32_MAX,
+               "select_tokens: bad arguments");
+  MB_CHECK_ARG((seeds_dev == nullptr) != (uniform_dev == nullptr), "select_tokens: exactly one of seeds and uniform");
+  if (B == 0) return MB200_OK;
+  select_tokens_kernel<<<(unsigned)B, SP_THREADS, 0, (cudaStream_t)stream>>>(logits, temperature_dev, top_p_dev, presence_dev, frequency_dev,
+                                                                            (const unsigned long long*)seeds_dev, uniform_dev, step_dev,
+                                                                            counts_dev, (long long*)out_dev, (int)vocab);
+  MB_CHECK_LAUNCH("select_tokens_kernel");
+  note_launch("select_tokens_kernel<%s, %s>", seeds_dev ? "philox" : "uniform", counts_dev ? "counts" : "nocounts");
+  return MB200_OK;
+}
+
 // ---- mixture of experts (csrc/moe.cuh) ---------------------------------------------------------------------------------------
 int mb200_moe_sizes(int64_t T, int64_t n_experts, int64_t top_k, int64_t* tile_rows, int64_t* rows_cap, int64_t* plan_words) {
   MB_CHECK_ARG(T >= 1 && n_experts >= 1 && top_k >= 1, "moe_sizes: bad arguments");

@@ -3,7 +3,10 @@
 //   argmax_rows_kernel      greedy pick: torch.argmax(logits, -1) (generate.py:156), first index on ties
 //   logprob_gather_kernel   log_softmax(logits, -1)[t, target[t]] (generate.py:101-117,134-135) without materialising [T, V]
 //   sample_top_p_kernel     softmax(logits / temperature) -> nucleus (top-p) filter -> one draw (generate.py:151-170)
-// The row argmax, the nucleus and the draw are device functions that the speculative acceptance kernels share.
+//   select_tokens_kernel    per-row sampling controls: presence / frequency penalties applied on load, then greedy or nucleus
+//                           with the row's own temperature, top_p and (seeded Philox or caller) uniform
+// The row argmax, the nucleus and the draw are device functions that the speculative acceptance kernels share.  They read a row
+// through a loader (RawRow: the logits as they are; PenalisedRow: the penalised logits), so no penalised copy is ever written.
 //
 // All three are one CTA per row over fp32 logits [T, V] (the lm head's output).  Roofline: HBM/L2 -- V * 4 bytes per row and
 // pass; argmax and logprob are single-pass (online log-sum-exp), top-p re-reads its row (L2 resident) during the threshold
@@ -36,11 +39,18 @@ __device__ __forceinline__ float block_max(float v, float* scratch) {
   return t;
 }
 
+// A row of fp32 logits as the selection reads it: row(i) is element i.
+struct RawRow {
+  const float* p;
+  __device__ __forceinline__ float operator()(int i) const { return p[i]; }
+};
+
 // argmax of one row with the first index on ties; the result is valid in thread 0 (the shared partials may be reused once
 // every thread has passed a __syncthreads after the call)
-__device__ __forceinline__ int block_argmax(const float* __restrict__ row, int V) {
+template <typename Row>
+__device__ __forceinline__ int block_argmax(const Row& row, int V) {
   unsigned long long best = 0ull;
-  for (int i = threadIdx.x; i < V; i += SP_THREADS) best = max(best, argmax_key(row[i], i));
+  for (int i = threadIdx.x; i < V; i += SP_THREADS) best = max(best, argmax_key(row(i), i));
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) best = max(best, __shfl_xor_sync(0xffffffffu, best, o));
   __shared__ unsigned long long sm[SP_WARPS];
@@ -53,6 +63,7 @@ __device__ __forceinline__ int block_argmax(const float* __restrict__ row, int V
   }
   return 0x7fffffff - (int)(best & 0xffffffffull);
 }
+__device__ __forceinline__ int block_argmax(const float* __restrict__ row, int V) { return block_argmax(RawRow{row}, V); }
 
 __global__ void __launch_bounds__(SP_THREADS) argmax_rows_kernel(const float* __restrict__ logits, long long* __restrict__ out, int V) {
   const int best = block_argmax(logits + (int64_t)blockIdx.x * V, V);
@@ -90,23 +101,30 @@ __global__ void __launch_bounds__(SP_THREADS) logprob_gather_kernel(const float*
 //   NucleusRow   softmax(row / temperature): the row maximum m and 1/Z, prob(i) = exp(row[i] / T - m) / Z
 //   nucleus_tau  the threshold tau of the kept set {i : prob(i) >= tau}
 //   block_draw   inverse-CDF draw over nonnegative weights w(i) in index order
-struct NucleusRow {
-  const float* row;
+template <typename Row>
+struct NucleusRowOf {
+  Row row;
   float inv_temperature, m, inv_z;
-  __device__ __forceinline__ float prob(int i) const { return expf(row[i] * inv_temperature - m) * inv_z; }
+  __device__ __forceinline__ float prob(int i) const { return expf(row(i) * inv_temperature - m) * inv_z; }
 };
+using NucleusRow = NucleusRowOf<RawRow>;
 
-__device__ __forceinline__ NucleusRow nucleus_row(const float* __restrict__ row, int V, float inv_temperature, float* scratch) {
+template <typename Row>
+__device__ __forceinline__ NucleusRowOf<Row> nucleus_row(const Row& row, int V, float inv_temperature, float* scratch) {
   float m = -INFINITY;
-  for (int i = threadIdx.x; i < V; i += SP_THREADS) m = fmaxf(m, row[i] * inv_temperature);
+  for (int i = threadIdx.x; i < V; i += SP_THREADS) m = fmaxf(m, row(i) * inv_temperature);
   m = block_max(m, scratch);
   float z = 0.f;
-  for (int i = threadIdx.x; i < V; i += SP_THREADS) z += expf(row[i] * inv_temperature - m);
+  for (int i = threadIdx.x; i < V; i += SP_THREADS) z += expf(row(i) * inv_temperature - m);
   z = block_sum(z, scratch);
-  return NucleusRow{row, inv_temperature, m, 1.0f / z};
+  return NucleusRowOf<Row>{row, inv_temperature, m, 1.0f / z};
+}
+__device__ __forceinline__ NucleusRow nucleus_row(const float* __restrict__ row, int V, float inv_temperature, float* scratch) {
+  return nucleus_row(RawRow{row}, V, inv_temperature, scratch);
 }
 
-__device__ __forceinline__ float nucleus_tau(const NucleusRow& r, int V, float top_p, float* scratch) {
+template <typename Row>
+__device__ __forceinline__ float nucleus_tau(const NucleusRowOf<Row>& r, int V, float top_p, float* scratch) {
   // bisection on the bit pattern of tau in (0, 1]: invariant S(hi) <= top_p (S(1.0) = 0), S(lo) > top_p or lo = 0
   unsigned lo = 0u, hi = __float_as_uint(1.0f);
   while (hi - lo > 1u) {
@@ -208,6 +226,78 @@ __global__ void __launch_bounds__(SP_THREADS) sample_top_p_kernel(const float* _
   const float tau = nucleus_tau(r, V, top_p, scratch);
   const int winner = block_draw([&](int i) { const float p = r.prob(i); return p >= tau ? p : 0.f; }, V, uniform[blockIdx.x]);
   if (threadIdx.x == 0) out[blockIdx.x] = winner;
+}
+
+// ---- per-row sampling controls (generate(temperature=[...], top_p=..., random_seed=..., presence_penalty=..., ...)) -------------
+// Penalised logits as the selection loads them: l'[v] = fp32(l[v] - pen[v]) with pen[v] = fp32(c[v] * frequency), plus presence
+// (one fp32 add) where c[v] > 0; c[v] counts the times the sequence generated v.  Round-to-nearest, no FMA contraction.  A NULL
+// count row (no count table, or both penalties of the row 0) reads the logits unchanged.
+struct PenalisedRow {
+  const float* p;
+  const int* count;
+  float presence, frequency;
+  __device__ __forceinline__ float operator()(int i) const {
+    const float x = p[i];
+    if (count == nullptr) return x;
+    const int c = count[i];
+    float pen = __fmul_rn((float)c, frequency);
+    if (c > 0) pen = __fadd_rn(pen, presence);
+    return __fsub_rn(x, pen);
+  }
+};
+
+// Philox4x32-10 (Salmon et al., SC'11), the Random123 constants.
+__device__ __forceinline__ uint4 philox4x32_10(uint4 ctr, uint2 key) {
+#pragma unroll
+  for (int r = 0; r < 10; ++r) {
+    if (r) {
+      key.x += 0x9E3779B9u;
+      key.y += 0xBB67AE85u;
+    }
+    const unsigned lo0 = 0xD2511F53u * ctr.x, hi0 = __umulhi(0xD2511F53u, ctr.x);
+    const unsigned lo1 = 0xCD9E8D57u * ctr.z, hi1 = __umulhi(0xCD9E8D57u, ctr.z);
+    ctr = make_uint4(hi1 ^ ctr.y ^ key.x, lo1, hi0 ^ ctr.w ^ key.y, lo0);
+  }
+  return ctr;
+}
+
+// The uniform of a seeded sequence at its step t: the top 24 bits of word 0 of Philox4x32-10 with key (seed mod 2^32, seed >> 32)
+// and counter (t, 0, 0, 0), times 2^-24 -- exactly representable, in [0, 1).
+__device__ __forceinline__ float philox_uniform(unsigned long long seed, unsigned step) {
+  const uint4 x = philox4x32_10(make_uint4(step, 0u, 0u, 0u), make_uint2((unsigned)seed, (unsigned)(seed >> 32)));
+  return (float)(x.x >> 8) * 0x1p-24f;
+}
+
+// One CTA per row b: temperature[b] == 0 is greedy (block_argmax), otherwise the nucleus draw of sample_top_p_kernel at
+// (temperature[b], top_p[b]) with u = philox_uniform(seeds[b], step[b]) when seeds is given, else uniform[b].  Then thread 0 adds 1
+// to counts[b, token] (when a table is given) and to step[b]: the barrier before it orders every thread's reads of the row's counts
+// and step before the increment.  Nothing the host changes between steps is an argument, so a captured launch replays as is.
+__global__ void __launch_bounds__(SP_THREADS) select_tokens_kernel(const float* __restrict__ logits, const float* __restrict__ temperature,
+                                                                   const float* __restrict__ top_p, const float* __restrict__ presence,
+                                                                   const float* __restrict__ frequency, const unsigned long long* __restrict__ seeds,
+                                                                   const float* __restrict__ uniform, int* step, int* counts,
+                                                                   long long* __restrict__ out, int V) {
+  const int b = blockIdx.x;
+  const float pres = presence[b], freq = frequency[b];
+  int* cnt = counts != nullptr ? counts + (int64_t)b * V : nullptr;
+  const PenalisedRow row{logits + (int64_t)b * V, (cnt != nullptr && (pres != 0.f || freq != 0.f)) ? cnt : nullptr, pres, freq};
+  const float t = temperature[b];
+  int token;
+  if (t == 0.f) {
+    token = block_argmax(row, V);  // valid in thread 0, the only reader
+  } else {
+    __shared__ float scratch[SP_WARPS];
+    const auto r = nucleus_row(row, V, __fdiv_rn(1.0f, t), scratch);
+    const float tau = nucleus_tau(r, V, top_p[b], scratch);
+    const float u = seeds != nullptr ? philox_uniform(seeds[b], (unsigned)step[b]) : uniform[b];
+    token = block_draw([&](int i) { const float p = r.prob(i); return p >= tau ? p : 0.f; }, V, u);
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    out[b] = token;
+    if (cnt != nullptr && token >= 0) cnt[token] += 1;
+    step[b] += 1;
+  }
 }
 
 }  // namespace mb200

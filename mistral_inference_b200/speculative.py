@@ -58,6 +58,15 @@ def check_draft(model: Transformer, draft: Transformer, images, prompts: List[Li
                              "so such a cache cannot roll back (generate without a draft, or keep the generation inside the window)")
 
 
+def check_draft_controls(controls, top_p) -> None:
+    """Per-sequence sampling controls are not built for speculative decoding: the acceptance kernels take one temperature and
+    top_p for the batch, and penalties would need the counts rolled back when proposals are rejected.  `controls` is
+    generate.sampling_controls' result (None: every control a scalar, no seed, no penalty)."""
+    if controls is not None or top_p != TOP_P:
+        raise ValueError(f"speculative decoding (draft=...) takes one scalar temperature and top_p={TOP_P}: per-sequence "
+                         "temperatures, another top_p, random_seed and presence / frequency penalties with a draft model are not built")
+
+
 def _prefill(m: Transformer, plan: _PromptPlan, cache: BufferCache, want_logprobs: bool):
     """The prompt, chunk by chunk: (prompt log-probabilities per chunk, logits [B, V] of each sequence's last token)."""
     dev = m.device
